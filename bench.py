@@ -40,21 +40,24 @@ sys.path.insert(0, ROOT)
 Q = 3329
 WORKLOADS = {
     "mlkem768": dict(k=3, name="ML-KEM-768", ek=1184, ct=1088, bytes_per_op=2336,
-                     desc="ML-KEM-768 full encaps (keccakf1600 GenA + NTT matvec) 2^20 batch on 1 B200, per-op ek"),
+                     desc="ML-KEM-768 full encaps (keccakf1600 GenA + NTT matvec) 2^20 batch on 1 H100, per-op ek"),
     "mlkem1024": dict(k=4, name="ML-KEM-1024", ek=1568, ct=1568, bytes_per_op=3200,
-                      desc="ML-KEM-1024 encaps 2^24 batch sharded across 8 B200 (2^21 per GPU), per-op ek, per-GPU + aggregate"),
+                      desc="ML-KEM-1024 encaps 2^24 batch sharded across 8 H100 (2^21 per GPU), per-op ek, per-GPU + aggregate"),
 }
 MLDSA = dict(name="ML-DSA-65", sk=4032, sig=3309, bytes_per_op=7373,
-             desc="ML-DSA-65 Sign 2^18 batch (q=8380417 NTT + rejection loop) on 1 B200, per-op sk, 32-byte messages")
-NTT_DESC = "2^20-batch Kyber 256-pt NTT on 1 B200, bit-exact vs common.nttGeneric"
+             desc="ML-DSA-65 Sign 2^18 batch (q=8380417 NTT + rejection loop) on 1 H100, per-op sk, 32-byte messages")
+NTT_DESC = "2^20-batch Kyber 256-pt NTT on 1 H100, bit-exact vs common.nttGeneric"
 KEY_POOL = ("1024 keys DeriveKeyPair(SHAKE256(0x00||LE32(j))), op i uses key i mod 1024; "
             "m_i = SHAKE256(0x01||LE64(i))")
-SM_HZ = 1.965e9
-# Keccak-f[1600] on the integer-ALU pipe: 24 rounds x (122 LOP3 + 58 SHF) per state and thread; the pipe issues one
-# warp instruction every second clock per SM sub-partition (measured: scripts/ubench_r02.cu reaches 0.496,
-# profiles/r02_ubench_keccak.txt), 148 SMs x 4 sub-partitions
+SM_HZ = 1.98e9  # H100 SXM maximum SM clock
+# Keccak-f[1600] on the integer-ALU pipe: 24 rounds x (122 LOP3 + 58 SHF) per state and thread; on sm_90 the pipe
+# issues one warp instruction every second clock per SM sub-partition (64 32-bit logic / shift results per clock and
+# SM), 4 sub-partitions per SM
 KECCAK_INSTR = 24 * 180
-KECCAK_PEAK = 148 * 4 * 0.5 * 32 * SM_HZ / KECCAK_INSTR
+
+
+def keccak_peak(sm_count: int) -> float:
+    return sm_count * 4 * 0.5 * 32 * SM_HZ / KECCAK_INSTR
 
 
 def env_int(name, default):
@@ -76,16 +79,6 @@ def host_threads() -> int:
     return n
 
 
-def ncu_traffic(kernel: str, units_per_launch: float):
-    """DRAM bytes per launch of `kernel` from the committed ncu capture (profiles/ncu_traffic.json), scaled
-    to the units this run's launches process; None if no capture exists for that kernel."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))[kernel]
-        return t["bytes_per_launch"] * units_per_launch / t["units_per_launch"]
-    except Exception:
-        return None
-
-
 def measured_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -93,13 +86,29 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "datasheet"  # H100 SXM HBM3
+
+
+DUMP_ROWS = 4096  # at most 4096 x 3310 float32 = 54 MB per dump (ML-DSA-65 signatures + status)
+
+
+def dump_outputs(dirname: str, arrays: dict, n: int) -> None:
+    """--dump-outputs: `arrays` (device tensors, one row per operation) as DIR/<name>.npy in float32, restricted to a
+    fixed, seeded sample of DUMP_ROWS operations (sorted; their indices in DIR/rows.npy) when the batch is larger."""
+    import numpy as np
+    import torch
+    os.makedirs(dirname, exist_ok=True)
+    rows = np.arange(n) if n <= DUMP_ROWS else np.sort(np.random.default_rng(0).choice(n, DUMP_ROWS, replace=False))
+    np.save(os.path.join(dirname, "rows.npy"), rows.astype(np.float64))
+    for name, t in arrays.items():
+        sel = t[torch.as_tensor(rows, device=t.device)]
+        np.save(os.path.join(dirname, name + ".npy"), sel.cpu().numpy().astype(np.float32))
 
 
 def mlkem_config(wl, n):
     """The `config` object of an ML-KEM line; identical in our arm and in the reference arm."""
     return {"workload": wl["desc"], "batch_per_gpu": n, "ek": "per-op (stride %d)" % wl["ek"], "key_pool": KEY_POOL,
-            "l2": "inputs+outputs %.1f GiB per step, larger than the 126 MB L2" % (n * wl["bytes_per_op"] / 2**30),
+            "l2": "inputs+outputs %.1f GiB per step, larger than the 50 MB L2" % (n * wl["bytes_per_op"] / 2**30),
             "sharding": "contiguous index ranges per rank; no collective during compute, results gathered to rank 0"}
 
 
@@ -181,7 +190,7 @@ def synth_polys(first_poly: int, n: int, device="cpu"):
 class ClockSampler:
     """SM clock and throttle reasons DURING the timed region.  The region is short (5 steps of ~18 ms), so the samples
     come from NVML in a thread (one query ~ 0.1 ms, every 2 ms) -- the same counters `nvidia-smi --query-gpu=clocks.sm,
-    clocks.max.sm,clocks_event_reasons.*` prints (B200_PROFILING.md), which is the fallback when pynvml is missing:
+    clocks.max.sm,clocks_event_reasons.*` prints, which is the fallback when pynvml is missing:
     nvidia-smi itself needs longer to start than the region lasts."""
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -415,6 +424,7 @@ class Ctx:
             dist.init_process_group("nccl", device_id=torch.device("cuda", self.local))
         circl_b200.init(self.local)
         self.peak, self.peak_kind = measured_peak()
+        self.keccak_peak = keccak_peak(torch.cuda.get_device_properties(self.local).multi_processor_count)
         self.torch = torch
 
     def barrier(self):
@@ -446,7 +456,7 @@ class Ctx:
 
 # ---------------------------------------------------------------- ML-KEM encaps (configs 3 and 5)
 def bench_mlkem(cx: Ctx, wl_key: str, log2n: int, steps: int, warmup: int, with_profile=True, with_cpu=True,
-                e2e_steps=5, sampler=None):
+                e2e_steps=5, sampler=None, dump=None):
     import numpy as np
     torch, L, check = cx.torch, cx.L, cx.check
     from circl_b200 import mlkem
@@ -469,7 +479,7 @@ def bench_mlkem(cx: Ctx, wl_key: str, log2n: int, steps: int, warmup: int, with_
     ss_d = torch.empty((n, 32), dtype=torch.uint8, device="cuda")
 
     # N > 1: results are gathered to rank 0 in global index order (the one exchange of this path).  The flow pushes every
-    # sub-batch of 8192 results into rank 0's buffer as soon as it exists (cb200_mlkem_encaps_push: peer copies by the
+    # sub-batch of 4096 results into rank 0's buffer as soon as it exists (cb200_mlkem_encaps_push: peer copies by the
     # copy engines over NVLink) while the next sub-batches compute.
     from circl_b200.shard import RowGather
     pg = RowGather(n, [wl["ct"], 32], transport="ipc") if world > 1 else None
@@ -482,7 +492,7 @@ def bench_mlkem(cx: Ctx, wl_key: str, log2n: int, steps: int, warmup: int, with_
         check(L.cb200_mlkem_encaps(wl["k"], eks_h.data_ptr(), wl["ek"], seeds_h.data_ptr(), ct_h.data_ptr(),
                                    ss_h.data_ptr(), None, n))
 
-    # ---- device-resident timing (inputs + outputs per step far larger than the 126 MB L2)
+    # ---- device-resident timing (inputs + outputs per step far larger than the 50 MB L2)
     for _ in range(warmup):
         step_device()
     cx.barrier()
@@ -499,6 +509,8 @@ def bench_mlkem(cx: Ctx, wl_key: str, log2n: int, steps: int, warmup: int, with_
     ms_step = cx.max_over_ranks(ev0.elapsed_time(ev1) / steps)
     scheme.check_last_status()
     clocks = sampler.stop() if (sampler is not None and rank == 0) else None
+    if dump and rank == 0:
+        dump_outputs(dump, {"ct": ct_d, "ss": ss_d}, n)
 
     # ---- N > 1: parity of the GATHERED buffer, the same step without the gather, and the gather alone
     gather = None
@@ -530,12 +542,12 @@ def bench_mlkem(cx: Ctx, wl_key: str, log2n: int, steps: int, warmup: int, with_
         cx.barrier()
         ms_gather = cx.max_over_ranks(ev0.elapsed_time(ev1))
         nbytes = (world - 1) * n * (wl["ct"] + 32)
-        gather = {"to": "rank 0", "bytes_per_step": nbytes, "chunks": (n + 8191) // 8192, "ms_alone": ms_gather,
+        gather = {"to": "rank 0", "bytes_per_step": nbytes, "chunks": (n + 4095) // 4096, "ms_alone": ms_gather,
                   "rank0_ingress_GBps": nbytes / 1e9 / (ms_gather * 1e-3),
                   "ms_per_step_without_gather": ms_nogather, "exposed_ms": ms_step - ms_nogather,
                   "gathered_outputs_match": match, "checked_rows": (len(idx) if rank == 0 else None),
                   "transport": "CUDA IPC mapping of rank 0's buffer + cudaMemcpyAsync peer copies on a copy stream "
-                               "(copy engines over NVLink; no SM), issued by the encaps flow itself per sub-batch of 8192 "
+                               "(copy engines over NVLink; no SM), issued by the encaps flow itself per sub-batch of 4096 "
                                "results (cb200_mlkem_encaps_push); torch.distributed/NCCL only for the handle and barriers",
                   "note": "value includes the gather, overlapped sub-batch by sub-batch with the kernels; the strided "
                           "sample of the gathered buffer on rank 0 is compared with the oracle"}
@@ -593,21 +605,21 @@ def bench_mlkem(cx: Ctx, wl_key: str, log2n: int, steps: int, warmup: int, with_
         dom_ms = dom["ms_total"] / dom["launches"]
         achieved = wl["bytes_per_op"] * units_per_launch / (dom_ms * 1e-3) / 1e9
         roofline = {"bound": "hbm", "kernel": dom_name, "achieved": achieved, "peak": cx.peak, "unit": "GB/s",
-                    "frac": achieved / cx.peak, "traffic": ncu_traffic(dom_name, units_per_launch),
+                    "frac": achieved / cx.peak,
                     "peak_kind": cx.peak_kind, "share_of_step": dom["ms_total"] / total_kernel_ms,
                     "note": "path is integer-ALU (Keccak) bound, not HBM bound; achieved = %d algorithmic B/op x %d ops per "
-                            "launch / mean launch time; traffic = ncu dram bytes per launch.  kernels_ms_per_step comes from "
+                            "launch / mean launch time.  kernels_ms_per_step comes from "
                             "a profiling pass that serialises the two internal lanes on one stream, so it sums to more "
                             "than ms_per_step; share_of_step is a share of that sum" % (wl["bytes_per_op"], int(units_per_launch)),
                     "kernels_ms_per_step": {k_: round(v["ms_total"], 4) for k_, v in kernels.items()}}
         # The binding resource is the integer-ALU pipe, so state that roofline too (Keccak-f/s of the kernel against the
-        # measured ceiling of the permutation, see KECCAK_PEAK)
+        # ceiling of the permutation, see keccak_peak)
         k = wl["k"]
         perms = {"mlkem_sample": 3 * k * k + (2 * k + 1), "mlkem_hash_ek": (384 * k + 32) // 136 + 1}.get(dom_name)
         if perms:
             alu_ach = perms * units_per_launch / (dom_ms * 1e-3)
-            roofline["alu"] = {"bound": "int-alu", "achieved": alu_ach, "peak": KECCAK_PEAK, "unit": "keccak-f/s",
-                               "frac": alu_ach / KECCAK_PEAK,
+            roofline["alu"] = {"bound": "int-alu", "achieved": alu_ach, "peak": cx.keccak_peak, "unit": "keccak-f/s",
+                               "frac": alu_ach / cx.keccak_peak,
                                "note": "%d Keccak-f per op in this kernel (3 SHAKE128 blocks per matrix entry + 1 SHAKE256 "
                                        "block per noise polynomial) x 180 ALU-pipe instructions per round; the remainder "
                                        "of the pipe time is rejection parsing and CBD" % perms}
@@ -691,22 +703,21 @@ def bench_ntt(cx: Ctx, steps: int, warmup: int, with_cpu: bool):
         return cx.max_over_ranks(statistics.median(a.elapsed_time(b) for a, b in ts))
 
     for label, fn in (("forward", kyber.ntt_), ("inverse", kyber.inv_ntt_)):
-        ms = timed(fn, pristine, max(steps, 10))
+        ms = timed(fn, pristine, steps)
         gbs = npoly * 1024 / (ms * 1e-3) / 1e9
         ntt[label] = {"value": cx.world * npoly / (ms * 1e-3), "unit": "NTT/s", "ms_per_step": ms,
                       "roofline": {"bound": "hbm", "achieved": gbs, "peak": cx.peak, "unit": "GB/s",
-                                   "frac": gbs / cx.peak, "peak_kind": cx.peak_kind,
-                                   "traffic": ncu_traffic("kyber_ntt" if label == "forward" else "kyber_invntt", npoly)}}
+                                   "frac": gbs / cx.peak, "peak_kind": cx.peak_kind}}
         if any16 is None:
             g = torch.Generator(device="cuda").manual_seed(1 + cx.rank)
             any16 = torch.randint(-32768, 32768, (npoly, 256), device="cuda", dtype=torch.int32, generator=g).to(torch.int16)
-        ms_any = timed(fn, any16, 5)
+        ms_any = timed(fn, any16, steps)
         ntt[label]["any_int16_inputs"] = {"ms_per_step": ms_any, "value": cx.world * npoly / (ms_any * 1e-3),
                                           "frac": npoly * 1024 / (ms_any * 1e-3) / 1e9 / cx.peak}
     del pristine, flush, any16
     ntt["config"] = {"workload": NTT_DESC, "polys_per_gpu": npoly, "bytes_per_ntt": 1024,
                      "inputs": "RandAbsLeQ (|c| <= q) restored before every timed call; any_int16_inputs: uniform int16",
-                     "l2": "input 512 MiB > 126 MB L2, flushed by a 256 MiB write before every timed call; "
+                     "l2": "input 512 MiB > 50 MB L2, flushed by a 256 MiB write before every timed call; "
                            "kernel reads and writes every byte once"}
     host_src = polys_h.clone()
     e2e_s = []
@@ -741,7 +752,7 @@ def bench_keccak(cx: Ctx, steps: int, warmup: int):
     for _ in range(warmup):
         keccak.permute_(st)
     cx.barrier()
-    evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(max(steps, 8))]
+    evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
     for a, b in evs:
         a.record()
         keccak.permute_(st)
@@ -755,14 +766,15 @@ def bench_keccak(cx: Ctx, steps: int, warmup: int):
     return {"metric": "Keccak-f[1600]/sec", "value": cx.world * v, "unit": "keccak-f/s", "ms_per_step": ms,
             "config": {"workload": "cb200_keccak_f1600 on 2^22 states per GPU (200 B each, in place), 24 rounds",
                        "l2": "800 MiB per pass, larger than L2"},
-            "roofline": {"bound": "int-alu", "achieved": v, "peak": KECCAK_PEAK, "unit": "keccak-f/s", "frac": v / KECCAK_PEAK,
-                         "note": "peak = 148 SMs x 4 sub-partitions x 0.5 warp-instr/clk x 32 lanes x 1.965 GHz / (24 x 180 "
-                                 "LOP3+SHF); scripts/ubench_r02.cu measures 4.27e9/s for the bare register loop",
+            "roofline": {"bound": "int-alu", "achieved": v, "peak": cx.keccak_peak, "unit": "keccak-f/s",
+                         "frac": v / cx.keccak_peak,
+                         "note": "peak = SMs x 4 sub-partitions x 0.5 warp-instr/clk x 32 lanes x 1.98 GHz / (24 x 180 "
+                                 "LOP3+SHF)",
                          "hbm": {"achieved": gbs, "peak": cx.peak, "unit": "GB/s", "frac": gbs / cx.peak}}}
 
 
 # ---------------------------------------------------------------- ML-DSA-65 (BASELINE configs[3])
-def bench_mldsa(cx: Ctx, log2n: int, steps: int, warmup: int, with_cpu: bool, sampler=None):
+def bench_mldsa(cx: Ctx, log2n: int, steps: int, warmup: int, with_cpu: bool, sampler=None, dump=None):
     import numpy as np
     torch, L, check = cx.torch, cx.L, cx.check
     rank, world = cx.rank, cx.world
@@ -806,6 +818,8 @@ def bench_mldsa(cx: Ctx, log2n: int, steps: int, warmup: int, with_cpu: bool, sa
     clocks = sampler.stop() if (sampler is not None and rank == 0) else None
     att = attempts.value / n
     assert int(st_d.sum().item()) == 0
+    if dump and rank == 0:
+        dump_outputs(dump, {"sig": sig_d, "status": st_d}, n)
     step_host()
     cx.barrier()
     t0 = time.perf_counter()
@@ -821,11 +835,10 @@ def bench_mldsa(cx: Ctx, log2n: int, steps: int, warmup: int, with_cpu: bool, sa
     # process the whole batch, so its per-step time is the launch duration the roofline refers to
     achieved = MLDSA["bytes_per_op"] * n / (kernels[dom_name]["ms_total"] * 1e-3) / 1e9
     roofline = {"bound": "hbm", "kernel": dom_name, "achieved": achieved, "peak": cx.peak, "unit": "GB/s",
-                "frac": achieved / cx.peak, "traffic": ncu_traffic(dom_name, n * att), "peak_kind": cx.peak_kind,
+                "frac": achieved / cx.peak, "peak_kind": cx.peak_kind,
                 "share_of_step": kernels[dom_name]["ms_total"] / tot,
                 "note": "integer-ALU (Keccak + NTT) bound; achieved = 7373 algorithmic B/op x batch / time of this kernel "
-                        "class summed over the rounds of one step; traffic = ncu dram bytes of the first round scaled to "
-                        "all op-rounds of the step",
+                        "class summed over the rounds of one step",
                 "kernels_ms_per_step": {k_: round(v["ms_total"], 3) for k_, v in kernels.items()}}
     cpu = None
     if with_cpu and rank == 0 and world == 1:
@@ -865,6 +878,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-ntt", action="store_true", help="skip the secondary NTT / Keccak measurements")
     ap.add_argument("--no-extras", action="store_true", help="skip the extra BASELINE configs (mldsa65 at N = 1, mlkem1024 at N > 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write rank 0's outputs of the last step as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -878,10 +893,11 @@ def main():
               "vs_baseline": None, "data": "synthetic"}
     if args.workload == "mldsa65":
         log2 = args.batch_log2 if args.batch_log2 != 20 else 18
-        rec, clocks = bench_mldsa(cx, log2, args.steps, args.warmup, with_cpu, sampler)
+        rec, clocks = bench_mldsa(cx, log2, args.steps, args.warmup, with_cpu, sampler, args.dump_outputs)
         line = dict(rec, **common, clocks=clocks)
     else:
-        rec, clocks = bench_mlkem(cx, args.workload, args.batch_log2, args.steps, args.warmup, True, with_cpu, 5, sampler)
+        rec, clocks = bench_mlkem(cx, args.workload, args.batch_log2, args.steps, args.warmup, True, with_cpu, 5, sampler,
+                                  args.dump_outputs)
         line = dict(rec, **common, dtype="int16", clocks=clocks)
         line.pop("per_gpu", None)
         if not args.no_ntt:
@@ -889,10 +905,10 @@ def main():
             line["keccak"] = bench_keccak(cx, args.steps, args.warmup)
         if not args.no_extras and args.workload == "mlkem768" and args.batch_log2 == 20:
             if cx.world == 1:
-                line["mldsa65"], _ = bench_mldsa(cx, 18, min(args.steps, 5), 3, with_cpu)
+                line["mldsa65"], _ = bench_mldsa(cx, 18, args.steps, 3, with_cpu)
             else:
                 # BASELINE configs[4]: 2^21 per GPU = 2^24 over 8 GPUs, gathered to rank 0 (26.8 GB at N = 8)
-                line["mlkem1024"], _ = bench_mlkem(cx, "mlkem1024", 21, min(args.steps, 5), 3, with_profile=False,
+                line["mlkem1024"], _ = bench_mlkem(cx, "mlkem1024", 21, args.steps, 3, with_profile=False,
                                                    with_cpu=False, e2e_steps=2)
     if cx.rank == 0:
         print(json.dumps(line))

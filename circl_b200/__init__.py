@@ -1,4 +1,4 @@
-"""circl_b200 -- B200 (sm_100a) batch polynomial-ring engine for CIRCL's
+"""circl_b200 -- H100 (sm_90a) batch polynomial-ring engine for CIRCL's
 module-lattice hot path (ML-KEM / ML-DSA).
 
 The product is ``libcirclb200.so`` (hand-written CUDA behind the C ABI in

@@ -114,7 +114,7 @@ def lib() -> C.CDLL:
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            # Not a fallback: the only way forward is the CUDA library itself, so build it (nvcc, sm_100a).
+            # Not a fallback: the only way forward is the CUDA library itself, so build it (nvcc, sm_90a).
             try:
                 from .build import build_library
                 build_library()

@@ -1,4 +1,4 @@
-"""Builds circl_b200/libcirclb200.so in-tree with nvcc for sm_100a (no JIT, no torch)."""
+"""Builds circl_b200/libcirclb200.so in-tree with nvcc for sm_90a (no JIT, no torch)."""
 from __future__ import annotations
 
 import concurrent.futures as cf
@@ -14,7 +14,7 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libcirclb200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -54,7 +54,7 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
         objs = list(ex.map(lambda s: _compile(s, digest, verbose), srcs))
     newest = max(os.path.getmtime(o) for o in objs)
     if force or not os.path.exists(LIB) or os.path.getmtime(LIB) < newest:
-        r = subprocess.run([NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a",
+        r = subprocess.run([NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a",
                             "-cudart", "static"], capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

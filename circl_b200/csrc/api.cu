@@ -263,8 +263,8 @@ static int dev_create(int device, std::unique_ptr<Dev>* out) {
   CB200_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   CB200_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("cb200_init: device %d is sm_%d%d; this build contains only sm_100a code", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("cb200_init: device %d is sm_%d%d; this build contains only sm_90a code", device, prop.major, prop.minor);
     return CB200_ERR_NOT_INIT;
   }
   std::unique_ptr<Dev> d(new Dev);
@@ -550,7 +550,7 @@ using namespace cb200;
 
 extern "C" {
 
-const char* cb200_version(void) { return "circl_b200 0.2 (sm_100a)"; }
+const char* cb200_version(void) { return "circl_b200 0.2 (sm_90a)"; }
 const char* cb200_last_error(void) { return g_err; }
 
 int cb200_device_count(void) {
@@ -690,7 +690,7 @@ void* cb200_host_alloc(size_t bytes) {
 }
 // One pinned buffer for a batch that cb200_* host-pointer calls will split over all active GPUs: the rows of shard s
 // (the split of for_each_shard) are first touched by the worker thread of the GPU that will copy them, which runs on
-// that GPU's NUMA node, so every GPU's copies stay on its own socket (profiles/r02_pcie_multi_probe.txt).
+// that GPU's NUMA node, so every GPU's copies stay on its own socket.
 static std::mutex g_map_mu;
 static std::map<void*, size_t> g_mapped;  // buffers of cb200_host_alloc_batch: mmap + cudaHostRegister
 

@@ -1,12 +1,10 @@
-// circl_b200/csrc/common.cuh -- shared helpers for the sm_100a kernels.
+// circl_b200/csrc/common.cuh -- shared helpers for the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
 
 namespace cb200 {
-
-constexpr int kNumSM = 148;  // B200: 2 dies x 74 SMs
 
 // Error plumbing for the C ABI: every failure is recorded and surfaced through
 // cb200_last_error(); there is no CPU fallback anywhere in the library.

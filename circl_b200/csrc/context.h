@@ -55,7 +55,7 @@ struct WorkSet {
 
 struct Dev {
   int device = -1;
-  int sm_count = 148;           // multiprocessors of the device (sizes the persistent grids)
+  int sm_count = 0;             // multiprocessors of the device (sizes the persistent grids)
   void* kyber_tw = nullptr;     // 128 x {zeta, zetaq}, then 128 x {zp, kk} (kyber.cuh, low format)
   void* dil_tw = nullptr;       // 256 x {zeta, invzeta}
   void* x25519_table = nullptr; // 32 KiB: multiples 1..8 of 256^i B for the fixed-base X25519 KeyGen (x25519.cuh)

@@ -1,4 +1,4 @@
-// circl_b200/csrc/dil_kernels.cu -- batched q=8380417 kernels (sm_100a), launchers and C ABI.
+// circl_b200/csrc/dil_kernels.cu -- batched q=8380417 kernels (sm_90a), launchers and C ABI.
 //
 // cb200_dil_ntt      <- (*Poly).NTT / InvNTT   sign/internal/dilithium/generic.go:11,15 (stubs_amd64.go:8-14)
 // cb200_dil_mulhat   <- (*Poly).MulHat         generic.go:19 (poly.go:88)
@@ -149,7 +149,7 @@ __global__ void __launch_bounds__(256) pack_le16_kernel(uint32_t* __restrict__ o
 
 static int grid_for(size_t units, int per_cta, int ctas_per_sm) {
   size_t want = (units + per_cta - 1) / per_cta;
-  size_t cap = (size_t)kNumSM * ctas_per_sm;
+  size_t cap = (size_t)ctx().sm_count * ctas_per_sm;
   return (int)(want < cap ? (want ? want : 1) : cap);
 }
 

@@ -1,4 +1,4 @@
-// circl_b200/csrc/dilithium.cuh -- q = 8380417 ring arithmetic for sm_100a.
+// circl_b200/csrc/dilithium.cuh -- q = 8380417 ring arithmetic for sm_90a.
 //
 // Replaces (bit-exactly, *generic* semantics; the reference's AVX2 path equals generic here):
 //   sign/internal/dilithium/field.go:5-32     ReduceLe2Q / le2qModQ / montReduceLe2Q
@@ -80,9 +80,8 @@ __device__ __forceinline__ uint32_t mont_le2q(uint64_t x) {  // field.go:20-24
   return (uint32_t)((x + (uint64_t)m * Q) >> 32);
 }
 __device__ __forceinline__ uint32_t mont_mul(uint32_t a, uint32_t b) { return mont_le2q((uint64_t)a * b); }
-// hi32(k * b).  Written as a wide multiplication on purpose: IMAD.WIDE.U32 issues faster than IMAD.HI.U32 on this part
-// (0.24 against 0.18 warp instructions per clock and sub-partition, profiles/r01c_ubench_imad_wide.txt,
-// r01_ubench_pipes.txt), and the compiler turns the plain C expression into the latter.
+// hi32(k * b).  Written as a wide multiplication on purpose (IMAD.WIDE.U32; scripts/ubench_pipes.cu measures its issue
+// rate against IMAD.HI.U32): the compiler turns the plain C expression into the latter.
 __host__ __device__ __forceinline__ uint32_t mulhi_wide(uint32_t k, uint32_t b) {
 #ifdef __CUDA_ARCH__
   uint32_t hi;

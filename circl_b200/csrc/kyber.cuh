@@ -1,4 +1,4 @@
-// circl_b200/csrc/kyber.cuh -- q = 3329 ring arithmetic for sm_100a.
+// circl_b200/csrc/kyber.cuh -- q = 3329 ring arithmetic for sm_90a.
 //
 // Replaces (bit-exactly, standard coefficient order, *generic* semantics):
 //   pke/kyber/internal/common/field.go:4-74       montReduce / barrettReduce / csubq / toMont

@@ -1,4 +1,4 @@
-// circl_b200/csrc/kyber_kernels.cu -- batched q=3329 kernels (sm_100a) and their launchers.
+// circl_b200/csrc/kyber_kernels.cu -- batched q=3329 kernels (sm_90a) and their launchers.
 //
 // cb200_kyber_ntt      <- (*Poly).NTT / InvNTT      pke/kyber/internal/common/generic.go:24,36 (stubs_amd64.go:8-14)
 // cb200_kyber_mulhat   <- (*Poly).MulHat            generic.go:49 (stubs_amd64.go:17)
@@ -88,12 +88,10 @@ constexpr int kFwdCtasPerSm = 5, kInvCtasPerSm = 6;
 //   * In-contract polynomials (words_in_range, warp-uniform vote) run the low-format fast path of kyber.cuh: 5-instruction
 //     butterflies, 128-bit transposition through the octet's own tile, per-lane twiddle pairs in registers.  Any other
 //     input runs the general high-half code (int16 wrap-around exact) on the same words.
-// Measured on a B200 (profiles/r02y_*): 92 registers, 5 CTAs per SM; both integer pipes ~70 % busy, issue 78 %.
-// Slower in the same sweep (profiles/r02y_ntt_variants*.json): the pairs read from shared memory at 6 / 7 CTAs per SM,
-// two slots per octet, the whole shared-memory carve-out.  Also measured and dropped (profiles/r02z4_bench.json): output /
-// input of the C-layout side in 128-byte-contiguous order through the tile, which takes the Dilithium kernels from 0.62 to
-// 0.89 of the HBM peak (their lanes are 128 bytes apart and the kernel waits on the memory pipeline) but costs these
-// pipe-bound kernels 1-2 % (eight more shared-memory instructions per polynomial, lanes only 64 bytes apart).
+// 5 CTAs per SM: the kernel is bound by the two integer pipes.  Tried and dropped: the pairs read from shared memory at
+// 6 / 7 CTAs per SM, two slots per octet, the whole shared-memory carve-out, and output / input of the C-layout side in
+// 128-byte-contiguous order through the tile (what the Dilithium kernels do: their lanes are 128 bytes apart and they wait
+// on the memory pipeline), which costs these pipe-bound kernels eight more shared-memory instructions per polynomial.
 __global__ void __launch_bounds__(kThreads, kFwdCtasPerSm) ntt_fwd_kernel(uint32_t* __restrict__ polys, size_t n,
                                                                           const TwPair* __restrict__ tw) {
   extern __shared__ __align__(16) unsigned char dsm[];
@@ -251,7 +249,7 @@ __global__ void __launch_bounds__(kThreads, kInvCtasPerSm) ntt_inv_kernel(uint32
 
 static int grid_for(size_t units, int per_cta, int ctas_per_sm) {
   size_t want = (units + per_cta - 1) / per_cta;
-  size_t cap = (size_t)kNumSM * ctas_per_sm;
+  size_t cap = (size_t)ctx().sm_count * ctas_per_sm;
   return (int)(want < cap ? (want ? want : 1) : cap);
 }
 

@@ -1,4 +1,4 @@
-// circl_b200/csrc/mldsa.cu -- batched ML-DSA-65 Sign on sm_100a.
+// circl_b200/csrc/mldsa.cu -- batched ML-DSA-65 Sign on sm_90a.
 //
 // Replaces, per signature and bit-exactly:
 //   (*PrivateKey).Unpack        sign/mldsa/mldsa65/internal/dilithium.go:142-163  (ExpandA, NTT of s1, s2, t0)
@@ -485,12 +485,10 @@ __device__ __forceinline__ void decompose(uint32_t a, uint32_t& a0plusq, uint32_
 // each octet keeps kWSlots 1 KB bulk copies (TMA engine, one mbarrier per slot) in flight into the octet's ring in
 // shared memory, always kWSlots polynomials ahead of the arithmetic, also across the end of a row, so the DRAM
 // latency of the next row hides behind the inverse NTT and Decompose of the current one.
-// Measured on a B200 (profiles/r02_sweeps.txt, ML-DSA-65, 2^18 signatures): the kernel is bound by latency, not by a pipe
-// or by HBM, and resident warps are what it responds to.  Twiddles read from shared memory (154 -> 120 registers) and a
-// ring of two slots instead of three fit four CTAs per SM instead of three: 20.9 -> 18.7 ms per step.  Summing the L
-// products of a coefficient as 64-bit integers with one Montgomery reduction at the end saves a tenth of the
-// instructions but costs 32 registers (19.3 ms at three CTAs, 19.9 ms with spills at four); y-hat one polynomial ahead
-// in registers costs another 32 and is far slower at two CTAs per SM (33 ms).
+// The kernel is bound by latency, not by a pipe or by HBM, and resident warps are what it responds to: twiddles read from
+// shared memory and a ring of two slots instead of three fit four CTAs per SM instead of three.  Summing the L products
+// of a coefficient as 64-bit integers with one Montgomery reduction at the end saves a tenth of the instructions but
+// costs 32 registers, and y-hat one polynomial ahead in registers costs another 32: both lose resident warps.
 constexpr int kWSlots = 2;
 constexpr int kWCtas = 4;  // CTAs per SM the grid and the register allocation are sized for
 struct WSm {

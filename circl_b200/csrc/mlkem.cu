@@ -1,4 +1,4 @@
-// circl_b200/csrc/mlkem.cu -- batched ML-KEM-768 / ML-KEM-1024 Encapsulate on sm_100a.
+// circl_b200/csrc/mlkem.cu -- batched ML-KEM-768 / ML-KEM-1024 Encapsulate on sm_90a.
 //
 // Replaces, per operation and bit-exactly:
 //   scheme.UnmarshalBinaryPublicKey   kem/mlkem/mlkem768/kyber.go:390-396 -> :247-263
@@ -164,9 +164,9 @@ __device__ __forceinline__ void cbd2_store(const uint64_t (&a)[25], int16_t* __r
   }
 }
 
-// sub-batch size: A^T + noise of one sub-batch (8 KiB / op for K=3, 12.5 KiB for K=4) stay L2-resident
-// (measured on a B200, profiles/r02_sweeps.txt: 8192 and 12288 are equally fast, 6144 is 1 % and 4096 is 7 % slower)
-constexpr size_t kSub = 8192;
+// sub-batch size: A^T + noise of one sub-batch (8 KiB / op for K=3, 12.5 KiB for K=4) stay in the 50 MB L2
+// (ML-KEM-768, 2^20 per-op keys, H100 SXM at 400 W: 24.7 ms per step at 4096, 25.5 at 8192, 30.0 at 2048)
+constexpr size_t kSub = 4096;
 constexpr int kRowWords = 129;  // 256 int16 + 2 slack, odd word stride
 constexpr int kSampleSmem = 128 * kRowWords * 4;
 
@@ -505,8 +505,8 @@ __device__ __forceinline__ int32_t mont_red_lo(int32_t p) { return mont_red_hi(p
 // directly -- floor((x' 2^d + 1664) / q) as a 32 x 32 -> 64 multiplication by ceil(2^40 / q), exact below 2^28 -- and the
 // Normalize of cpapke.go:176-177 needs no instruction of its own.  Checked exhaustively against the reference's two
 // constant pairs for every 16-bit x' and d in {4, 5, 10, 11} (tests/test_compress_identity.py).
-// hi32(a * b) as a wide multiplication: IMAD.WIDE.U32 issues faster than the IMAD.HI.U32 __umulhi compiles to (0.24
-// against 0.18 per clock and sub-partition, profiles/r01c_ubench_imad_wide.txt)
+// hi32(a * b) as a wide multiplication (IMAD.WIDE.U32) rather than the IMAD.HI.U32 __umulhi compiles to; the issue rates
+// of the two are what scripts/ubench_pipes.cu measures
 __device__ __forceinline__ uint32_t umulhi_wide(uint32_t a, uint32_t b) {
   uint32_t hi;
   asm("{ .reg .b64 t; mul.wide.u32 t, %1, %2; mov.b64 {_, %0}, t; }" : "=r"(hi) : "r"(a), "r"(b));
@@ -828,8 +828,8 @@ template <int K>
 static int launch_encrypt(const uint8_t* ek, size_t ek_stride, const int16_t* A, int a_shared, const int16_t* noise,
                           const uint8_t* m, size_t n, uint8_t* ct, uint8_t* ss, uint8_t* status, int lenient,
                           cudaStream_t st) {
-  // 7 CTAs of 64 threads per SM (K = 4: 6, its operands and registers are larger); measured against 6 and 5:
-  // profiles/r02_sweeps.txt
+  // 7 CTAs of 64 threads per SM (K = 4: 6, its operands and registers are larger); H100 has the register file and
+  // shared memory per SM these were sized for
   return launch_encrypt_v<K, (K == 4 ? 6 : 7)>(ek, ek_stride, A, a_shared, noise, m, n, ct, ss, status, lenient, st);
 }
 
@@ -1815,7 +1815,7 @@ __global__ void __launch_bounds__(256) replicate_kernel(const uint4* __restrict_
 int replicate_rows(const uint8_t* src, uint8_t* dst, size_t width, size_t n, cudaStream_t st) {
   KernelScope ks(KID_HYBRID_GLUE, st);
   const size_t total = n * (width / 16);
-  replicate_kernel<<<(unsigned)std::min<size_t>((total + 255) / 256, 148 * 8), 256, 0, st>>>(
+  replicate_kernel<<<(unsigned)std::min<size_t>((total + 255) / 256, (size_t)ctx().sm_count * 8), 256, 0, st>>>(
       (const uint4*)src, (uint4*)dst, (int)(width / 16), n);
   CB200_CUDA(cudaGetLastError());
   return 0;

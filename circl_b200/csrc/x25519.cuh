@@ -5,7 +5,7 @@
 // (curve.go:7-37) and a Montgomery ladder over 64-bit limbs (curve.go:40-75, math/fp25519).
 //
 // Representation: ten signed limbs of alternately 26 and 25 bits (value = sum v[i] 2^ceil(25.5 i)), products
-// accumulated in 64 bits -- on sm_100a each product-accumulate is one IMAD.WIDE.  With ten independent accumulators
+// accumulated in 64 bits -- on sm_90a each product-accumulate is one IMAD.WIDE.  With ten independent accumulators
 // per multiplication the wide-multiply latency is covered inside a single thread, so the kernel runs one scalar
 // multiplication per thread and needs no shared memory.
 #pragma once

@@ -1,7 +1,7 @@
 //go:build cuda && cgo
 
 // Package cb200 is the cgo binding of libcirclb200.so (include/circl_b200.h):
-// the B200 batch engine for CIRCL's module-lattice hot path.
+// the cb200 batch engine for CIRCL's module-lattice hot path.
 //
 // NOTE: this file is delivered as source.  The build image has no Go toolchain
 // (`go version` fails), so it is reviewed, not compiled, here; every executable

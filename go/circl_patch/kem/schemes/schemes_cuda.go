@@ -1,7 +1,7 @@
 //go:build cuda && cgo
 
 // Drop-in file for github.com/cloudflare/circl/kem/schemes (next to schemes.go): with the `cuda` build tag the registry
-// entries "ML-KEM-768", "ML-KEM-1024" and "X-Wing" (kem/schemes/schemes.go:30-55) are served by the B200 engine; every
+// entries "ML-KEM-768", "ML-KEM-1024" and "X-Wing" (kem/schemes/schemes.go:30-55) are served by the cb200 engine; every
 // other scheme, and every build without the tag, is untouched.  ByName keeps matching on the lower-cased Name()
 // (schemes.go:57-72), which the GPU schemes do not change.
 //
@@ -22,7 +22,7 @@ import (
 // The file name sorts after schemes.go on purpose: the init functions of a package run in file-name order and the map
 // written here is made by the init of schemes.go.
 func init() {
-	if cb200.Init() != nil { // no usable B200: keep CIRCL's own schemes (the library itself has no CPU fallback)
+	if cb200.Init() != nil { // no usable H100: keep CIRCL's own schemes (the library itself has no CPU fallback)
 		return
 	}
 	for _, s := range []kem.Scheme{mlkem768cuda.Scheme(), mlkem1024cuda.Scheme(), xwingcuda.Scheme()} {

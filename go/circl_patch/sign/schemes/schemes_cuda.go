@@ -1,7 +1,7 @@
 //go:build cuda && cgo
 
 // Drop-in file for github.com/cloudflare/circl/sign/schemes (next to schemes.go): with the `cuda` build tag "ML-DSA-65"
-// (sign/schemes/schemes.go:33-50) is served by the B200 engine; ByName (schemes.go:56-71) is unchanged.
+// (sign/schemes/schemes.go:33-50) is served by the cb200 engine; ByName (schemes.go:56-71) is unchanged.
 //
 // Delivered as source: the build image has no Go toolchain (see INTEGRATION.md section 3).
 package schemes

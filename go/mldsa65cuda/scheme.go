@@ -1,6 +1,6 @@
 //go:build cuda && cgo
 
-// Package mldsa65cuda registers "ML-DSA-65" backed by the B200 engine, keeping sign.Scheme
+// Package mldsa65cuda registers "ML-DSA-65" backed by the cb200 engine, keeping sign.Scheme
 // (sign/sign.go:48-94) intact: Sign / Verify / DeriveKey go through the GPU (batch of one), everything
 // else (marshalling, crypto.Signer plumbing) delegates to CIRCL's own mldsa65 scheme; SignBatch and
 // VerifyBatch are the entry points that make a GPU worthwhile.

@@ -1,6 +1,6 @@
 //go:build cuda && cgo
 
-// Package mlkem1024cuda registers "ML-KEM-1024" backed by the B200 engine.  It keeps
+// Package mlkem1024cuda registers "ML-KEM-1024" backed by the cb200 engine.  It keeps
 // kem.Scheme (kem/kem.go:33-82) intact: every method that is not on the accelerated
 // path delegates to CIRCL's own mlkem1024 scheme; Encapsulate* go through the GPU
 // (batch of one), and EncapsulateBatch is the entry point that makes a GPU worthwhile.

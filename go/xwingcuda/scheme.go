@@ -1,6 +1,6 @@
 //go:build cuda && cgo
 
-// Package xwingcuda backs kem/xwing's scheme (kem/xwing/scheme.go:1-140) with the B200 engine.  As in
+// Package xwingcuda backs kem/xwing's scheme (kem/xwing/scheme.go:1-140) with the cb200 engine.  As in
 // mlkem768cuda, everything off the accelerated path delegates to CIRCL's own singleton; the deterministic
 // encapsulation is a batch of one and EncapsulateBatch is the entry point that makes a GPU worthwhile.  The
 // same pattern applies to kem/hybrid's X25519MLKEM768 with cb200.HybridEncaps (64-byte shared secrets).

@@ -1,5 +1,5 @@
 /*
- * include/circl_b200.h -- C ABI of libcirclb200.so, the B200 (sm_100a) batch
+ * include/circl_b200.h -- C ABI of libcirclb200.so, the H100 (sm_90a) batch
  * polynomial-ring engine behind CIRCL's module-lattice hot path.
  *
  * This is the surface a cgo shim binds (see INTEGRATION.md and go/).  Plain
@@ -187,7 +187,7 @@ int cb200_dil_pack_le16(uint8_t *out, const uint32_t *polys, size_t n);
 int cb200_mlkem_encaps(int k, const uint8_t *ek, size_t ek_stride, const uint8_t *seeds, uint8_t *ct, uint8_t *ss,
                        uint8_t *status, size_t n);
 /* The same on device pointers, with the result gather of the one-process-per-GPU launch fused into the flow: the rows of
- * every sub-batch (8192 operations) are also copied to push_ct + i*CiphertextSize / push_ss + i*32 -- typically this
+ * every sub-batch (4096 operations) are also copied to push_ct + i*CiphertextSize / push_ss + i*32 -- typically this
  * rank's place in rank 0's cb200_gather_alloc buffer, opened with cb200_gather_open -- as soon as they exist, by the
  * copy engines over NVLink while the following sub-batches compute.  Either may be NULL.  The calling thread's stream
  * is ordered after the pushes. */

@@ -7,7 +7,7 @@ root=$(git rev-parse --show-toplevel)
 wt=$(mktemp -d)
 git -C "$root" worktree add -q "$wt" "$ref"
 trap 'git -C "$root" worktree remove --force "$wt"' EXIT
-FL="-O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr"
+FL="-O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr"
 norm() { cuobjdump -sass "$1" | grep -E "^\s+/\*[0-9a-f]{4,5}\*/|Function :" | sed -E 's/\/\* 0x[0-9a-f]+ \*\///' | md5sum | cut -d' ' -f1; }
 rc=0
 for src in "$root"/circl_b200/csrc/*.cu; do

@@ -1,9 +1,16 @@
-// Is IDP.2A (dp2a: 16-bit x 8-bit pairs, accumulate) as fast as IMAD on sm_100a?  Decides the inner product of the
+// Is IDP.2A (dp2a: 16-bit x 8-bit pairs, accumulate) as fast as IMAD on sm_90a?  Decides the inner product of the
 // fused K-PKE encrypt kernel (csrc/mlkem.cu, matvec on packed coefficient pairs).
-// nvcc -O3 -gencode arch=compute_100a,code=sm_100a scripts/ubench_dp2a.cu -o /tmp/ubench_dp2a && /tmp/ubench_dp2a
+// nvcc -O3 -gencode arch=compute_90a,code=sm_90a scripts/ubench_dp2a.cu -o ubench_dp2a && ./ubench_dp2a
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+
+// multiprocessors of device 0: the grids below put the same number of CTAs on every SM
+static int sms() {
+  static int n = 0;
+  if (!n) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, 0);
+  return n;
+}
 
 #define ITERS 4096
 template <int MODE>
@@ -36,15 +43,15 @@ __global__ void k(uint32_t* out, uint32_t seed) {
 template <int MODE>
 void run(const char* name, int ops) {
   uint32_t* d;
-  cudaMalloc(&d, 148 * 1024 * 4);
+  cudaMalloc(&d, sms() * 1024 * 4);
   for (int warps = 8; warps <= 32; warps *= 2) {
-    k<MODE><<<148, warps * 32>>>(d, 12345);
+    k<MODE><<<sms(), warps * 32>>>(d, 12345);
     cudaDeviceSynchronize();
     cudaEvent_t a, b;
     cudaEventCreate(&a);
     cudaEventCreate(&b);
     cudaEventRecord(a);
-    k<MODE><<<148, warps * 32>>>(d, 12345);
+    k<MODE><<<sms(), warps * 32>>>(d, 12345);
     cudaEventRecord(b);
     cudaEventSynchronize(b);
     float ms;

@@ -1,8 +1,15 @@
-// Pipe-throughput microbenchmark for the integer ops the NTT butterflies use (sm_100a).
-// nvcc -O3 -gencode arch=compute_100a,code=sm_100a scripts/ubench_pipes.cu -o /tmp/ubench && /tmp/ubench
+// Pipe-throughput microbenchmark for the integer ops the NTT butterflies use (sm_90a).
+// nvcc -O3 -gencode arch=compute_90a,code=sm_90a scripts/ubench_pipes.cu -o ubench_pipes && ./ubench_pipes
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdint.h>
+
+// multiprocessors of device 0: the grids below put the same number of CTAs on every SM
+static int sms() {
+  static int n = 0;
+  if (!n) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, 0);
+  return n;
+}
 
 #define ITERS 4096
 template <int MODE>
@@ -72,15 +79,15 @@ __global__ void k(int32_t* out, int32_t seed) {
 template <int MODE>
 void run(const char* name, int ops_per_inner) {
   int32_t* d;
-  cudaMalloc(&d, 148 * 8 * 256 * 4);
+  cudaMalloc(&d, sms() * 8 * 256 * 4);
   for (int warps = 4; warps <= 32; warps *= 2) {
     // one CTA per SM with `warps` warps -> warps/4 per SMSP
-    k<MODE><<<148, warps * 32>>>(d, 12345);
+    k<MODE><<<sms(), warps * 32>>>(d, 12345);
     cudaDeviceSynchronize();
     cudaEvent_t a, b;
     cudaEventCreate(&a); cudaEventCreate(&b);
     cudaEventRecord(a);
-    k<MODE><<<148, warps * 32>>>(d, 12345);
+    k<MODE><<<sms(), warps * 32>>>(d, 12345);
     cudaEventRecord(b);
     cudaEventSynchronize(b);
     float ms; cudaEventElapsedTime(&ms, a, b);

@@ -1,14 +1,21 @@
-// Round-2 pipe microbenchmarks (sm_100a): where can ALU-pipe work of the ML-KEM step move to?
+// Round-2 pipe microbenchmarks (sm_90a): where can ALU-pipe work of the ML-KEM step move to?
 //   1. Keccak-f[1600] with H of its 58 32-bit half-rotations per round computed on the FMA pipe
 //      (IMAD.WIDE by 2^r from the constant bank + IMAD) instead of SHF on the ALU pipe.
 //   2. The q = 3329 butterfly in exact fp32 integer arithmetic (FMUL/FFMA/FADD) against the int32 Montgomery one.
 //   3. Both kinds of warps resident together (do the pipes overlap?).
-// nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -I circl_b200/csrc scripts/ubench_r02.cu -o gpurun_out/ubench_r02
+// nvcc -O3 -std=c++17 --expt-relaxed-constexpr -gencode arch=compute_90a,code=sm_90a -I circl_b200/csrc scripts/ubench_r02.cu -o ubench_r02
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
 
 #include "keccak.cuh"
+
+// multiprocessors of device 0: the grids below put the same number of CTAs on every SM
+static int sms() {
+  static int n = 0;
+  if (!n) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, 0);
+  return n;
+}
 
 using namespace cb200;
 
@@ -243,7 +250,7 @@ static float time_ms(void (*launch)(void)) {
 }
 
 static uint64_t* g_out;
-static int g_ctas = 148 * 4;
+static int g_ctas = 0;  // set in main
 constexpr int kPerms = 512, kIters = 4096;
 
 template <int H>
@@ -256,7 +263,7 @@ static void launch_mixed() { mixed_kernel<H, M><<<g_ctas, 128>>>(g_out, kPerms, 
 template <int H>
 static void report_keccak(const char* tag) {
   for (int per_sm : {3, 4, 6}) {
-    g_ctas = 148 * per_sm;
+    g_ctas = sms() * per_sm;
     const float ms = time_ms(launch_keccak<H>);
     const double perms = (double)g_ctas * 128 * kPerms;
     printf("keccak %-10s H=%3d  ctas/SM=%d  %.3f ms  %.3e keccak-f/s\n", tag, H, per_sm, ms, perms / (ms * 1e-3));
@@ -289,7 +296,7 @@ int main() {
   uint32_t p2[32];
   for (int i = 0; i < 32; i++) p2[i] = 1u << i;
   cudaMemcpyToSymbol(kPow2, p2, sizeof p2);
-  cudaMalloc(&g_out, (size_t)148 * 8 * 128 * 8);
+  cudaMalloc(&g_out, (size_t)sms() * 8 * 128 * 8);
   check<12>();
   check<29>();
   check<58>();
@@ -304,7 +311,7 @@ int main() {
   report_keccak<46>("mix");
   report_keccak<58>("mix");
   for (int per_sm : {4, 6, 8}) {
-    g_ctas = 148 * per_sm;
+    g_ctas = sms() * per_sm;
     float ms = time_ms(launch_bfly<0>);
     double nb = (double)g_ctas * 128 * kIters * 16;
     printf("bfly int32  ctas/SM=%d %.3f ms  %.3e bfly/s\n", per_sm, ms, nb / (ms * 1e-3));
@@ -312,7 +319,7 @@ int main() {
     printf("bfly fp32   ctas/SM=%d %.3f ms  %.3e bfly/s\n", per_sm, ms, nb / (ms * 1e-3));
   }
   for (int per_sm : {4, 6}) {
-    g_ctas = 148 * per_sm;
+    g_ctas = sms() * per_sm;
     printf("mixed (half the warps each; perms=%d iters=%d) ctas/SM=%d: keccak H=0 + int %.3f ms, H=0 + fp32 %.3f ms, "
            "H=29 + fp32 %.3f ms, H=29 + int %.3f ms\n",
            kPerms, kIters, per_sm, time_ms(launch_mixed<0, 0>), time_ms(launch_mixed<0, 1>), time_ms(launch_mixed<29, 1>),
