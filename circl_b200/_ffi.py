@@ -69,6 +69,7 @@ SYMBOLS = {
     "cb200_kyber_kem_encaps": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_kyber_kem_decaps": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_x25519": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_x448": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_xwing_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_xwing_encaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_xwing_decaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]),
@@ -78,6 +79,9 @@ SYMBOLS = {
     "cb200_hybrid_public_key_size": (C.c_size_t, [C.c_int]),
     "cb200_hybrid_private_key_size": (C.c_size_t, [C.c_int]),
     "cb200_hybrid_ciphertext_size": (C.c_size_t, [C.c_int]),
+    "cb200_hybrid_shared_key_size": (C.c_size_t, [C.c_int]),
+    "cb200_hybrid_seed_size": (C.c_size_t, [C.c_int]),
+    "cb200_hybrid_encapsulation_seed_size": (C.c_size_t, [C.c_int]),
     "cb200_mldsa_sign": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
     "cb200_mldsa_verify": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,

@@ -1,8 +1,10 @@
 // Callers on the wire side of the ML-KEM core (SURVEY.md 8(f) row 4), batched on the device:
 //   dh/x25519/key.go:44-56                      KeyGen / Shared            -> x25519_kernel (thread per op)
+//   dh/x448/key.go:33-46                        KeyGen / Shared            -> x448_kernel (thread per op)
 //   kem/xwing/xwing.go:47-66,108-130,209-272    X-Wing                      -> expand / combiner kernels around the
 //   kem/hybrid/hybrid.go:197-283, xkem.go       X25519MLKEM768,                ML-KEM / Kyber flows of mlkem.cu
-//                                               Kyber768-X25519, Kyber512-X25519
+//                                               Kyber768-X25519, Kyber512-X25519,
+//                                               Kyber768-X448, Kyber1024-X448
 // The lattice half of every scheme runs through the same device flows as cb200_mlkem_* / cb200_kyber_kem_*
 // (mlkem_internal.h); this file adds the curve half, the SHAKE256 seed splitting, the X-Wing combiner and the
 // strided copies that put the two halves next to each other in the packed keys and ciphertexts.
@@ -15,6 +17,7 @@
 #include "keccak.cuh"
 #include "mlkem_internal.h"
 #include "x25519.cuh"
+#include "x448.cuh"
 
 namespace cb200 {
 namespace hybrid {
@@ -60,6 +63,32 @@ __global__ void __launch_bounds__(128) x25519_base_kernel(const uint8_t* __restr
   ld8(k, scalars + i * s_stride);
   x25519::scalarmult_base(r, k, table);
   st8(out + i * o_stride, r);
+}
+
+__device__ __forceinline__ void ld14(uint32_t (&w)[x448::kWords], const uint8_t* p) {
+#pragma unroll
+  for (int i = 0; i < x448::kWords; i++) w[i] = reinterpret_cast<const uint32_t*>(p)[i];
+}
+// out[i] = X448(scalar[i], point[i] or u = 5); status[i] |= 1 when the point is of low order
+// (x448.Shared returning false -> kem.ErrPubKey in xkem.go:150-156).  All strides are multiples of 4.
+__global__ void __launch_bounds__(128) x448_kernel(const uint8_t* __restrict__ scalars, size_t s_stride,
+                                                   const uint8_t* __restrict__ points, size_t p_stride,
+                                                   uint8_t* __restrict__ out, size_t o_stride, uint8_t* __restrict__ status,
+                                                   size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint32_t p[x448::kWords], r[x448::kWords];
+  if (points) {
+    ld14(p, points + i * p_stride);
+  } else {  // KeyGen (key.go:33-35): u(G) = 5
+    p[0] = 5;
+#pragma unroll
+    for (int q = 1; q < x448::kWords; q++) p[q] = 0;
+  }
+  const bool ok = x448::scalarmult(r, reinterpret_cast<const uint32_t*>(scalars + i * s_stride), p);
+#pragma unroll
+  for (int q = 0; q < x448::kWords; q++) reinterpret_cast<uint32_t*>(out + i * o_stride)[q] = r[q];
+  if (status && !ok) status[i] |= 1;
 }
 
 // out[i] = SHAKE256(in[i] (inlen bytes, <= 64), outlen <= 128 bytes), thread per op; inlen and outlen multiples of 8
@@ -121,6 +150,15 @@ __global__ void __launch_bounds__(256) copy_rows_kernel(const uint8_t* __restric
   const int u = (int)(t % units);
   reinterpret_cast<uint4*>(dst + i * dst_stride)[u] = reinterpret_cast<const uint4*>(src + i * src_stride)[u];
 }
+// the same with 8-byte units, for the X448 hybrids whose lattice half starts at byte 56 of a row
+__global__ void __launch_bounds__(256) copy_rows8_kernel(const uint8_t* __restrict__ src, size_t src_stride,
+                                                         uint8_t* __restrict__ dst, size_t dst_stride, int units, size_t n) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n * units) return;
+  const size_t i = t / units;
+  const int u = (int)(t % units);
+  reinterpret_cast<uint2*>(dst + i * dst_stride)[u] = reinterpret_cast<const uint2*>(src + i * src_stride)[u];
+}
 __global__ void or_status_kernel(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, uint8_t mask, size_t n) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n && src[i]) dst[i] |= mask;
@@ -131,6 +169,15 @@ static inline unsigned blocks(size_t units, size_t per) { return (unsigned)((uni
 static void copy_rows(const uint8_t* src, size_t ss, uint8_t* dst, size_t ds, size_t width, size_t n, cudaStream_t st) {
   KernelScope ks(KID_HYBRID_GLUE, st);
   copy_rows_kernel<<<blocks(n * (width / 16), 256), 256, 0, st>>>(src, ss, dst, ds, (int)(width / 16), n);
+}
+static void copy_rows8(const uint8_t* src, size_t ss, uint8_t* dst, size_t ds, size_t width, size_t n, cudaStream_t st) {
+  KernelScope ks(KID_HYBRID_GLUE, st);
+  copy_rows8_kernel<<<blocks(n * (width / 8), 256), 256, 0, st>>>(src, ss, dst, ds, (int)(width / 8), n);
+}
+static void x448_launch(const uint8_t* k, size_t ks_, const uint8_t* p, size_t ps, uint8_t* o, size_t os, uint8_t* status,
+                        size_t n, cudaStream_t st) {
+  KernelScope ks(KID_X448, st);
+  x448_kernel<<<blocks(n, 128), 128, 0, st>>>(k, ks_, p, ps, o, os, status, n);
 }
 static void x25519_launch(const uint8_t* k, size_t ks_, const uint8_t* p, size_t ps, uint8_t* o, size_t os, uint8_t* status,
                           size_t n, cudaStream_t st) {
@@ -232,12 +279,15 @@ static int xwing_decaps_dev(const uint8_t* sk, size_t sk_stride, const uint8_t* 
 struct Hyb {
   int k, mlkem, x_first;
   size_t ek, dk, ct;  // sizes of the lattice half
+  size_t xs;          // size of the X half: 32 (X25519) or 56 (X448); its key, ciphertext, secret and seeds (xkem.go:41-46)
 };
 static bool hyb_of(int id, Hyb* h) {
   switch (id) {
-    case CB200_HYBRID_X25519MLKEM768: *h = {3, 1, 0, 1184, 2400, 1088}; return true;  // hybrid.go:58-62
-    case CB200_HYBRID_KYBER768_X25519: *h = {3, 0, 1, 1184, 2400, 1088}; return true;  // hybrid.go:40-44
-    case CB200_HYBRID_KYBER512_X25519: *h = {2, 0, 1, 800, 1632, 768}; return true;    // hybrid.go:34-38
+    case CB200_HYBRID_X25519MLKEM768: *h = {3, 1, 0, 1184, 2400, 1088, 32}; return true;  // hybrid.go:58-62
+    case CB200_HYBRID_KYBER768_X25519: *h = {3, 0, 1, 1184, 2400, 1088, 32}; return true;  // hybrid.go:40-44
+    case CB200_HYBRID_KYBER512_X25519: *h = {2, 0, 1, 800, 1632, 768, 32}; return true;    // hybrid.go:34-38
+    case CB200_HYBRID_KYBER768_X448: *h = {3, 0, 1, 1184, 2400, 1088, 56}; return true;    // hybrid.go:83-87
+    case CB200_HYBRID_KYBER1024_X448: *h = {4, 0, 1, 1568, 3168, 1568, 56}; return true;   // hybrid.go:89-93
   }
   return false;
 }
@@ -317,6 +367,71 @@ static int hybrid_decaps_dev(const Hyb& H, const uint8_t* sk, size_t sk_stride, 
   return 0;
 }
 
+// ---- the X448 hybrids (ids 3-4): X448 || round-3 Kyber.  The lattice half starts at byte 56 of every row, which is
+// 8- but not 16-byte aligned, so it is staged through aligned work areas (copy_rows8) for the 128-bit loads of the
+// lattice flows.  Seeds: key 64 -> SHAKE256 -> X seed (56) || Kyber seed (64); encapsulation 56 -> X seed (56) ||
+// Kyber seed (32) (hybrid.go:197-261); the X half's secret is SHAKE256(X seed, 56) (xkem.go:112-123).
+// ss = ss_X (56) || ss_Kyber (32).  Round-3 Kyber has no error of its own, so status carries only bit 0.
+static int hybrid448_keygen_dev(const Hyb& H, const uint8_t* seeds, uint8_t* pk, uint8_t* sk, size_t n, cudaStream_t st,
+                                int slot) {
+  Arena A;
+  int rc = arena(slot, n * (120 + 64 + H.ek + H.dk) + 8192, &A);
+  if (rc) return rc;
+  uint8_t *ex = A.take(n * 120), *ms = A.take(n * 64), *ek = A.take(n * H.ek), *dk = A.take(n * H.dk);
+  const size_t pks = H.ek + 56, sks = H.dk + 56;
+  shake_launch(seeds, 64, 64, ex, 120, 120, n, st);
+  shake_launch(ex, 120, 56, sk, sks, 56, n, st);
+  x448_launch(sk, sks, nullptr, 0, pk, pks, nullptr, n, st);
+  copy_rows8(ex + 56, 120, ms, 64, 64, n, st);
+  rc = mlkem::dev_keygen(H.k, 0, ms, ek, dk, n, st, slot);
+  if (rc) return rc;
+  copy_rows8(ek, H.ek, pk + 56, pks, H.ek, n, st);
+  copy_rows8(dk, H.dk, sk + 56, sks, H.dk, n, st);
+  CB200_CUDA(cudaGetLastError());
+  return 0;
+}
+// pk_stride 0: one public key for the whole batch
+static int hybrid448_encaps_dev(const Hyb& H, const uint8_t* pk, size_t pk_stride, const uint8_t* seeds, uint8_t* ct,
+                                uint8_t* ss, uint8_t* status, size_t n, cudaStream_t st, int slot) {
+  const size_t nk = pk_stride ? n : 1;
+  Arena A;
+  int rc = arena(slot, n * (88 + 56 + 32 + H.ct + 32) + nk * H.ek + 8192, &A);
+  if (rc) return rc;
+  uint8_t *ex = A.take(n * 88), *esk = A.take(n * 56), *m = A.take(n * 32), *ctm = A.take(n * H.ct),
+          *ssm = A.take(n * 32), *ek = A.take(nk * H.ek);
+  const size_t cts = H.ct + 56;
+  CB200_CUDA(cudaMemsetAsync(status, 0, n, st));
+  shake_launch(seeds, 56, 56, ex, 88, 88, n, st);
+  shake_launch(ex, 88, 56, esk, 56, 56, n, st);                  // ephemeral sk = SHAKE256(seed_X, 56)  (xkem.go:172)
+  x448_launch(esk, 56, nullptr, 0, ct, cts, nullptr, n, st);     // ct_X = its public key
+  x448_launch(esk, 56, pk, pk_stride, ss, 88, status, n, st);    // ss_X = Shared(esk, pk_X)
+  copy_rows8(ex + 56, 88, m, 32, 32, n, st);
+  copy_rows8(pk + 56, pk_stride, ek, H.ek, H.ek, nk, st);
+  rc = mlkem::dev_encaps(H.k, 0, ek, pk_stride ? H.ek : 0, m, ctm, ssm, nullptr, n, st, slot);
+  if (rc) return rc;
+  copy_rows8(ctm, H.ct, ct + 56, cts, H.ct, n, st);
+  copy_rows8(ssm, 32, ss + 56, 88, 32, n, st);
+  CB200_CUDA(cudaGetLastError());
+  return 0;
+}
+static int hybrid448_decaps_dev(const Hyb& H, const uint8_t* sk, size_t sk_stride, const uint8_t* ct, uint8_t* ss,
+                                uint8_t* status, size_t n, cudaStream_t st, int slot) {
+  Arena A;
+  int rc = arena(slot, n * (H.ct + H.dk + 32) + 8192, &A);
+  if (rc) return rc;
+  uint8_t *ctm = A.take(n * H.ct), *dk = A.take(n * H.dk), *ssm = A.take(n * 32);
+  const size_t cts = H.ct + 56;
+  CB200_CUDA(cudaMemsetAsync(status, 0, n, st));
+  x448_launch(sk, sk_stride, ct, cts, ss, 88, status, n, st);
+  copy_rows8(ct + 56, cts, ctm, H.ct, H.ct, n, st);
+  copy_rows8(sk + 56, sk_stride, dk, H.dk, H.dk, n, st);
+  rc = mlkem::dev_decaps(H.k, 0, dk, H.dk, ctm, ssm, nullptr, n, st, slot);
+  if (rc) return rc;
+  copy_rows8(ssm, 32, ss + 56, 88, 32, n, st);
+  CB200_CUDA(cudaGetLastError());
+  return 0;
+}
+
 // Every buffer of a call lives on the same side.  Host calls go through the staging pipeline in chunks.
 static bool same_side(std::initializer_list<const void*> ps, bool* dev) {
   bool first = true;
@@ -350,6 +465,13 @@ static bool aligned16(std::initializer_list<const void*> ps, std::initializer_li
   for (const void* p : ps) acc |= (uintptr_t)p;
   for (size_t v : strides) acc |= v;
   return (acc & 15) == 0;
+}
+// the X448 entry points and hybrids read and write their rows in 32- and 64-bit units
+static bool aligned8(std::initializer_list<const void*> ps, std::initializer_list<size_t> strides) {
+  uintptr_t acc = 0;
+  for (const void* p : ps) acc |= (uintptr_t)p;
+  for (size_t v : strides) acc |= v;
+  return (acc & 7) == 0;
 }
 
 }  // namespace hybrid
@@ -402,6 +524,50 @@ int cb200_x25519(const uint8_t* scalars, const uint8_t* points, uint8_t* out, ui
   rc = hc.run(n);
   if (rc) return rc;
   return status_result(hc.bit0, hc.bit1, n, "cb200_x25519");
+}
+
+int cb200_x448(const uint8_t* scalars, const uint8_t* points, uint8_t* out, uint8_t* status, size_t n) {
+  int rc = require_ready();
+  if (rc) return rc;
+  if (!scalars || !out) {
+    set_error("cb200_x448: null pointer");
+    return CB200_ERR_ARG;
+  }
+  if (n == 0) return 0;
+  bool dev = false;
+  if (!same_side({scalars, points, out, status}, &dev)) {
+    set_error("cb200_x448: mixed host/device pointers");
+    return CB200_ERR_ARG;
+  }
+  if (dev) {
+    if (!aligned8({scalars, points, out}, {})) {
+      set_error("cb200_x448: device buffers must be 8-byte aligned");
+      return CB200_ERR_ARG;
+    }
+    DeviceCall call(out);
+    if (call.rc) return call.rc;
+    if (status) CB200_CUDA(cudaMemsetAsync(status, 0, n, call.st));
+    x448_launch(scalars, 56, points, 56, out, 56, status, n, call.st);
+    CB200_CUDA(cudaGetLastError());
+    return 0;
+  }
+  HostCall hc;
+  hc.bufs = {Buf{scalars, nullptr, 56, false, 0}, Buf{nullptr, out, 56, false, 0}, Buf{nullptr, nullptr, 1, false, 0}};
+  if (points) hc.bufs.push_back(Buf{points, nullptr, 56, false, 0});
+  hc.chunk = 1u << 17;
+  hc.min_shard = 1u << 14;
+  hc.status_buf = 2;
+  hc.user_status = status;
+  hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int) -> int {
+    CB200_CUDA(cudaMemsetAsync(d[2], 0, cnt, st));
+    x448_launch((const uint8_t*)d[0], 56, points ? (const uint8_t*)d[3] : nullptr, 56, (uint8_t*)d[1], 56, (uint8_t*)d[2],
+                cnt, st);
+    CB200_CUDA(cudaGetLastError());
+    return 0;
+  };
+  rc = hc.run(n);
+  if (rc) return rc;
+  return status_result(hc.bit0, hc.bit1, n, "cb200_x448");
 }
 
 int cb200_xwing_keygen(const uint8_t* seeds, uint8_t* pk, size_t n) {
@@ -502,15 +668,27 @@ int cb200_xwing_decaps(const uint8_t* sk, size_t sk_stride, const uint8_t* ct, u
 
 size_t cb200_hybrid_public_key_size(int id) {
   Hyb h;
-  return hyb_of(id, &h) ? h.ek + 32 : 0;
+  return hyb_of(id, &h) ? h.ek + h.xs : 0;
 }
 size_t cb200_hybrid_private_key_size(int id) {
   Hyb h;
-  return hyb_of(id, &h) ? h.dk + 32 : 0;
+  return hyb_of(id, &h) ? h.dk + h.xs : 0;
 }
 size_t cb200_hybrid_ciphertext_size(int id) {
   Hyb h;
-  return hyb_of(id, &h) ? h.ct + 32 : 0;
+  return hyb_of(id, &h) ? h.ct + h.xs : 0;
+}
+size_t cb200_hybrid_shared_key_size(int id) {  // hybrid.go:141-143
+  Hyb h;
+  return hyb_of(id, &h) ? 32 + h.xs : 0;
+}
+size_t cb200_hybrid_seed_size(int id) {  // max(X seed, lattice seed 64), hybrid.go:131-139
+  Hyb h;
+  return hyb_of(id, &h) ? 64 : 0;
+}
+size_t cb200_hybrid_encapsulation_seed_size(int id) {  // max(X seed, lattice seed 32), hybrid.go:149-157
+  Hyb h;
+  return hyb_of(id, &h) ? h.xs : 0;
 }
 
 int cb200_hybrid_keygen(int id, const uint8_t* seeds, uint8_t* pk, uint8_t* sk, size_t n) {
@@ -526,6 +704,22 @@ int cb200_hybrid_keygen(int id, const uint8_t* seeds, uint8_t* pk, uint8_t* sk, 
   if (!same_side({seeds, pk, sk}, &dev)) {
     set_error("cb200_hybrid_keygen: mixed host/device pointers");
     return CB200_ERR_ARG;
+  }
+  if (H.xs == 56) {
+    if (dev) {
+      if (!aligned8({seeds, pk, sk}, {})) {
+        set_error("cb200_hybrid_keygen: device buffers must be 8-byte aligned");
+        return CB200_ERR_ARG;
+      }
+      DeviceCall call(pk);
+      if (call.rc) return call.rc;
+      return hybrid448_keygen_dev(H, seeds, pk, sk, n, call.st, kDevSlot);
+    }
+    std::vector<Buf> bufs = {Buf{seeds, nullptr, 64, false, 0}, Buf{nullptr, pk, H.ek + 56, false, 0},
+                             Buf{nullptr, sk, H.dk + 56, false, 0}};
+    return run_host(bufs, n, 1u << 15, 1u << 13, [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
+      return hybrid448_keygen_dev(H, (const uint8_t*)d[0], (uint8_t*)d[1], (uint8_t*)d[2], cnt, st, slot);
+    });
   }
   if (dev) {
     if (!aligned16({seeds, pk, sk}, {})) {
@@ -548,7 +742,9 @@ int cb200_hybrid_encaps(int id, const uint8_t* pk, size_t pk_stride, const uint8
   int rc = require_ready();
   if (rc) return rc;
   Hyb H;
-  if (!hyb_of(id, &H) || !pk || !seeds || !ct || !ss || (pk_stride != 0 && pk_stride < H.ek + 32) || (pk_stride & 15)) {
+  // row strides: multiples of 16 for the X25519 hybrids, of 8 for the X448 ones
+  if (!hyb_of(id, &H) || !pk || !seeds || !ct || !ss || (pk_stride != 0 && pk_stride < H.ek + H.xs) ||
+      (pk_stride & (H.xs == 56 ? 7 : 15))) {
     set_error("cb200_hybrid_encaps: bad argument");
     return CB200_ERR_ARG;
   }
@@ -563,6 +759,15 @@ int cb200_hybrid_encaps(int id, const uint8_t* pk, size_t pk_stride, const uint8
       set_error("cb200_hybrid_encaps: device-pointer calls need a status array (it carries kem.ErrPubKey)");
       return CB200_ERR_ARG;
     }
+    if (H.xs == 56) {
+      if (!aligned8({pk, seeds, ct, ss}, {pk_stride})) {
+        set_error("cb200_hybrid_encaps: device buffers must be 8-byte aligned");
+        return CB200_ERR_ARG;
+      }
+      DeviceCall call(ct);
+      if (call.rc) return call.rc;
+      return hybrid448_encaps_dev(H, pk, pk_stride, seeds, ct, ss, status, n, call.st, kDevSlot);
+    }
     if (!aligned16({pk, seeds, ct, ss}, {pk_stride})) {
       set_error("cb200_hybrid_encaps: device buffers must be 16-byte aligned");
       return CB200_ERR_ARG;
@@ -570,6 +775,23 @@ int cb200_hybrid_encaps(int id, const uint8_t* pk, size_t pk_stride, const uint8
     DeviceCall call(ct);
     if (call.rc) return call.rc;
     return hybrid_encaps_dev(H, pk, pk_stride, seeds, ct, ss, status, n, call.st, kDevSlot);
+  }
+  if (H.xs == 56) {
+    const size_t pks = H.ek + 56;
+    HostCall hc;
+    hc.bufs = {Buf{pk, nullptr, pks, pk_stride == 0, pk_stride}, Buf{seeds, nullptr, 56, false, 0},
+               Buf{nullptr, ct, H.ct + 56, false, 0}, Buf{nullptr, ss, 88, false, 0}, Buf{nullptr, nullptr, 1, false, 0}};
+    hc.chunk = 1u << 15;
+    hc.min_shard = 1u << 13;
+    hc.status_buf = 4;
+    hc.user_status = status;
+    hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
+      return hybrid448_encaps_dev(H, (const uint8_t*)d[0], pk_stride == 0 ? 0 : pks, (const uint8_t*)d[1], (uint8_t*)d[2],
+                                  (uint8_t*)d[3], (uint8_t*)d[4], cnt, st, slot);
+    };
+    rc = hc.run(n);
+    if (rc) return rc;
+    return status_result(hc.bit0, hc.bit1, n, "cb200_hybrid_encaps");
   }
   const size_t pks = H.ek + 32;
   HostCall hc;
@@ -592,7 +814,7 @@ int cb200_hybrid_decaps(int id, const uint8_t* sk, size_t sk_stride, const uint8
   int rc = require_ready();
   if (rc) return rc;
   Hyb H;
-  if (!hyb_of(id, &H) || !sk || !ct || !ss || sk_stride < H.dk + 32 || (sk_stride & 15)) {
+  if (!hyb_of(id, &H) || !sk || !ct || !ss || sk_stride < H.dk + H.xs || (sk_stride & (H.xs == 56 ? 7 : 15))) {
     set_error("cb200_hybrid_decaps: bad argument (one decapsulation key per operation: sk_stride >= key size)");
     return CB200_ERR_ARG;
   }
@@ -607,6 +829,15 @@ int cb200_hybrid_decaps(int id, const uint8_t* sk, size_t sk_stride, const uint8
       set_error("cb200_hybrid_decaps: device-pointer calls need a status array (it carries kem.ErrPubKey / kem.ErrPrivKey)");
       return CB200_ERR_ARG;
     }
+    if (H.xs == 56) {
+      if (!aligned8({sk, ct, ss}, {})) {
+        set_error("cb200_hybrid_decaps: device buffers must be 8-byte aligned");
+        return CB200_ERR_ARG;
+      }
+      DeviceCall call(ss);
+      if (call.rc) return call.rc;
+      return hybrid448_decaps_dev(H, sk, sk_stride, ct, ss, status, n, call.st, kDevSlot);
+    }
     if (!aligned16({sk, ct, ss}, {})) {
       set_error("cb200_hybrid_decaps: device buffers must be 16-byte aligned");
       return CB200_ERR_ARG;
@@ -614,6 +845,23 @@ int cb200_hybrid_decaps(int id, const uint8_t* sk, size_t sk_stride, const uint8
     DeviceCall call(ss);
     if (call.rc) return call.rc;
     return hybrid_decaps_dev(H, sk, sk_stride, ct, ss, status, n, call.st, kDevSlot);
+  }
+  if (H.xs == 56) {
+    const size_t sks = H.dk + 56;
+    HostCall hc;
+    hc.bufs = {Buf{sk, nullptr, sks, false, sk_stride}, Buf{ct, nullptr, H.ct + 56, false, 0},
+               Buf{nullptr, ss, 88, false, 0}, Buf{nullptr, nullptr, 1, false, 0}};
+    hc.chunk = 1u << 15;
+    hc.min_shard = 1u << 13;
+    hc.status_buf = 3;
+    hc.user_status = status;
+    hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
+      return hybrid448_decaps_dev(H, (const uint8_t*)d[0], sks, (const uint8_t*)d[1], (uint8_t*)d[2], (uint8_t*)d[3], cnt, st,
+                                  slot);
+    };
+    rc = hc.run(n);
+    if (rc) return rc;
+    return status_result(hc.bit0, hc.bit1, n, "cb200_hybrid_decaps");
   }
   const size_t sks = H.dk + 32;
   HostCall hc;

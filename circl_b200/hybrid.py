@@ -195,22 +195,22 @@ class Hybrid(_Base):
     def PublicKeySize(self): return lib().cb200_hybrid_public_key_size(self._id)
     def PrivateKeySize(self): return lib().cb200_hybrid_private_key_size(self._id)
     def CiphertextSize(self): return lib().cb200_hybrid_ciphertext_size(self._id)
-    def SeedSize(self): return 64              # max(first.SeedSize, second.SeedSize), hybrid.go:91-99
-    def EncapsulationSeedSize(self): return 32  # hybrid.go:109-117
-    def SharedKeySize(self): return 64
+    def SeedSize(self): return lib().cb200_hybrid_seed_size(self._id)  # max(first, second), hybrid.go:131-139
+    def EncapsulationSeedSize(self): return lib().cb200_hybrid_encapsulation_seed_size(self._id)  # hybrid.go:149-157
+    def SharedKeySize(self): return lib().cb200_hybrid_shared_key_size(self._id)  # hybrid.go:141-143
 
     def DeriveKeyPairBatch(self, seeds):
-        s = _prep(seeds, 64, ValueError("kem: invalid seed size"))
+        s = _prep(seeds, self.SeedSize(), ValueError("kem: invalid seed size"))
         n = s.shape[0]
         pk, sk = _new(s, (n, self.PublicKeySize())), _new(s, (n, self.PrivateKeySize()))
         check(lib().cb200_hybrid_keygen(self._id, _ptr(s), _ptr(pk), _ptr(sk), n))
         return pk, sk
 
     def EncapsulateBatch(self, pks, seeds):
-        es = _prep(seeds, 32, ErrSeedSize("kem: invalid seed size"))
+        es = _prep(seeds, self.EncapsulationSeedSize(), ErrSeedSize("kem: invalid seed size"))
         n = es.shape[0]
         pk, stride = self._keys(pks, PublicKey, self.PublicKeySize(), n, es, ErrPubKeySize("kem: invalid public key size"))
-        ct, ss, status = _new(es, (n, self.CiphertextSize())), _new(es, (n, 64)), _zeros(es, (n,))
+        ct, ss, status = _new(es, (n, self.CiphertextSize())), _new(es, (n, self.SharedKeySize())), _zeros(es, (n,))
         try:
             check(lib().cb200_hybrid_encaps(self._id, _ptr(pk), stride, _ptr(es), _ptr(ct), _ptr(ss), _ptr(status), n))
         except Cb200Error as e:
@@ -225,7 +225,7 @@ class Hybrid(_Base):
         sk, stride = self._keys(sks, PrivateKey, sksz, n, c, ErrPrivKeySize("kem: invalid private key size"))
         if stride == 0:  # the decapsulation flows take one key per operation
             sk = sk.repeat(n, 1) if _is_torch(sk) else np.repeat(sk, n, axis=0)
-        ss, status = _new(c, (n, 64)), _zeros(c, (n,))
+        ss, status = _new(c, (n, self.SharedKeySize())), _zeros(c, (n,))
         try:
             check(lib().cb200_hybrid_decaps(self._id, _ptr(sk), sksz, _ptr(c), _ptr(ss), _ptr(status), n))
         except Cb200Error as e:

@@ -205,11 +205,13 @@ func MLDSA65Sign(sk []byte, shared bool, msgs [][]byte, ctx, rnd, sig []byte) er
 	})
 }
 
-// Hybrid scheme identifiers of include/circl_b200.h (kem/hybrid/hybrid.go:34-62).
+// Hybrid scheme identifiers of include/circl_b200.h (kem/hybrid/hybrid.go:34-93).
 const (
 	HybridX25519MLKEM768 = 0
 	HybridKyber768X25519 = 1
 	HybridKyber512X25519 = 2
+	HybridKyber768X448   = 3
+	HybridKyber1024X448  = 4
 )
 
 // X25519Batch: x25519.KeyGen (points == nil) or x25519.Shared (dh/x25519/key.go:44-56) on n 32-byte keys.
@@ -242,6 +244,36 @@ func X25519Batch(scalars, points, out []byte, ok []bool) error {
 	return err
 }
 
+// X448Batch: x448.KeyGen (points == nil) or x448.Shared (dh/x448/key.go:33-46) on n 56-byte keys.
+// ok[i] is false where Shared would have returned false (low-order point); out[i] is then all zero.
+func X448Batch(scalars, points, out []byte, ok []bool) error {
+	n := len(scalars) / 56
+	if len(out) != n*56 || (points != nil && len(points) != n*56) || (ok != nil && len(ok) != n) {
+		panic("cb200: X448Batch buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	status := make([]byte, n)
+	var pp *C.uint8_t
+	if points != nil {
+		pp = (*C.uint8_t)(unsafe.Pointer(&points[0]))
+	}
+	var rc C.int
+	err := call(func() C.int {
+		rc = C.cb200_x448((*C.uint8_t)(unsafe.Pointer(&scalars[0])), pp, (*C.uint8_t)(unsafe.Pointer(&out[0])),
+			(*C.uint8_t)(unsafe.Pointer(&status[0])), C.size_t(n))
+		if rc == C.CB200_ERR_PUBKEY { // reported per operation through ok, like the bool of x448.Shared
+			return 0
+		}
+		return rc
+	})
+	for i := range ok {
+		ok[i] = status[i] == 0
+	}
+	return err
+}
+
 // XWingEncaps: batched xwing.Encapsulate (kem/xwing/xwing.go:173-182).  pk: one packed 1216-byte key (shared) or n keys;
 // seeds: n*64 bytes; ct: n*1120; ss: n*32.  kem.ErrPubKey is returned if any ML-KEM half is not canonical.
 func XWingEncaps(pk []byte, shared bool, seeds, ct, ss []byte) error {
@@ -263,16 +295,22 @@ func XWingEncaps(pk []byte, shared bool, seeds, ct, ss []byte) error {
 }
 
 // HybridEncaps: batched hybrid.scheme.EncapsulateDeterministically (kem/hybrid/hybrid.go:233-261); id is one of the
-// Hybrid* constants; seeds: n*32 bytes; ss: n*64 bytes (the two shared secrets side by side, hybrid.go:260).
+// Hybrid* constants; seeds: n*EncapsulationSeedSize bytes (32, or 56 for the X448 hybrids); ss: n*SharedKeySize
+// bytes (64, or 88 for the X448 hybrids: the two shared secrets side by side, hybrid.go:260).
 func HybridEncaps(id int, pk []byte, shared bool, seeds, ct, ss []byte) error {
-	n := len(seeds) / 32
+	seedSize := int(C.cb200_hybrid_encapsulation_seed_size(C.int(id)))
+	ssSize := int(C.cb200_hybrid_shared_key_size(C.int(id)))
+	if seedSize == 0 {
+		panic("cb200: HybridEncaps: unknown scheme id")
+	}
+	n := len(seeds) / seedSize
 	pkSize := int(C.cb200_hybrid_public_key_size(C.int(id)))
 	ctSize := int(C.cb200_hybrid_ciphertext_size(C.int(id)))
 	stride := C.size_t(pkSize)
 	if shared {
 		stride = 0
 	}
-	if len(ct) != n*ctSize || len(ss) != n*64 || (shared && len(pk) != pkSize) || (!shared && len(pk) != n*pkSize) {
+	if len(ct) != n*ctSize || len(ss) != n*ssSize || (shared && len(pk) != pkSize) || (!shared && len(pk) != n*pkSize) {
 		panic("cb200: HybridEncaps buffers have the wrong length")
 	}
 	if n == 0 {

@@ -225,6 +225,10 @@ int cb200_kyber_kem_decaps(int k, const uint8_t *dk, size_t dk_stride, const uin
  * 32-byte scalars / points; status[i] = 1 where the point has small order (Shared returning false); the output is
  * then all zero and the host-pointer call returns CB200_ERR_PUBKEY after finishing the batch. */
 int cb200_x25519(const uint8_t *scalars, const uint8_t *points, uint8_t *out, uint8_t *status, size_t n);
+/* dh/x448 KeyGen (points == NULL: u = 5, key.go:33-35) or Shared (key.go:41-46) on n 56-byte scalars / points;
+ * status and return value as cb200_x25519 (low order: the residue mod p is 0, 1 or p - 1, curve.go:76-104).
+ * Device pointers: 8-byte aligned. */
+int cb200_x448(const uint8_t *scalars, const uint8_t *points, uint8_t *out, uint8_t *status, size_t n);
 
 /* X-Wing (kem/xwing/xwing.go:32-44): seed / sk 32, pk 1216 (ML-KEM-768 ek || X25519 pk), encapsulation seed 64,
  * ct 1120, ss 32.  keygen = DeriveKeyPairPacked (:131-141; the packed sk is the seed itself), encaps = Encapsulate
@@ -235,12 +239,16 @@ int cb200_xwing_encaps(const uint8_t *pk, size_t pk_stride, const uint8_t *eseed
                        uint8_t *status, size_t n);
 int cb200_xwing_decaps(const uint8_t *sk, size_t sk_stride, const uint8_t *ct, uint8_t *ss, size_t n);
 
-/* kem/hybrid (hybrid.go:197-283 over xkem.go): keys, ciphertexts and the 64-byte shared secret are the two halves
- * side by side in the order of hybrid.go:34-62; key seed 64, encapsulation seed 32.
- * status bit 0 = kem.ErrPubKey (non-canonical ML-KEM ek or small-order X25519 share), bit 1 = kem.ErrPrivKey. */
+/* kem/hybrid (hybrid.go:197-283 over xkem.go): keys, ciphertexts and shared secrets are the two halves side by side
+ * in the order of hybrid.go:34-93.  The sizes follow from the id (cb200_hybrid_*_size): shared secret 64 for the
+ * X25519 hybrids and 88 for the X448 ones, key seed 64, encapsulation seed 32 (X25519) or 56 (X448).
+ * status bit 0 = kem.ErrPubKey (non-canonical ML-KEM ek or low-order X25519 / X448 share), bit 1 = kem.ErrPrivKey.
+ * Device pointers and strides: 16-byte aligned for ids 0-2, 8-byte aligned for ids 3-4. */
 #define CB200_HYBRID_X25519MLKEM768 0  /* ML-KEM-768 || X25519:  pk 1216, sk 2432, ct 1120 */
 #define CB200_HYBRID_KYBER768_X25519 1 /* X25519 || Kyber768:    pk 1216, sk 2432, ct 1120 */
 #define CB200_HYBRID_KYBER512_X25519 2 /* X25519 || Kyber512:    pk 832,  sk 1664, ct 800  */
+#define CB200_HYBRID_KYBER768_X448  3  /* X448 || Kyber768:      pk 1240, sk 2456, ct 1144, ss 88 */
+#define CB200_HYBRID_KYBER1024_X448 4  /* X448 || Kyber1024:     pk 1624, sk 3224, ct 1624, ss 88 */
 int cb200_hybrid_keygen(int id, const uint8_t *seeds, uint8_t *pk, uint8_t *sk, size_t n);
 int cb200_hybrid_encaps(int id, const uint8_t *pk, size_t pk_stride, const uint8_t *seeds, uint8_t *ct, uint8_t *ss,
                         uint8_t *status, size_t n);
@@ -249,6 +257,9 @@ int cb200_hybrid_decaps(int id, const uint8_t *sk, size_t sk_stride, const uint8
 size_t cb200_hybrid_public_key_size(int id);
 size_t cb200_hybrid_private_key_size(int id);
 size_t cb200_hybrid_ciphertext_size(int id);
+size_t cb200_hybrid_shared_key_size(int id);         /* 64 for ids 0-2, 88 for ids 3-4 */
+size_t cb200_hybrid_seed_size(int id);               /* 64 for every id */
+size_t cb200_hybrid_encapsulation_seed_size(int id); /* 32 for ids 0-2, 56 for ids 3-4 */
 
 /* ---- ML-DSA (mode = 44, 65 or 87) and round-3 Dilithium (mode = 2, 3 or 5); sign/dilithium/gen.go:80-162 ----
  * Same contracts as the ML-DSA-65 entry points documented below, with the parameter set as first argument:

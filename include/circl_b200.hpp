@@ -93,7 +93,8 @@ class PrivateKey {  // kem.PrivateKey (kem/kem.go:22-30)
 //   MLKEM   ML-KEM-512/768/1024            kem/mlkem/mlkem768/kyber.go:267-407
 //   KYBER3  round-3 Kyber512/768/1024      kem/kyber/kyber768/kyber.go:267-407
 //   XWING   X-Wing                         kem/xwing/scheme.go:1-140
-//   HYBRID  X25519MLKEM768, Kyber768-X25519, Kyber512-X25519   kem/hybrid/hybrid.go:76-315
+//   HYBRID  X25519MLKEM768, Kyber768-X25519, Kyber512-X25519,
+//           Kyber768-X448, Kyber1024-X448                      kem/hybrid/hybrid.go:76-315
 class Scheme {
  public:
   enum Kind { MLKEM, KYBER3, XWING, HYBRID };
@@ -103,15 +104,17 @@ class Scheme {
   size_t CiphertextSize() const {
     return kind_ == XWING ? 1120 : kind_ == HYBRID ? cb200_hybrid_ciphertext_size(k_) : cb200_mlkem_ciphertext_size(k_);
   }
-  size_t SharedKeySize() const { return kind_ == HYBRID ? 64 : 32; }
+  size_t SharedKeySize() const { return kind_ == HYBRID ? cb200_hybrid_shared_key_size(k_) : 32; }
   size_t PrivateKeySize() const {
     return kind_ == XWING ? 32 : kind_ == HYBRID ? cb200_hybrid_private_key_size(k_) : cb200_mlkem_private_key_size(k_);
   }
   size_t PublicKeySize() const {
     return kind_ == XWING ? 1216 : kind_ == HYBRID ? cb200_hybrid_public_key_size(k_) : cb200_mlkem_public_key_size(k_);
   }
-  size_t SeedSize() const { return kind_ == XWING ? 32 : 64; }
-  size_t EncapsulationSeedSize() const { return kind_ == XWING ? 64 : 32; }
+  size_t SeedSize() const { return kind_ == XWING ? 32 : kind_ == HYBRID ? cb200_hybrid_seed_size(k_) : 64; }
+  size_t EncapsulationSeedSize() const {
+    return kind_ == XWING ? 64 : kind_ == HYBRID ? cb200_hybrid_encapsulation_seed_size(k_) : 32;
+  }
 
   std::pair<PublicKey, PrivateKey> DeriveKeyPair(const Bytes& seed) const {  // kyber.go:337-346
     if (seed.size() != SeedSize()) throw std::logic_error("kem: invalid seed size");  // Go panics here
@@ -232,13 +235,15 @@ inline PublicKey PrivateKey::Public() const {
     return PublicKey(s, std::move(pk));
   }
   if (s->kind() == Scheme::HYBRID) {  // {first.Public(), second.Public()} (hybrid.go:151-153, xkem.go:68-84)
-    const size_t dk = s->PrivateKeySize() - 32, ek = s->PublicKeySize() - 32, kk = (dk - 96) / 768;
+    const size_t xs = s->SharedKeySize() - 32;  // size of the X half: 32 (X25519) or 56 (X448)
+    const size_t dk = s->PrivateKeySize() - xs, ek = s->PublicKeySize() - xs, kk = (dk - 96) / 768;
     const bool x_first = s->k() != CB200_HYBRID_X25519MLKEM768;
     Bytes pk(s->PublicKeySize());
-    const uint8_t* skm = packed_.data() + (x_first ? 32 : 0);
+    const uint8_t* skm = packed_.data() + (x_first ? xs : 0);
     const uint8_t* skx = packed_.data() + (x_first ? 0 : dk);
-    std::copy(skm + 384 * kk, skm + 384 * kk + ek, pk.begin() + (x_first ? 32 : 0));
-    if (cb200_x25519(skx, nullptr, pk.data() + (x_first ? 0 : ek), nullptr, 1)) throw Error(cb200_last_error());
+    std::copy(skm + 384 * kk, skm + 384 * kk + ek, pk.begin() + (x_first ? xs : 0));
+    uint8_t* pkx = pk.data() + (x_first ? 0 : ek);
+    if ((xs == 56 ? cb200_x448 : cb200_x25519)(skx, nullptr, pkx, nullptr, 1)) throw Error(cb200_last_error());
     return PublicKey(s, std::move(pk));
   }
   const int k = s->k();
@@ -254,8 +259,10 @@ inline const std::vector<const Scheme*>& All() {  // kem/schemes/schemes.go:75
   static const Scheme k512("Kyber512", 2, true), k768("Kyber768", 3, true), k1024("Kyber1024", 4, true);
   static const Scheme xw("X-Wing", Scheme::XWING, 0), xm("X25519MLKEM768", Scheme::HYBRID, CB200_HYBRID_X25519MLKEM768),
       k7x("Kyber768-X25519", Scheme::HYBRID, CB200_HYBRID_KYBER768_X25519),
-      k5x("Kyber512-X25519", Scheme::HYBRID, CB200_HYBRID_KYBER512_X25519);
-  static const std::vector<const Scheme*> all = {&s512, &s768, &s1024, &k512, &k768, &k1024, &k5x, &k7x, &xm, &xw};
+      k5x("Kyber512-X25519", Scheme::HYBRID, CB200_HYBRID_KYBER512_X25519),
+      k7x4("Kyber768-X448", Scheme::HYBRID, CB200_HYBRID_KYBER768_X448),
+      k10x4("Kyber1024-X448", Scheme::HYBRID, CB200_HYBRID_KYBER1024_X448);
+  static const std::vector<const Scheme*> all = {&s512, &s768, &s1024, &k512, &k768, &k1024, &k5x, &k7x, &k7x4, &k10x4, &xm, &xw};
   return all;
 }
 inline const Scheme* ByName(const std::string& name) {  // kem/schemes/schemes.go:70 (nullptr = no such scheme)

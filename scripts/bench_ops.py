@@ -84,6 +84,30 @@ for name in ("X-Wing", "X25519MLKEM768"):
                              "roundtrip_ok": bool(torch.equal(ss, sch.DecapsulateBatch(sk, ct)))}
     del seeds, es, pk, sk, ct, ss
     torch.cuda.empty_cache()
+# X448 and the X448 hybrids, device-resident at 2^18
+from circl_b200 import x448  # noqa: E402
+k56 = torch.randint(0, 256, (n, 56), generator=g, device="cuda", dtype=torch.uint8)
+t = timed(lambda: x448.x448_keygen(k56), steps=3)
+pub = x448.x448_keygen(k56)
+res["X448 KeyGen"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+t = timed(lambda: x448.x448_shared(k56, pub), steps=3)
+res["X448 Shared"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+del k56, pub
+for sch in x448.All():
+    name = sch.Name()
+    seeds = torch.randint(0, 256, (n, sch.SeedSize()), generator=g, device="cuda", dtype=torch.uint8)
+    es = torch.randint(0, 256, (n, sch.EncapsulationSeedSize()), generator=g, device="cuda", dtype=torch.uint8)
+    t = timed(lambda: sch.DeriveKeyPairBatch(seeds), steps=3)
+    pk, sk = sch.DeriveKeyPairBatch(seeds)
+    res[f"{name} keygen"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+    t = timed(lambda: sch.EncapsulateBatch(pk, es), steps=3)
+    ct, ss = sch.EncapsulateBatch(pk, es)
+    res[f"{name} encaps"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+    t = timed(lambda: sch.DecapsulateBatch(sk, ct), steps=3)
+    res[f"{name} decaps"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3),
+                             "roundtrip_ok": bool(torch.equal(ss, sch.DecapsulateBatch(sk, ct)))}
+    del seeds, es, pk, sk, ct, ss
+    torch.cuda.empty_cache()
 k768 = mlkem.ByName("Kyber768")
 seeds = torch.randint(0, 256, (n, 64), generator=g, device="cuda", dtype=torch.uint8)
 ms = torch.randint(0, 256, (n, 32), generator=g, device="cuda", dtype=torch.uint8)
