@@ -98,6 +98,22 @@ SYMBOLS = {
     "cb200_mldsa65_public_key_size": (C.c_size_t, []),
     "cb200_mldsa65_signature_size": (C.c_size_t, []),
     "cb200_mldsa65_private_key_size": (C.c_size_t, []),
+    "cb200_ed25519_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_ed25519_sign": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_ed25519_verify": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_ed25519_public_key_size": (C.c_size_t, []),
+    "cb200_ed25519_private_key_size": (C.c_size_t, []),
+    "cb200_ed25519_signature_size": (C.c_size_t, []),
+    "cb200_ed25519_seed_size": (C.c_size_t, []),
+    "cb200_eddilithium2_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_eddilithium2_sign": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_size_t]),
+    "cb200_eddilithium2_verify": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_size_t]),
+    "cb200_eddilithium2_public_key_size": (C.c_size_t, []),
+    "cb200_eddilithium2_private_key_size": (C.c_size_t, []),
+    "cb200_eddilithium2_signature_size": (C.c_size_t, []),
+    "cb200_eddilithium2_seed_size": (C.c_size_t, []),
     "cb200_mlkem_decaps": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_mlkem_keygen": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_mlkem_private_key_size": (C.c_size_t, [C.c_int]),

@@ -1,0 +1,472 @@
+// sign/ed25519 and sign/eddilithium2, batched on the device:
+//   sign/ed25519/ed25519.go:206-223,290-294,329-368   NewKeyFromSeed / Sign / Verify   -> ed25519_*_kernel (thread per op)
+//   sign/eddilithium2/eddilithium.go:59-115           Ed25519-Dilithium2               -> the round-3 Dilithium2 flows of
+//                                                                                         mldsa.cu (mldsa_internal.h) + the
+//                                                                                         Ed25519 kernels
+// The curve code is ed25519.cuh; [k]B uses the fixed-base table that cb200_init builds for X25519 KeyGen.
+#include <algorithm>
+#include <cstring>
+#include <functional>
+#include <initializer_list>
+#include <vector>
+
+#include "../../include/circl_b200.h"
+#include "common.cuh"
+#include "context.h"
+#include "ed25519.cuh"
+#include "flow_internal.h"
+#include "mldsa_internal.h"
+
+namespace cb200 {
+namespace eddsa {
+
+template <int N>
+__device__ __forceinline__ void ldw(uint32_t (&w)[N], const uint8_t* p) {
+#pragma unroll
+  for (int i = 0; i < N; i++) w[i] = reinterpret_cast<const uint32_t*>(p)[i];
+}
+template <int N>
+__device__ __forceinline__ void stw(uint8_t* p, const uint32_t (&w)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; i++) reinterpret_cast<uint32_t*>(p)[i] = w[i];
+}
+
+// pk[i] = A, and sk[i] = seed || A when sk is not null.  Rows are 4-byte aligned.
+__global__ void __launch_bounds__(128) ed25519_keygen_kernel(const uint8_t* __restrict__ seeds, size_t s_stride,
+                                                             uint8_t* __restrict__ pk, size_t pk_stride,
+                                                             uint8_t* __restrict__ sk, const int32_t* __restrict__ table,
+                                                             size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint32_t seed[8], A[8];
+  ldw(seed, seeds + i * s_stride);
+  ed25519::public_from_seed(A, seed, table);
+  stw(pk + i * pk_stride, A);
+  if (sk) {
+    stw(sk + 64 * i, seed);
+    stw(sk + 64 * i + 32, A);
+  }
+}
+
+// sig[i] = Sign(sk[i], msg i).  sk rows hold seed || A (ed25519.PrivateKey); with derive_a they hold the seed only
+// and A is recomputed from it (eddilithium2's PrivateKey.Unpack).  sk_stride 0: one key for the batch.
+__global__ void __launch_bounds__(128) ed25519_sign_kernel(const uint8_t* __restrict__ sk, size_t sk_stride, int derive_a,
+                                                           const uint8_t* __restrict__ msgs,
+                                                           const uint64_t* __restrict__ msg_off, uint8_t* __restrict__ sig,
+                                                           size_t sig_stride, const int32_t* __restrict__ table, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint8_t* row = sk + i * sk_stride;
+  uint32_t seed[8], A[8], R[8], S[8];
+  ldw(seed, row);
+  if (derive_a)
+    ed25519::public_from_seed(A, seed, table);
+  else
+    ldw(A, row + 32);
+  const uint64_t m0 = msg_off[i], m1 = msg_off[i + 1];
+  ed25519::sign(R, S, seed, A, msgs + m0, m1 - m0, table);
+  stw(sig + i * sig_stride, R);
+  stw(sig + i * sig_stride + 32, S);
+}
+
+// ok[i] = Verify(pk[i], msg i, sig[i]); with and_ok the result is ANDed into ok[i] (the composite's other half)
+__global__ void __launch_bounds__(128) ed25519_verify_kernel(const uint8_t* __restrict__ pk, size_t pk_stride,
+                                                             const uint8_t* __restrict__ msgs,
+                                                             const uint64_t* __restrict__ msg_off,
+                                                             const uint8_t* __restrict__ sig, size_t sig_stride,
+                                                             uint8_t* __restrict__ ok, int and_ok,
+                                                             const int32_t* __restrict__ table, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint32_t A[8], R[8], S[8];
+  ldw(A, pk + i * pk_stride);
+  ldw(R, sig + i * sig_stride);
+  ldw(S, sig + i * sig_stride + 32);
+  const uint64_t m0 = msg_off[i], m1 = msg_off[i + 1];
+  const bool good = ed25519::verify(A, msgs + m0, m1 - m0, R, S, table);
+  if (and_ok)
+    ok[i] = (ok[i] && good) ? 1 : 0;
+  else
+    ok[i] = good ? 1 : 0;
+}
+
+// ------------------------------------------------------------------ host side
+static inline unsigned blocks(size_t units, size_t per) { return (unsigned)((units + per - 1) / per); }
+static const int32_t* base_table() { return (const int32_t*)ctx().x25519_table; }
+
+static int ed_keygen_dev(const uint8_t* seeds, size_t s_stride, uint8_t* pk, size_t pk_stride, uint8_t* sk, size_t n,
+                         cudaStream_t st) {
+  {
+    KernelScope ks(KID_ED25519, st);
+    ed25519_keygen_kernel<<<blocks(n, 128), 128, 0, st>>>(seeds, s_stride, pk, pk_stride, sk, base_table(), n);
+  }
+  CB200_CUDA(cudaGetLastError());
+  return 0;
+}
+static int ed_sign_dev(const uint8_t* sk, size_t sk_stride, int derive_a, const uint8_t* msgs, const uint64_t* msg_off,
+                       uint8_t* sig, size_t sig_stride, size_t n, cudaStream_t st) {
+  {
+    KernelScope ks(KID_ED25519, st);
+    ed25519_sign_kernel<<<blocks(n, 128), 128, 0, st>>>(sk, sk_stride, derive_a, msgs, msg_off, sig, sig_stride, base_table(),
+                                                        n);
+  }
+  CB200_CUDA(cudaGetLastError());
+  return 0;
+}
+static int ed_verify_dev(const uint8_t* pk, size_t pk_stride, const uint8_t* msgs, const uint64_t* msg_off,
+                         const uint8_t* sig, size_t sig_stride, uint8_t* ok, int and_ok, size_t n, cudaStream_t st) {
+  {
+    KernelScope ks(KID_ED25519, st);
+    ed25519_verify_kernel<<<blocks(n, 128), 128, 0, st>>>(pk, pk_stride, msgs, msg_off, sig, sig_stride, ok, and_ok,
+                                                          base_table(), n);
+  }
+  CB200_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---- Ed25519-Dilithium2 (eddilithium.go): pk = Dilithium2 pk (1312) || A (32), sk = Dilithium2 sk (2528) || Ed25519
+// seed (32), sig = Dilithium2 sig (2420) || Ed25519 sig (64).  The Dilithium2 flows read and write contiguous rows,
+// so the parts that do not sit at a row start with the flows' own stride go through aligned scratch in the level-1
+// work area (level 0 belongs to those flows) and are moved with 2D copies on the call's stream.
+constexpr size_t kDPk = 1312, kDSk = 2528, kDSig = 2420;
+constexpr size_t kEdPk = kDPk + 32, kEdSk = kDSk + 32, kEdSig = kDSig + 64;
+
+static int copy2d(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t n, cudaStream_t st) {
+  CB200_CUDA(cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, n, cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
+// NewKeyFromSeed (eddilithium.go:59-78): SHAKE256(seed) -> Dilithium2 seed (32) || Ed25519 seed (32)
+static int edd2_keygen_dev(const uint8_t* seeds, uint8_t* pk, uint8_t* sk, size_t n, cudaStream_t st, int slot) {
+  Arena A;
+  int rc = arena(slot, n * (64 + 32 + kDPk + kDSk) + 4096, &A);
+  if (rc) return rc;
+  uint8_t *ex = A.take(n * 64), *dseed = A.take(n * 32), *dpk = A.take(n * kDPk), *dsk = A.take(n * kDSk);
+  hybrid::shake256_rows(seeds, 32, 32, ex, 64, 64, n, st);
+  if ((rc = copy2d(dseed, 32, ex, 64, 32, n, st))) return rc;
+  if ((rc = copy2d(sk + kDSk, kEdSk, ex + 32, 64, 32, n, st))) return rc;
+  rc = mldsa::dev_keygen(2, dseed, dpk, dsk, n, st, slot);
+  if (rc) return rc;
+  if ((rc = copy2d(pk, kEdPk, dpk, kDPk, kDPk, n, st))) return rc;
+  if ((rc = copy2d(sk, kEdSk, dsk, kDSk, kDSk, n, st))) return rc;
+  return ed_keygen_dev(ex + 32, 64, pk + kDPk, kEdPk, nullptr, n, st);
+}
+// SignTo (eddilithium.go:82-93): the Dilithium2 half reads the key rows in place (their stride is a multiple of 16)
+static int edd2_sign_dev(const uint8_t* sk, size_t sk_stride, const uint8_t* msgs, const uint64_t* msg_off, uint8_t* sig,
+                         uint8_t* status, size_t n, cudaStream_t st, int slot) {
+  Arena A;
+  int rc = arena(slot, n * (kDSig + 1) + 4096, &A);
+  if (rc) return rc;
+  uint8_t* dsig = A.take(n * kDSig);
+  if (!status) status = A.take(n);  // the flow always writes per-op status bytes
+  rc = mldsa::dev_sign(2, sk, sk_stride, msgs, msg_off, dsig, status, n, st, slot, (volatile uint32_t*)wset(slot).pin);
+  if (rc) return rc;
+  if ((rc = copy2d(sig, kEdSig, dsig, kDSig, kDSig, n, st))) return rc;
+  return ed_sign_dev(sk + kDSk, sk_stride, 1, msgs, msg_off, sig + kDSig, kEdSig, n, st);
+}
+// Verify (eddilithium.go:96-115): both halves must hold
+static int edd2_verify_dev(const uint8_t* pk, size_t pk_stride, const uint8_t* msgs, const uint64_t* msg_off,
+                           const uint8_t* sig, uint8_t* ok, size_t n, cudaStream_t st, int slot) {
+  Arena A;
+  int rc = arena(slot, n * kDSig + 4096, &A);
+  if (rc) return rc;
+  uint8_t* dsig = A.take(n * kDSig);
+  if ((rc = copy2d(dsig, kDSig, sig, kEdSig, kDSig, n, st))) return rc;
+  rc = mldsa::dev_verify(2, pk, pk_stride, msgs, msg_off, dsig, ok, n, st, slot);
+  if (rc) return rc;
+  return ed_verify_dev(pk + kDPk, pk_stride, msgs, msg_off, sig + kDSig, kEdSig, ok, 1, n, st);
+}
+
+// ---- host-pointer calls with variable-length messages: one contiguous range per GPU, staged in chunks through
+// scratch slot 0 (flows run with slot 0).  rows[j]: fixed-width per-op buffers (shared = one row for the batch).
+struct Row {
+  const uint8_t* in;
+  uint8_t* out;
+  size_t unit;
+  size_t host_stride;  // 0 = dense
+  bool shared;
+};
+using MsgBody = std::function<int(uint8_t** d, const uint8_t* msgs, const uint64_t* off, size_t cnt, cudaStream_t st)>;
+static int run_msgs(size_t n, const std::vector<Row>& rows, const uint8_t* msgs, const uint64_t* msg_off, const MsgBody& body) {
+  return for_each_shard(n, 1u << 12, [&](size_t f0, size_t sn) -> int {
+    Dev& c = ctx();
+    cudaStream_t st = c.pipe[0];
+    constexpr size_t kChunk = 1u << 15;
+    std::vector<uint64_t> ro;
+    for (size_t first = f0; first < f0 + sn; first += kChunk) {
+      const size_t cnt = std::min(kChunk, f0 + sn - first);
+      const uint64_t m0 = msg_off[first];
+      const size_t mb = (size_t)(msg_off[first + cnt] - m0);
+      size_t off = 0;
+      auto take = [&](size_t bytes) {
+        size_t o = off;
+        off += (bytes + 255) & ~(size_t)255;
+        return o;
+      };
+      std::vector<size_t> ro_off(rows.size());
+      for (size_t j = 0; j < rows.size(); j++) ro_off[j] = take(rows[j].shared ? rows[j].unit : cnt * rows[j].unit);
+      const size_t oMsg = take(mb + 8), oOff = take((cnt + 1) * 8);
+      int rc = ensure_scratch(0, off);
+      if (rc) return rc;
+      char* d = (char*)c.scratch[0];
+      std::vector<uint8_t*> dp(rows.size());
+      for (size_t j = 0; j < rows.size(); j++) {
+        const Row& r = rows[j];
+        dp[j] = (uint8_t*)d + ro_off[j];
+        if (!r.in) continue;
+        const size_t hs = r.host_stride ? r.host_stride : r.unit;
+        if (r.shared)
+          CB200_CUDA(cudaMemcpyAsync(dp[j], r.in, r.unit, cudaMemcpyHostToDevice, st));
+        else if (hs == r.unit)
+          CB200_CUDA(cudaMemcpyAsync(dp[j], r.in + first * hs, cnt * r.unit, cudaMemcpyHostToDevice, st));
+        else
+          CB200_CUDA(cudaMemcpy2DAsync(dp[j], r.unit, r.in + first * hs, hs, r.unit, cnt, cudaMemcpyHostToDevice, st));
+      }
+      if (mb) CB200_CUDA(cudaMemcpyAsync(d + oMsg, msgs + m0, mb, cudaMemcpyHostToDevice, st));
+      ro.resize(cnt + 1);
+      for (size_t i = 0; i <= cnt; i++) ro[i] = msg_off[first + i] - m0;
+      CB200_CUDA(cudaMemcpyAsync(d + oOff, ro.data(), (cnt + 1) * 8, cudaMemcpyHostToDevice, st));
+      rc = body(dp.data(), (const uint8_t*)d + oMsg, (const uint64_t*)(d + oOff), cnt, st);
+      if (rc) return rc;
+      for (size_t j = 0; j < rows.size(); j++)
+        if (rows[j].out) CB200_CUDA(cudaMemcpyAsync(rows[j].out + first * rows[j].unit, dp[j], cnt * rows[j].unit,
+                                                    cudaMemcpyDeviceToHost, st));
+      CB200_CUDA(cudaStreamSynchronize(st));  // `ro` and the scratch are reused by the next chunk
+    }
+    return 0;
+  });
+}
+
+static bool same_side(std::initializer_list<const void*> ps, bool* dev) {
+  bool first = true;
+  for (const void* p : ps) {
+    if (!p) continue;
+    const bool d = is_device_ptr(p);
+    if (first) {
+      *dev = d;
+      first = false;
+    } else if (d != *dev) {
+      return false;
+    }
+  }
+  return true;
+}
+static bool aligned(std::initializer_list<const void*> ps, std::initializer_list<size_t> strides, uintptr_t a) {
+  uintptr_t acc = 0;
+  for (const void* p : ps) acc |= (uintptr_t)p;
+  for (size_t v : strides) acc |= v;
+  return (acc & (a - 1)) == 0;
+}
+
+}  // namespace eddsa
+}  // namespace cb200
+
+using namespace cb200;
+using namespace cb200::eddsa;
+
+extern "C" {
+
+size_t cb200_ed25519_public_key_size(void) { return 32; }
+size_t cb200_ed25519_private_key_size(void) { return 64; }
+size_t cb200_ed25519_signature_size(void) { return 64; }
+size_t cb200_ed25519_seed_size(void) { return 32; }
+size_t cb200_eddilithium2_public_key_size(void) { return kEdPk; }
+size_t cb200_eddilithium2_private_key_size(void) { return kEdSk; }
+size_t cb200_eddilithium2_signature_size(void) { return kEdSig; }
+size_t cb200_eddilithium2_seed_size(void) { return 32; }
+
+int cb200_ed25519_keygen(const uint8_t* seeds, uint8_t* pk, uint8_t* sk, size_t n) {
+  int rc = require_ready();
+  if (rc) return rc;
+  if (!seeds || !pk) {
+    set_error("cb200_ed25519_keygen: null pointer");
+    return CB200_ERR_ARG;
+  }
+  if (n == 0) return 0;
+  bool dev = false;
+  if (!same_side({seeds, pk, sk}, &dev)) {
+    set_error("cb200_ed25519_keygen: mixed host/device pointers");
+    return CB200_ERR_ARG;
+  }
+  if (dev) {
+    if (!aligned({seeds, pk, sk}, {}, 4)) {
+      set_error("cb200_ed25519_keygen: device buffers must be 4-byte aligned");
+      return CB200_ERR_ARG;
+    }
+    DeviceCall call(pk);
+    if (call.rc) return call.rc;
+    return ed_keygen_dev(seeds, 32, pk, 32, sk, n, call.st);
+  }
+  std::vector<Buf> bufs = {Buf{seeds, nullptr, 32, false, 0}, Buf{nullptr, pk, 32, false, 0}};
+  if (sk) bufs.push_back(Buf{nullptr, sk, 64, false, 0});
+  return run_host(bufs, n, 1u << 16, 1u << 13, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
+    return ed_keygen_dev((const uint8_t*)d[0], 32, (uint8_t*)d[1], 32, sk ? (uint8_t*)d[2] : nullptr, cnt, st);
+  });
+}
+
+int cb200_ed25519_sign(const uint8_t* sk, size_t sk_stride, const uint8_t* msgs, const uint64_t* msg_off, uint8_t* sig,
+                       size_t n) {
+  int rc = require_ready();
+  if (rc) return rc;
+  if (!sk || !msgs || !msg_off || !sig || (sk_stride != 0 && sk_stride < 64)) {
+    set_error("cb200_ed25519_sign: bad argument");
+    return CB200_ERR_ARG;
+  }
+  if (n == 0) return 0;
+  bool dev = false;
+  if (!same_side({sk, msgs, msg_off, sig}, &dev)) {
+    set_error("cb200_ed25519_sign: mixed host/device pointers");
+    return CB200_ERR_ARG;
+  }
+  if (dev) {
+    if (!aligned({sk, sig}, {sk_stride}, 4) || !aligned({msg_off}, {}, 8)) {
+      set_error("cb200_ed25519_sign: device sk, sk_stride and sig must be 4-byte aligned, msg_off 8-byte aligned");
+      return CB200_ERR_ARG;
+    }
+    DeviceCall call(sig);
+    if (call.rc) return call.rc;
+    return ed_sign_dev(sk, sk_stride, 0, msgs, msg_off, sig, 64, n, call.st);
+  }
+  std::vector<Row> rows = {Row{sk, nullptr, 64, sk_stride, sk_stride == 0}, Row{nullptr, sig, 64, 0, false}};
+  return run_msgs(n, rows, msgs, msg_off, [&](uint8_t** d, const uint8_t* m, const uint64_t* o, size_t cnt, cudaStream_t st) {
+    return ed_sign_dev(d[0], sk_stride ? 64 : 0, 0, m, o, d[1], 64, cnt, st);
+  });
+}
+
+int cb200_ed25519_verify(const uint8_t* pk, size_t pk_stride, const uint8_t* msgs, const uint64_t* msg_off,
+                         const uint8_t* sig, uint8_t* ok, size_t n) {
+  int rc = require_ready();
+  if (rc) return rc;
+  if (!pk || !msgs || !msg_off || !sig || !ok || (pk_stride != 0 && pk_stride < 32)) {
+    set_error("cb200_ed25519_verify: bad argument");
+    return CB200_ERR_ARG;
+  }
+  if (n == 0) return 0;
+  bool dev = false;
+  if (!same_side({pk, msgs, msg_off, sig, ok}, &dev)) {
+    set_error("cb200_ed25519_verify: mixed host/device pointers");
+    return CB200_ERR_ARG;
+  }
+  if (dev) {
+    if (!aligned({pk, sig}, {pk_stride}, 4) || !aligned({msg_off}, {}, 8)) {
+      set_error("cb200_ed25519_verify: device pk, pk_stride and sig must be 4-byte aligned, msg_off 8-byte aligned");
+      return CB200_ERR_ARG;
+    }
+    DeviceCall call(ok);
+    if (call.rc) return call.rc;
+    return ed_verify_dev(pk, pk_stride, msgs, msg_off, sig, 64, ok, 0, n, call.st);
+  }
+  std::vector<Row> rows = {Row{pk, nullptr, 32, pk_stride, pk_stride == 0}, Row{sig, nullptr, 64, 0, false},
+                           Row{nullptr, ok, 1, 0, false}};
+  return run_msgs(n, rows, msgs, msg_off, [&](uint8_t** d, const uint8_t* m, const uint64_t* o, size_t cnt, cudaStream_t st) {
+    return ed_verify_dev(d[0], pk_stride ? 32 : 0, m, o, d[1], 64, d[2], 0, cnt, st);
+  });
+}
+
+int cb200_eddilithium2_keygen(const uint8_t* seeds, uint8_t* pk, uint8_t* sk, size_t n) {
+  int rc = require_ready();
+  if (rc) return rc;
+  if (!seeds || !pk || !sk) {
+    set_error("cb200_eddilithium2_keygen: null pointer");
+    return CB200_ERR_ARG;
+  }
+  if (n == 0) return 0;
+  bool dev = false;
+  if (!same_side({seeds, pk, sk}, &dev)) {
+    set_error("cb200_eddilithium2_keygen: mixed host/device pointers");
+    return CB200_ERR_ARG;
+  }
+  if (dev) {
+    if (!aligned({seeds, pk, sk}, {}, 16)) {
+      set_error("cb200_eddilithium2_keygen: device buffers must be 16-byte aligned");
+      return CB200_ERR_ARG;
+    }
+    DeviceCall call(pk);
+    if (call.rc) return call.rc;
+    return edd2_keygen_dev(seeds, pk, sk, n, call.st, kDevSlot);
+  }
+  std::vector<Buf> bufs = {Buf{seeds, nullptr, 32, false, 0}, Buf{nullptr, pk, kEdPk, false, 0},
+                           Buf{nullptr, sk, kEdSk, false, 0}};
+  return run_host(bufs, n, 1u << 14, 1u << 12, [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
+    return edd2_keygen_dev((const uint8_t*)d[0], (uint8_t*)d[1], (uint8_t*)d[2], cnt, st, slot);
+  });
+}
+
+int cb200_eddilithium2_sign(const uint8_t* sk, size_t sk_stride, const uint8_t* msgs, const uint64_t* msg_off, uint8_t* sig,
+                            uint8_t* status, size_t n) {
+  int rc = require_ready();
+  if (rc) return rc;
+  if (!sk || !msgs || !msg_off || !sig || (sk_stride != 0 && sk_stride < kEdSk)) {
+    set_error("cb200_eddilithium2_sign: bad argument");
+    return CB200_ERR_ARG;
+  }
+  if (n == 0) return 0;
+  bool dev = false;
+  if (!same_side({sk, msgs, msg_off, sig, status}, &dev)) {
+    set_error("cb200_eddilithium2_sign: mixed host/device pointers");
+    return CB200_ERR_ARG;
+  }
+  if (dev) {
+    if (!aligned({sk, msg_off}, {sk_stride}, 16) || !aligned({sig}, {}, 4)) {
+      set_error("cb200_eddilithium2_sign: device sk, sk_stride and msg_off must be 16-byte aligned, sig 4-byte aligned");
+      return CB200_ERR_ARG;
+    }
+    if (n >= (1u << 24)) {  // the limit of the Dilithium2 signing flow
+      set_error("cb200_eddilithium2_sign: a device-pointer batch is limited to 2^24 - 1 signatures per call (got %zu)", n);
+      return CB200_ERR_ARG;
+    }
+    DeviceCall call(sig);
+    if (call.rc) return call.rc;
+    return edd2_sign_dev(sk, sk_stride, msgs, msg_off, sig, status, n, call.st, kDevSlot);
+  }
+  std::vector<uint8_t> own;
+  if (!status) {
+    own.resize(n);
+    status = own.data();
+  }
+  std::vector<Row> rows = {Row{sk, nullptr, kEdSk, sk_stride, sk_stride == 0}, Row{nullptr, sig, kEdSig, 0, false},
+                           Row{nullptr, status, 1, 0, false}};
+  rc = run_msgs(n, rows, msgs, msg_off, [&](uint8_t** d, const uint8_t* m, const uint64_t* o, size_t cnt, cudaStream_t st) {
+    return edd2_sign_dev(d[0], sk_stride ? kEdSk : 0, m, o, d[1], d[2], cnt, st, 0);
+  });
+  if (rc) return rc;
+  size_t bad = 0;
+  for (size_t i = 0; i < n; i++) bad += status[i] != 0;
+  if (bad) {
+    set_error("cb200_eddilithium2_sign: %zu of %zu signatures exhausted 576 attempts", bad, n);
+    return CB200_ERR_SIGN_ATTEMPTS;
+  }
+  return 0;
+}
+
+int cb200_eddilithium2_verify(const uint8_t* pk, size_t pk_stride, const uint8_t* msgs, const uint64_t* msg_off,
+                              const uint8_t* sig, uint8_t* ok, size_t n) {
+  int rc = require_ready();
+  if (rc) return rc;
+  if (!pk || !msgs || !msg_off || !sig || !ok || (pk_stride != 0 && pk_stride < kEdPk)) {
+    set_error("cb200_eddilithium2_verify: bad argument");
+    return CB200_ERR_ARG;
+  }
+  if (n == 0) return 0;
+  bool dev = false;
+  if (!same_side({pk, msgs, msg_off, sig, ok}, &dev)) {
+    set_error("cb200_eddilithium2_verify: mixed host/device pointers");
+    return CB200_ERR_ARG;
+  }
+  if (dev) {
+    if (!aligned({pk, msg_off}, {pk_stride}, 16) || !aligned({sig}, {}, 4)) {
+      set_error("cb200_eddilithium2_verify: device pk, pk_stride and msg_off must be 16-byte aligned, sig 4-byte aligned");
+      return CB200_ERR_ARG;
+    }
+    DeviceCall call(ok);
+    if (call.rc) return call.rc;
+    return edd2_verify_dev(pk, pk_stride, msgs, msg_off, sig, ok, n, call.st, kDevSlot);
+  }
+  std::vector<Row> rows = {Row{pk, nullptr, kEdPk, pk_stride, pk_stride == 0}, Row{sig, nullptr, kEdSig, 0, false},
+                           Row{nullptr, ok, 1, 0, false}};
+  return run_msgs(n, rows, msgs, msg_off, [&](uint8_t** d, const uint8_t* m, const uint64_t* o, size_t cnt, cudaStream_t st) {
+    return edd2_verify_dev(d[0], pk_stride ? kEdPk : 0, m, o, d[1], d[2], cnt, st, 0);
+  });
+}
+
+}  // extern "C"

@@ -14,6 +14,7 @@
 
 #include "../../include/circl_b200.h"
 #include "context.h"
+#include "flow_internal.h"
 #include "keccak.cuh"
 #include "mlkem_internal.h"
 #include "x25519.cuh"
@@ -192,23 +193,8 @@ static void shake_launch(const uint8_t* in, size_t is, int inlen, uint8_t* out, 
   KernelScope ks(KID_HYBRID_GLUE, st);
   shake_kernel<<<blocks(n, 128), 128, 0, st>>>(in, is, inlen, out, os, outlen, n);
 }
-
-struct Arena {  // bump allocator over the second-level work area of a slot
-  char* base = nullptr;
-  size_t off = 0;
-  uint8_t* take(size_t bytes) {
-    uint8_t* p = (uint8_t*)(base + off);
-    off += (bytes + 255) & ~(size_t)255;
-    return p;
-  }
-};
-static int arena(int slot, size_t bytes, Arena* a) {
-  void* p = nullptr;
-  int rc = ensure_work(kLevel1 + slot, bytes + 4096, &p);  // the level-1 areas belong to this file, level 0 to the lattice flows
-  if (rc) return rc;
-  a->base = (char*)p;
-  a->off = 0;
-  return 0;
+void shake256_rows(const uint8_t* in, size_t is, int inlen, uint8_t* out, size_t os, int outlen, size_t n, cudaStream_t st) {
+  shake_launch(in, is, inlen, out, os, outlen, n, st);
 }
 
 // ---- X-Wing (ML-KEM-768 + X25519): pk = ek || pk_X (1216), sk = seed (32), ct = ct_M || ct_X (1120)

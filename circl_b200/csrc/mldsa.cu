@@ -25,6 +25,7 @@
 #include "context.h"
 #include "dilithium.cuh"
 #include "keccak.cuh"
+#include "mldsa_internal.h"
 
 namespace cb200 {
 namespace mldsa {
@@ -2340,3 +2341,24 @@ int cb200_dil_derive_ball(int mode, uint32_t* polys, const uint8_t* seeds, size_
 }
 
 }  // extern "C"
+
+// device-level entry points for the composite signatures of eddsa.cu (mldsa_internal.h); defined after the C entry
+// points so that the flows are instantiated in the same order as before
+namespace cb200 {
+namespace mldsa {
+
+int dev_keygen(int mode, const uint8_t* seeds, uint8_t* pk, uint8_t* sk, size_t n, cudaStream_t st, int slot) {
+  return dispatch_keygen(mode, seeds, pk, sk, n, st, slot);
+}
+int dev_sign(int mode, const uint8_t* sk, size_t sk_stride, const uint8_t* msgs, const uint64_t* msg_off, uint8_t* sig,
+             uint8_t* status, size_t n, cudaStream_t st, int slot, volatile uint32_t* h_count) {
+  return dispatch_sign(mode, sk, sk_stride, msgs, msg_off, (const uint8_t*)nullptr, 0, (const uint8_t*)nullptr, sig, status, n,
+                       0, st, slot, (uint64_t*)nullptr, h_count);
+}
+int dev_verify(int mode, const uint8_t* pk, size_t pk_stride, const uint8_t* msgs, const uint64_t* msg_off,
+               const uint8_t* sig, uint8_t* ok, size_t n, cudaStream_t st, int slot) {
+  return dispatch_verify(mode, pk, pk_stride, msgs, msg_off, (const uint8_t*)nullptr, 0, sig, ok, n, 0, st, slot);
+}
+
+}  // namespace mldsa
+}  // namespace cb200

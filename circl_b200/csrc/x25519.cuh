@@ -405,13 +405,13 @@ inline void build_base_table(int32_t* table) {
   }
 }
 
-// out = u([clamp(k)] G) from the table (device pointer on the GPU, host pointer in the CPU test)
-CB200_XHD void scalarmult_base(uint32_t (&out)[8], const uint32_t (&kin)[8], const int32_t* __restrict__ table) {
+// h = [k] B in extended coordinates for k < 2^255 (the top digit then stays within 1..8), from the table (device
+// pointer on the GPU, host pointer in the CPU test).  The caller prepares the scalar: X25519 KeyGen clamps it, Ed25519
+// passes a clamped or a reduced one.
+CB200_XHD void ge_scalarmult_base(GeExt& h, const uint32_t (&kin)[8], const int32_t* __restrict__ table) {
   uint32_t k[8];
 #pragma unroll
   for (int i = 0; i < 8; i++) k[i] = kin[i];
-  k[0] &= 0xfffffff8u;
-  k[7] = (k[7] & 0x7fffffffu) | 0x40000000u;  // key.go:17-22
   // signed radix-16 digits: nibble i of k + 0x88...8 minus 8; the carry out of the top nibble stays in digit 63
   uint32_t carry = 0;
 #pragma unroll
@@ -428,7 +428,6 @@ CB200_XHD void scalarmult_base(uint32_t (&out)[8], const uint32_t (&kin)[8], con
     if (i == 63) e += 16 * (int)carry;
     return e;
   };
-  GeExt h;
   fe_set(h.X, 0);
   fe_set(h.Y, 1);
   fe_set(h.Z, 1);
@@ -480,6 +479,17 @@ CB200_XHD void scalarmult_base(uint32_t (&out)[8], const uint32_t (&kin)[8], con
 #pragma unroll 1
 #endif
   for (int i = 0; i < 64; i += 2) add_digit(i);
+}
+
+// out = u([clamp(k)] G) from the table
+CB200_XHD void scalarmult_base(uint32_t (&out)[8], const uint32_t (&kin)[8], const int32_t* __restrict__ table) {
+  uint32_t k[8];
+#pragma unroll
+  for (int i = 0; i < 8; i++) k[i] = kin[i];
+  k[0] &= 0xfffffff8u;
+  k[7] = (k[7] & 0x7fffffffu) | 0x40000000u;  // key.go:17-22
+  GeExt h;
+  ge_scalarmult_base(h, k, table);
   Fe num, den;
   fe_add(num, h.Z, h.Y);
   fe_sub(den, h.Z, h.Y);

@@ -205,6 +205,153 @@ func MLDSA65Sign(sk []byte, shared bool, msgs [][]byte, ctx, rnd, sig []byte) er
 	})
 }
 
+// packMsgs lays messages back to back with n+1 offsets and the 8 bytes of read padding the sign entry points need.
+func packMsgs(msgs [][]byte) ([]byte, []uint64) {
+	n := len(msgs)
+	off := make([]uint64, n+1)
+	total := 0
+	for i, m := range msgs {
+		off[i] = uint64(total)
+		total += len(m)
+	}
+	off[n] = uint64(total)
+	blob := make([]byte, total+8)
+	for i, m := range msgs {
+		copy(blob[off[i]:], m)
+	}
+	return blob, off
+}
+
+func u8(b []byte) *C.uint8_t { return (*C.uint8_t)(unsafe.Pointer(&b[0])) }
+
+// Ed25519KeyGen: ed25519.NewKeyFromSeed (sign/ed25519/ed25519.go:206-223) on n 32-byte seeds; pk receives n*32
+// bytes, sk n*64 (seed || public key).
+func Ed25519KeyGen(seeds, pk, sk []byte) error {
+	n := len(seeds) / 32
+	if len(seeds) != n*32 || len(pk) != n*32 || len(sk) != n*64 {
+		panic("cb200: seeds/pk/sk have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return call(func() C.int { return C.cb200_ed25519_keygen(u8(seeds), u8(pk), u8(sk), C.size_t(n)) })
+}
+
+// Ed25519SignBatch: ed25519.Sign (ed25519.go:290-294) on len(msgs) messages.  sk holds one 64-byte private key
+// (shared) or one per message; its public half is used as given.  sig receives len(msgs)*64 bytes.
+func Ed25519SignBatch(sk []byte, shared bool, msgs [][]byte, sig []byte) error {
+	n := len(msgs)
+	if (shared && len(sk) != 64) || (!shared && len(sk) != n*64) || len(sig) != n*64 {
+		panic("cb200: sk/sig have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	blob, off := packMsgs(msgs)
+	stride := C.size_t(64)
+	if shared {
+		stride = 0
+	}
+	return call(func() C.int {
+		return C.cb200_ed25519_sign(u8(sk), stride, u8(blob), (*C.uint64_t)(unsafe.Pointer(&off[0])), u8(sig), C.size_t(n))
+	})
+}
+
+// Ed25519VerifyBatch: ed25519.Verify (ed25519.go:329-368) on len(msgs) 64-byte signatures; pk holds one 32-byte public
+// key (shared) or one per message.  ok[i] is the reference's result.
+func Ed25519VerifyBatch(pk []byte, shared bool, msgs [][]byte, sig []byte, ok []bool) error {
+	n := len(msgs)
+	if (shared && len(pk) != 32) || (!shared && len(pk) != n*32) || len(sig) != n*64 || len(ok) != n {
+		panic("cb200: pk/sig/ok have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return verifyBatch(n, msgs, ok, func(blob []byte, off []uint64, res []byte) C.int {
+		stride := C.size_t(32)
+		if shared {
+			stride = 0
+		}
+		return C.cb200_ed25519_verify(u8(pk), stride, u8(blob), (*C.uint64_t)(unsafe.Pointer(&off[0])), u8(sig), u8(res),
+			C.size_t(n))
+	})
+}
+
+func verifyBatch(n int, msgs [][]byte, ok []bool, f func(blob []byte, off []uint64, res []byte) C.int) error {
+	blob, off := packMsgs(msgs)
+	res := make([]byte, n)
+	if err := call(func() C.int { return f(blob, off, res) }); err != nil {
+		return err
+	}
+	for i := range ok {
+		ok[i] = res[i] != 0
+	}
+	return nil
+}
+
+// Sizes of Ed25519-Dilithium2 (sign/eddilithium2/eddilithium.go:16-28).
+const (
+	EdDilithium2PublicKeySize  = 1344
+	EdDilithium2PrivateKeySize = 2560
+	EdDilithium2SignatureSize  = 2484
+)
+
+// EdDilithium2KeyGen: eddilithium2.NewKeyFromSeed (eddilithium.go:59-78) on n 32-byte seeds; pk and sk receive the
+// packed keys (n*1344 and n*2560 bytes).
+func EdDilithium2KeyGen(seeds, pk, sk []byte) error {
+	n := len(seeds) / 32
+	if len(seeds) != n*32 || len(pk) != n*EdDilithium2PublicKeySize || len(sk) != n*EdDilithium2PrivateKeySize {
+		panic("cb200: seeds/pk/sk have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return call(func() C.int { return C.cb200_eddilithium2_keygen(u8(seeds), u8(pk), u8(sk), C.size_t(n)) })
+}
+
+// EdDilithium2SignBatch: eddilithium2.SignTo (eddilithium.go:82-93) on len(msgs) messages with one packed key
+// (shared) or one per message; sig receives len(msgs)*2484 bytes.  An error is returned if a Dilithium2 half
+// exhausted its 576 attempts (the reference panics there).
+func EdDilithium2SignBatch(sk []byte, shared bool, msgs [][]byte, sig []byte) error {
+	n := len(msgs)
+	if (shared && len(sk) != EdDilithium2PrivateKeySize) || (!shared && len(sk) != n*EdDilithium2PrivateKeySize) ||
+		len(sig) != n*EdDilithium2SignatureSize {
+		panic("cb200: sk/sig have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	blob, off := packMsgs(msgs)
+	stride := C.size_t(EdDilithium2PrivateKeySize)
+	if shared {
+		stride = 0
+	}
+	return call(func() C.int {
+		return C.cb200_eddilithium2_sign(u8(sk), stride, u8(blob), (*C.uint64_t)(unsafe.Pointer(&off[0])), u8(sig), nil,
+			C.size_t(n))
+	})
+}
+
+// EdDilithium2VerifyBatch: eddilithium2.Verify (eddilithium.go:96-115): both halves must verify.
+func EdDilithium2VerifyBatch(pk []byte, shared bool, msgs [][]byte, sig []byte, ok []bool) error {
+	n := len(msgs)
+	if (shared && len(pk) != EdDilithium2PublicKeySize) || (!shared && len(pk) != n*EdDilithium2PublicKeySize) ||
+		len(sig) != n*EdDilithium2SignatureSize || len(ok) != n {
+		panic("cb200: pk/sig/ok have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return verifyBatch(n, msgs, ok, func(blob []byte, off []uint64, res []byte) C.int {
+		stride := C.size_t(EdDilithium2PublicKeySize)
+		if shared {
+			stride = 0
+		}
+		return C.cb200_eddilithium2_verify(u8(pk), stride, u8(blob), (*C.uint64_t)(unsafe.Pointer(&off[0])), u8(sig),
+			u8(res), C.size_t(n))
+	})
+}
+
 // Hybrid scheme identifiers of include/circl_b200.h (kem/hybrid/hybrid.go:34-93).
 const (
 	HybridX25519MLKEM768 = 0

@@ -277,6 +277,42 @@ size_t cb200_mldsa_public_key_size(int mode);
 size_t cb200_mldsa_private_key_size(int mode);
 size_t cb200_mldsa_signature_size(int mode);
 
+/* ---- Ed25519 (sign/ed25519, RFC 8032 pure Ed25519) ----
+ * keygen = NewKeyFromSeed (ed25519.go:206-223): seeds n x 32 -> pk n x 32, sk n x 64 (= seed || pk; may be NULL).
+ * sign = Sign (ed25519.go:290-294): sk rows of 64 bytes at sk + i*sk_stride (0 = one key for the batch); A is read
+ * from bytes 32..63 of the key as given, as the reference does; sig n x 64.
+ * verify = Verify (ed25519.go:329-368): ok[i] = 1 iff S < L, pk decodes and encode([S]B - [k]A) == R (cofactorless).
+ * Messages as in cb200_mldsa_sign (msgs back to back, n + 1 offsets, 8 bytes of read padding behind the last one).
+ * The kernels read messages in aligned 8-byte words: besides the padding, a device-pointer call may read the bytes of
+ * the 8-byte-aligned word that holds msgs[0] in front of it (their values are not used).
+ * Device pointers: seeds, pk, sk, sig and the strides 4-byte aligned, msg_off 8-byte aligned. */
+int cb200_ed25519_keygen(const uint8_t *seeds, uint8_t *pk, uint8_t *sk, size_t n);
+int cb200_ed25519_sign(const uint8_t *sk, size_t sk_stride, const uint8_t *msgs, const uint64_t *msg_off, uint8_t *sig,
+                       size_t n);
+int cb200_ed25519_verify(const uint8_t *pk, size_t pk_stride, const uint8_t *msgs, const uint64_t *msg_off,
+                         const uint8_t *sig, uint8_t *ok, size_t n);
+size_t cb200_ed25519_public_key_size(void);  /* 32 */
+size_t cb200_ed25519_private_key_size(void); /* 64 */
+size_t cb200_ed25519_signature_size(void);   /* 64 */
+size_t cb200_ed25519_seed_size(void);        /* 32 */
+
+/* ---- Ed25519-Dilithium2 (sign/eddilithium2): pk = Dilithium2 pk (1312) || Ed25519 pk (32) = 1344, sk = Dilithium2
+ * packed sk (2528) || Ed25519 seed (32) = 2560, sig = Dilithium2 sig (2420) || Ed25519 sig (64) = 2484, seed 32.
+ * keygen = NewKeyFromSeed (eddilithium.go:59-78, SHAKE256(seed) -> Dilithium2 seed || Ed25519 seed); sign = SignTo
+ * (:82-93; the Ed25519 public key is re-derived from the seed, as PrivateKey.Unpack does); verify = Verify (:96-115,
+ * both halves).  status (optional): 1 = Dilithium2's 576-attempt cap (CB200_ERR_SIGN_ATTEMPTS for host pointers).
+ * No context string (sign.ErrContextNotSupported).  Device pointers: seeds, pk, sk, their strides and msg_off 16-byte
+ * aligned; sig 4-byte aligned (its Ed25519 half starts at byte 2420). */
+int cb200_eddilithium2_keygen(const uint8_t *seeds, uint8_t *pk, uint8_t *sk, size_t n);
+int cb200_eddilithium2_sign(const uint8_t *sk, size_t sk_stride, const uint8_t *msgs, const uint64_t *msg_off, uint8_t *sig,
+                            uint8_t *status, size_t n);
+int cb200_eddilithium2_verify(const uint8_t *pk, size_t pk_stride, const uint8_t *msgs, const uint64_t *msg_off,
+                              const uint8_t *sig, uint8_t *ok, size_t n);
+size_t cb200_eddilithium2_public_key_size(void);  /* 1344 */
+size_t cb200_eddilithium2_private_key_size(void); /* 2560 */
+size_t cb200_eddilithium2_signature_size(void);   /* 2484 */
+size_t cb200_eddilithium2_seed_size(void);        /* 32 */
+
 /* ---- ML-DSA-65 ---- */
 /* sign.Scheme.Sign / SignTo    sign/mldsa/mldsa65/dilithium.go:282-303,56-84  ->
  * internal.SignTo (ML-DSA.Sign_internal)  sign/mldsa/mldsa65/internal/dilithium.go:340-470,

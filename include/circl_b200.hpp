@@ -309,20 +309,32 @@ class PrivateKey {
   Bytes packed_;
 };
 
-class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 44, 65, 87) and round-3 Dilithium2/3/5 (2, 3, 5)
+class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 44, 65, 87), round-3 Dilithium2/3/5 (2, 3, 5),
+                // Ed25519 (sign/ed25519/signapi.go) and Ed25519-Dilithium2 (sign/eddilithium2/signapi.go)
  public:
-  Scheme(std::string name, int mode) : name_(std::move(name)), mode_(mode) {}
+  enum Family { kMLDSA, kEd25519, kEdDilithium2 };
+  Scheme(std::string name, int mode, Family family = kMLDSA) : name_(std::move(name)), mode_(mode), family_(family) {}
   const std::string& Name() const { return name_; }
-  size_t PublicKeySize() const { return cb200_mldsa_public_key_size(mode_); }
-  size_t PrivateKeySize() const { return cb200_mldsa_private_key_size(mode_); }
-  size_t SignatureSize() const { return cb200_mldsa_signature_size(mode_); }
+  size_t PublicKeySize() const {
+    return family_ == kEd25519 ? cb200_ed25519_public_key_size()
+           : family_ == kEdDilithium2 ? cb200_eddilithium2_public_key_size() : cb200_mldsa_public_key_size(mode_);
+  }
+  size_t PrivateKeySize() const {
+    return family_ == kEd25519 ? cb200_ed25519_private_key_size()
+           : family_ == kEdDilithium2 ? cb200_eddilithium2_private_key_size() : cb200_mldsa_private_key_size(mode_);
+  }
+  size_t SignatureSize() const {
+    return family_ == kEd25519 ? cb200_ed25519_signature_size()
+           : family_ == kEdDilithium2 ? cb200_eddilithium2_signature_size() : cb200_mldsa_signature_size(mode_);
+  }
   size_t SeedSize() const { return 32; }
-  bool SupportsContext() const { return mode_ > 10; }  // round 3: sign.ErrContextNotSupported
+  // round 3, Ed25519 and Ed25519-Dilithium2: sign.ErrContextNotSupported
+  bool SupportsContext() const { return family_ == kMLDSA && mode_ > 10; }
 
-  std::pair<PublicKey, PrivateKey> DeriveKey(const Bytes& seed) const {  // dilithium.go:266-276
+  std::pair<PublicKey, PrivateKey> DeriveKey(const Bytes& seed) const {  // dilithium.go:266-276, ed25519 signapi.go
     if (seed.size() != SeedSize()) throw std::logic_error("sign: invalid seed size");  // Go panics here
-    Bytes pk(PublicKeySize()), sk(PrivateKeySize());
-    check(cb200_mldsa_keygen(mode_, seed.data(), pk.data(), sk.data(), 1));
+    Bytes pk, sk;
+    DeriveKeyBatch(seed, pk, sk);
     return {PublicKey(this, std::move(pk)), PrivateKey(this, std::move(sk))};
   }
   std::pair<PublicKey, PrivateKey> GenerateKey() const {
@@ -338,27 +350,34 @@ class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 4
     if (b.size() != PrivateKeySize()) throw ErrPrivKeySize();
     return PrivateKey(this, b);
   }
-  // deterministic signing, as sign.Scheme.Sign does (dilithium.go:282-303)
+  // PrivateKey.Public() of Ed25519 (ed25519.go: the second half of the private key).  The ML-DSA and composite
+  // private keys do not hold their public key; their Public() needs the seed (DeriveKey).
+  PublicKey Public(const PrivateKey& sk) const {
+    if (family_ != kEd25519) throw std::logic_error("sign: Public() from a packed private key is served for Ed25519 only");
+    const Bytes& b = sk.MarshalBinary();
+    return PublicKey(this, Bytes(b.begin() + 32, b.end()));
+  }
+  // deterministic signing, as sign.Scheme.Sign does (dilithium.go:282-303, ed25519 signapi.go)
   Bytes Sign(const PrivateKey& sk, const Bytes& msg, const SignatureOpts* opts = nullptr) const {
     const std::string ctx = opts ? opts->Context : std::string();
-    if (!ctx.empty() && !SupportsContext()) throw ErrContextNotSupported();
-    if (ctx.size() > 255) throw ErrContextTooLong();
-    Bytes sig(SignatureSize());
-    const uint64_t off[2] = {0, msg.size()};
-    Bytes padded(msg);
-    padded.resize(msg.size() + 8);
-    check(cb200_mldsa_sign(mode_, sk.MarshalBinary().data(), 0, padded.data(), off, (const uint8_t*)ctx.data(), ctx.size(), nullptr,
-                             sig.data(), nullptr, 1, 0, nullptr));
-    return sig;
+    Bytes sigs;
+    SignBatch(sk.MarshalBinary(), msg, {0, msg.size()}, ctx, sigs);
+    return sigs;
   }
   bool Verify(const PublicKey& pk, const Bytes& msg, const Bytes& sig, const SignatureOpts* opts = nullptr) const {
     const std::string ctx = opts ? opts->Context : std::string();
-    if (ctx.size() > 255 || sig.size() != SignatureSize()) return false;  // dilithium.go:116-118
+    if (!ctx.empty() && family_ != kMLDSA) throw ErrContextNotSupported();
+    if (ctx.size() > 255 || sig.size() != SignatureSize()) return false;  // dilithium.go:116-118, ed25519.go:330-334
     uint8_t ok = 0;
     const uint64_t off[2] = {0, msg.size()};
     Bytes padded(msg);
     padded.resize(msg.size() + 8);
-    check(cb200_mldsa_verify(mode_, pk.MarshalBinary().data(), 0, padded.data(), off, (const uint8_t*)ctx.data(), ctx.size(),
+    if (family_ == kEd25519)
+      check(cb200_ed25519_verify(pk.MarshalBinary().data(), 0, padded.data(), off, sig.data(), &ok, 1));
+    else if (family_ == kEdDilithium2)
+      check(cb200_eddilithium2_verify(pk.MarshalBinary().data(), 0, padded.data(), off, sig.data(), &ok, 1));
+    else
+      check(cb200_mldsa_verify(mode_, pk.MarshalBinary().data(), 0, padded.data(), off, (const uint8_t*)ctx.data(), ctx.size(),
                                sig.data(), &ok, 1, 0));
     return ok != 0;
   }
@@ -372,8 +391,14 @@ class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 4
     sigs.resize(n * SignatureSize());
     Bytes padded(msgs);
     padded.resize(msgs.size() + 8);
-    check(cb200_mldsa_sign(mode_, sks.data(), shared ? 0 : PrivateKeySize(), padded.data(), off.data(), (const uint8_t*)ctx.data(),
-                             ctx.size(), nullptr, sigs.data(), nullptr, n, 0, nullptr));
+    const size_t stride = shared ? 0 : PrivateKeySize();
+    if (family_ == kEd25519)
+      check(cb200_ed25519_sign(sks.data(), stride, padded.data(), off.data(), sigs.data(), n));
+    else if (family_ == kEdDilithium2)
+      check(cb200_eddilithium2_sign(sks.data(), stride, padded.data(), off.data(), sigs.data(), nullptr, n));
+    else
+      check(cb200_mldsa_sign(mode_, sks.data(), stride, padded.data(), off.data(), (const uint8_t*)ctx.data(), ctx.size(), nullptr,
+                             sigs.data(), nullptr, n, 0, nullptr));
   }
   // ok[i] = 1 where signature i verifies; pks: one key (shared) or n keys
   void VerifyBatch(const Bytes& pks, const Bytes& msgs, const std::vector<uint64_t>& off, const std::string& ctx,
@@ -386,15 +411,26 @@ class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 4
     if (ctx.size() > 255 || sigs.size() != n * SignatureSize()) return;  // dilithium.go:116-118: such signatures are invalid
     Bytes padded(msgs);
     padded.resize(msgs.size() + 8);
-    check(cb200_mldsa_verify(mode_, pks.data(), shared ? 0 : PublicKeySize(), padded.data(), off.data(), (const uint8_t*)ctx.data(),
-                               ctx.size(), sigs.data(), ok.data(), n, 0));
+    const size_t stride = shared ? 0 : PublicKeySize();
+    if (family_ == kEd25519)
+      check(cb200_ed25519_verify(pks.data(), stride, padded.data(), off.data(), sigs.data(), ok.data(), n));
+    else if (family_ == kEdDilithium2)
+      check(cb200_eddilithium2_verify(pks.data(), stride, padded.data(), off.data(), sigs.data(), ok.data(), n));
+    else
+      check(cb200_mldsa_verify(mode_, pks.data(), stride, padded.data(), off.data(), (const uint8_t*)ctx.data(), ctx.size(),
+                               sigs.data(), ok.data(), n, 0));
   }
   void DeriveKeyBatch(const Bytes& seeds, Bytes& pks, Bytes& sks) const {
     if (seeds.size() % SeedSize()) throw ErrSeedSize();
     const size_t n = seeds.size() / SeedSize();
     pks.resize(n * PublicKeySize());
     sks.resize(n * PrivateKeySize());
-    check(cb200_mldsa_keygen(mode_, seeds.data(), pks.data(), sks.data(), n));
+    if (family_ == kEd25519)
+      check(cb200_ed25519_keygen(seeds.data(), pks.data(), sks.data(), n));
+    else if (family_ == kEdDilithium2)
+      check(cb200_eddilithium2_keygen(seeds.data(), pks.data(), sks.data(), n));
+    else
+      check(cb200_mldsa_keygen(mode_, seeds.data(), pks.data(), sks.data(), n));
   }
 
  private:
@@ -405,12 +441,15 @@ class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 4
   }
   std::string name_;
   int mode_;
+  Family family_;
 };
 
+// in the order of sign/schemes/schemes.go:31-44 for the schemes served here
 inline const std::vector<const Scheme*>& All() {
+  static const Scheme e25519("Ed25519", 0, Scheme::kEd25519), ed2("Ed25519-Dilithium2", 2, Scheme::kEdDilithium2);
   static const Scheme s44("ML-DSA-44", 44), s65("ML-DSA-65", 65), s87("ML-DSA-87", 87);
   static const Scheme d2("Dilithium2", 2), d3("Dilithium3", 3), d5("Dilithium5", 5);
-  static const std::vector<const Scheme*> all = {&s44, &s65, &s87, &d2, &d3, &d5};
+  static const std::vector<const Scheme*> all = {&e25519, &ed2, &s44, &s65, &s87, &d2, &d3, &d5};
   return all;
 }
 inline const Scheme* ByName(const std::string& name) {  // sign/schemes/schemes.go:69 (nullptr = no such scheme)

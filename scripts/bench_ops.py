@@ -28,6 +28,66 @@ def timed(fn, steps=5, warm=3):
     return a.elapsed_time(b) / steps
 
 
+def eddsa_lines(res):
+    """Ed25519 and Ed25519-Dilithium2 through the C ABI, device-resident, 2^18 operations, per-op keys, 32-byte messages
+    (plus Ed25519 Verify on 1 KiB messages), with X25519 KeyGen / Shared of the same run for comparison."""
+    from circl_b200 import hybrid
+    from circl_b200._ffi import check, lib
+    L = lib()
+    check(L.cb200_set_stream(torch.cuda.current_stream().cuda_stream))
+    n = 1 << 18
+    g = torch.Generator(device="cuda").manual_seed(11)
+    k32 = torch.randint(0, 256, (n, 32), generator=g, device="cuda", dtype=torch.uint8)
+    t = timed(lambda: hybrid.x25519_keygen(k32), steps=3)
+    pub = hybrid.x25519_keygen(k32)
+    res["X25519 KeyGen"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+    t = timed(lambda: hybrid.x25519_shared(k32, pub), steps=3)
+    res["X25519 Shared"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+    # the same KeyGen through the C ABI into a preallocated buffer, as the Ed25519 lines below are timed
+    t = timed(lambda: check(L.cb200_x25519(k32.data_ptr(), None, pub.data_ptr(), None, n)), steps=3)
+    res["X25519 KeyGen (C ABI, preallocated output)"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+    for mlen in (32, 1024):
+        msg = torch.randint(0, 256, (n * mlen + 8,), generator=g, device="cuda", dtype=torch.uint8)
+        off = (torch.arange(n + 1, device="cuda", dtype=torch.int64) * mlen).contiguous()
+        pk = torch.empty((n, 32), dtype=torch.uint8, device="cuda")
+        sk = torch.empty((n, 64), dtype=torch.uint8, device="cuda")
+        sig = torch.empty((n, 64), dtype=torch.uint8, device="cuda")
+        ok = torch.zeros((n,), dtype=torch.uint8, device="cuda")
+        tag = "" if mlen == 32 else " (1 KiB messages)"
+        t = timed(lambda: check(L.cb200_ed25519_keygen(k32.data_ptr(), pk.data_ptr(), sk.data_ptr(), n)), steps=3)
+        if mlen == 32:
+            res["Ed25519 KeyGen"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+        t = timed(lambda: check(L.cb200_ed25519_sign(sk.data_ptr(), 64, msg.data_ptr(), off.data_ptr(), sig.data_ptr(), n)),
+                  steps=3)
+        res["Ed25519 Sign" + tag] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+        t = timed(lambda: check(L.cb200_ed25519_verify(pk.data_ptr(), 32, msg.data_ptr(), off.data_ptr(), sig.data_ptr(),
+                                                       ok.data_ptr(), n)), steps=3)
+        res["Ed25519 Verify" + tag] = {"n": n, "ms": t, "per_s": n / (t * 1e-3), "all_valid": bool(ok.all().item())}
+    msg = torch.randint(0, 256, (n * 32 + 8,), generator=g, device="cuda", dtype=torch.uint8)
+    off = (torch.arange(n + 1, device="cuda", dtype=torch.int64) * 32).contiguous()
+    pk = torch.empty((n, 1344), dtype=torch.uint8, device="cuda")
+    sk = torch.empty((n, 2560), dtype=torch.uint8, device="cuda")
+    sig = torch.empty((n, 2484), dtype=torch.uint8, device="cuda")
+    st = torch.zeros((n,), dtype=torch.uint8, device="cuda")
+    ok = torch.zeros((n,), dtype=torch.uint8, device="cuda")
+    t = timed(lambda: check(L.cb200_eddilithium2_keygen(k32.data_ptr(), pk.data_ptr(), sk.data_ptr(), n)), steps=3)
+    res["Ed25519-Dilithium2 KeyGen"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+    t = timed(lambda: check(L.cb200_eddilithium2_sign(sk.data_ptr(), 2560, msg.data_ptr(), off.data_ptr(), sig.data_ptr(),
+                                                      st.data_ptr(), n)), steps=2, warm=2)
+    res["Ed25519-Dilithium2 Sign"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+    t = timed(lambda: check(L.cb200_eddilithium2_verify(pk.data_ptr(), 1344, msg.data_ptr(), off.data_ptr(), sig.data_ptr(),
+                                                        ok.data_ptr(), n)), steps=3)
+    res["Ed25519-Dilithium2 Verify"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3), "all_valid": bool(ok.all().item())}
+    del msg, off, pk, sk, sig, st, ok, k32, pub
+    torch.cuda.empty_cache()
+
+
+if "--eddsa" in sys.argv:  # only the signature lines above and the X25519 lines they are compared with
+    eddsa_lines(res)
+    print(json.dumps(res, indent=1))
+    sys.exit(0)
+
+
 for name, k, log2 in (("ML-KEM-768", 3, 20), ("ML-KEM-1024", 4, 20)):
     scheme = mlkem.ByName(name)
     n = 1 << log2
@@ -146,4 +206,5 @@ for name, mode in (("ML-DSA-44", 44), ("ML-DSA-65", 65), ("ML-DSA-87", 87), ("Di
     res[f"{name} verify"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3), "all_valid": bool(ok.all().item())}
     del pk, sk, sig
     torch.cuda.empty_cache()
+eddsa_lines(res)
 print(json.dumps(res, indent=1))

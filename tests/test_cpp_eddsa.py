@@ -1,0 +1,53 @@
+"""The Ed25519 and Ed25519-Dilithium2 entries of the C++ sign::Scheme (include/circl_b200.hpp), through
+tests/cpp/test_sign_eddsa.cpp: registry order and sizes on the CPU, transcripts against OpenSSL and the oracle on the
+GPU."""
+import os
+import subprocess
+
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def _build(tmp_path):
+    from circl_b200 import _ffi
+    _ffi.lib()
+    exe = str(tmp_path / "test_sign_eddsa")
+    cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-I", os.path.join(ROOT, "include"),
+           os.path.join(ROOT, "tests", "cpp", "test_sign_eddsa.cpp"), "-o", exe,
+           "-L", os.path.join(ROOT, "circl_b200"), "-lcirclb200", "-Wl,-rpath," + os.path.join(ROOT, "circl_b200")]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    return exe
+
+
+def test_registry_and_sizes(tmp_path):
+    exe = _build(tmp_path)
+    r = subprocess.run([exe], capture_output=True, text=True, timeout=120, env=dict(os.environ, CB200_SIZES_ONLY="1"))
+    assert r.returncode == 0 and "ALL OK" in r.stdout, r.stdout + r.stderr
+
+
+@pytest.mark.gpu
+def test_transcripts_match_openssl_and_oracle(tmp_path):
+    from cryptography.hazmat.primitives.asymmetric.ed25519 import Ed25519PrivateKey
+    from oracle import ed25519 as oe
+    exe = _build(tmp_path)
+    r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
+    assert r.returncode == 0 and "ALL OK" in r.stdout, r.stdout + r.stderr
+    blocks, cur = {}, None
+    for line in r.stdout.splitlines():
+        if line.startswith("scheme="):
+            cur = line.split("=", 1)[1]
+            blocks[cur] = {}
+        elif "=" in line and cur:
+            k, v = line.split("=", 1)
+            blocks[cur][k] = bytes.fromhex(v)
+    seed = bytes((5 * i + 2) & 0xFF for i in range(32))
+    b = blocks["Ed25519"]
+    k = Ed25519PrivateKey.from_private_bytes(seed)
+    assert b["pk"] == k.public_key().public_bytes_raw() and b["sk"] == seed + b["pk"]
+    assert b["sig"] == k.sign(b"hello")
+    b = blocks["Ed25519-Dilithium2"]
+    pk, sk = oe.eddilithium2_keygen(seed)
+    assert (b["pk"], b["sk"]) == (pk, sk)
+    assert b["sig"] == oe.eddilithium2_sign(sk, b"hello")
