@@ -114,6 +114,24 @@ SYMBOLS = {
     "cb200_eddilithium2_private_key_size": (C.c_size_t, []),
     "cb200_eddilithium2_signature_size": (C.c_size_t, []),
     "cb200_eddilithium2_seed_size": (C.c_size_t, []),
+    "cb200_ed448_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_ed448_sign": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                   C.c_size_t]),
+    "cb200_ed448_verify": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                     C.c_void_p, C.c_size_t]),
+    "cb200_ed448_public_key_size": (C.c_size_t, []),
+    "cb200_ed448_private_key_size": (C.c_size_t, []),
+    "cb200_ed448_signature_size": (C.c_size_t, []),
+    "cb200_ed448_seed_size": (C.c_size_t, []),
+    "cb200_eddilithium3_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_eddilithium3_sign": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_size_t]),
+    "cb200_eddilithium3_verify": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_size_t]),
+    "cb200_eddilithium3_public_key_size": (C.c_size_t, []),
+    "cb200_eddilithium3_private_key_size": (C.c_size_t, []),
+    "cb200_eddilithium3_signature_size": (C.c_size_t, []),
+    "cb200_eddilithium3_seed_size": (C.c_size_t, []),
     "cb200_mlkem_decaps": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_mlkem_keygen": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_mlkem_private_key_size": (C.c_size_t, [C.c_int]),

@@ -59,6 +59,7 @@ struct Dev {
   void* kyber_tw = nullptr;     // 128 x {zeta, zetaq}, then 128 x {zp, kk} (kyber.cuh, low format)
   void* dil_tw = nullptr;       // 256 x {zeta, invzeta}
   void* x25519_table = nullptr; // 32 KiB: multiples 1..8 of 256^i B for the fixed-base X25519 KeyGen (x25519.cuh)
+  void* ed448_table = nullptr;  // 84 KiB: multiples 1..8 of 256^i G for Ed448's fixed base (ed448.cuh)
   // host staging pipeline (owned by the worker thread).  A chunk lives in one of kSlots slots (device images of its
   // buffers + a work set); all input copies go down one stream, all output copies down another, the kernels of a
   // slot down that slot's stream, tied by events: the input copy of chunk c + kSlots waits only for the KERNELS of
@@ -104,7 +105,8 @@ enum KernelId {
   KID_MLKEM_HASH_EK, KID_MLKEM_G, KID_MLKEM_SAMPLE, KID_MLKEM_ENCRYPT,
   KID_DIL_NTT, KID_DIL_INVNTT, KID_DIL_DOT, KID_DIL_EW,
   KID_MLDSA_EXPAND, KID_MLDSA_MU, KID_MLDSA_MASK, KID_MLDSA_W, KID_MLDSA_CHALLENGE, KID_MLDSA_RESPONSE,
-  KID_MLDSA_COMPACT, KID_X25519, KID_HYBRID_GLUE, KID_KECCAK, KID_SAMPLER, KID_MLKEM_SAMPLE_FIX, KID_X448, KID_ED25519, KID_COUNT
+  KID_MLDSA_COMPACT, KID_X25519, KID_HYBRID_GLUE, KID_KECCAK, KID_SAMPLER, KID_MLKEM_SAMPLE_FIX, KID_X448, KID_ED25519, KID_ED448,
+  KID_COUNT
 };
 const char* kernel_name(int id);
 

@@ -29,4 +29,5 @@ void dil_fill_twiddles(uint32_t* out);
 // tables.cu: twiddle tables other than Kyber's (ML-DSA) and the X25519 base table; called once per GPU at init
 struct Dev;
 int init_extra_tables(Dev& d);
+int init_ed448_table(Dev& d);  // ed448.cu
 }  // namespace cb200

@@ -20,6 +20,7 @@ int init_extra_tables(Dev& c) {  // device c.device is current
   if (c.x25519_table) cudaFree(c.x25519_table);
   CB200_CUDA(cudaMalloc(&c.x25519_table, xt.size() * sizeof(int32_t)));
   CB200_CUDA(cudaMemcpy(c.x25519_table, xt.data(), xt.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-  return 0;
+  // fixed-base table of Ed448 (ed448.cu)
+  return init_ed448_table(c);
 }
 }  // namespace cb200

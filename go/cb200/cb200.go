@@ -352,6 +352,133 @@ func EdDilithium2VerifyBatch(pk []byte, shared bool, msgs [][]byte, sig []byte, 
 	})
 }
 
+// ctxPtr returns a pointer to the context bytes (nil for an empty context).
+func ctxPtr(ctx []byte) *C.uint8_t {
+	if len(ctx) == 0 {
+		return nil
+	}
+	return u8(ctx)
+}
+
+// Ed448KeyGen: ed448.NewKeyFromSeed (sign/ed448/ed448.go:191-205) on n 57-byte seeds; pk receives n*57 bytes, sk
+// n*114 (seed || public key).
+func Ed448KeyGen(seeds, pk, sk []byte) error {
+	n := len(seeds) / 57
+	if len(seeds) != n*57 || len(pk) != n*57 || len(sk) != n*114 {
+		panic("cb200: seeds/pk/sk have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return call(func() C.int { return C.cb200_ed448_keygen(u8(seeds), u8(pk), u8(sk), C.size_t(n)) })
+}
+
+// Ed448SignBatch: ed448.Sign (ed448.go:207-271) on len(msgs) messages with the context ctx (at most 255 bytes; longer
+// returns an error where the reference panics).  sk holds one 114-byte private key (shared) or one per message; its
+// public half is used as given.  sig receives len(msgs)*114 bytes.
+func Ed448SignBatch(sk []byte, shared bool, msgs [][]byte, ctx []byte, sig []byte) error {
+	n := len(msgs)
+	if (shared && len(sk) != 114) || (!shared && len(sk) != n*114) || len(sig) != n*114 {
+		panic("cb200: sk/sig have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	blob, off := packMsgs(msgs)
+	stride := C.size_t(114)
+	if shared {
+		stride = 0
+	}
+	return call(func() C.int {
+		return C.cb200_ed448_sign(u8(sk), stride, u8(blob), (*C.uint64_t)(unsafe.Pointer(&off[0])), ctxPtr(ctx),
+			C.size_t(len(ctx)), u8(sig), C.size_t(n))
+	})
+}
+
+// Ed448VerifyBatch: ed448.Verify (ed448.go:294-339) on len(msgs) 114-byte signatures with the context ctx; pk holds
+// one 57-byte public key (shared) or one per message.  ok[i] is the reference's result (all false for a context over
+// 255 bytes).
+func Ed448VerifyBatch(pk []byte, shared bool, msgs [][]byte, ctx []byte, sig []byte, ok []bool) error {
+	n := len(msgs)
+	if (shared && len(pk) != 57) || (!shared && len(pk) != n*57) || len(sig) != n*114 || len(ok) != n {
+		panic("cb200: pk/sig/ok have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return verifyBatch(n, msgs, ok, func(blob []byte, off []uint64, res []byte) C.int {
+		stride := C.size_t(57)
+		if shared {
+			stride = 0
+		}
+		return C.cb200_ed448_verify(u8(pk), stride, u8(blob), (*C.uint64_t)(unsafe.Pointer(&off[0])), ctxPtr(ctx),
+			C.size_t(len(ctx)), u8(sig), u8(res), C.size_t(n))
+	})
+}
+
+// Sizes of Ed448-Dilithium3 (sign/eddilithium3/eddilithium.go:16-28).
+const (
+	EdDilithium3PublicKeySize  = 2009
+	EdDilithium3PrivateKeySize = 4057
+	EdDilithium3SignatureSize  = 3407
+)
+
+// EdDilithium3KeyGen: eddilithium3.NewKeyFromSeed (eddilithium.go:59-78) on n 57-byte seeds; pk and sk receive the
+// packed keys (n*2009 and n*4057 bytes).
+func EdDilithium3KeyGen(seeds, pk, sk []byte) error {
+	n := len(seeds) / 57
+	if len(seeds) != n*57 || len(pk) != n*EdDilithium3PublicKeySize || len(sk) != n*EdDilithium3PrivateKeySize {
+		panic("cb200: seeds/pk/sk have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return call(func() C.int { return C.cb200_eddilithium3_keygen(u8(seeds), u8(pk), u8(sk), C.size_t(n)) })
+}
+
+// EdDilithium3SignBatch: eddilithium3.SignTo (eddilithium.go:82-93) on len(msgs) messages with one packed key
+// (shared) or one per message; sig receives len(msgs)*3407 bytes.  An error is returned if a Dilithium3 half
+// exhausted its 576 attempts (the reference panics there).
+func EdDilithium3SignBatch(sk []byte, shared bool, msgs [][]byte, sig []byte) error {
+	n := len(msgs)
+	if (shared && len(sk) != EdDilithium3PrivateKeySize) || (!shared && len(sk) != n*EdDilithium3PrivateKeySize) ||
+		len(sig) != n*EdDilithium3SignatureSize {
+		panic("cb200: sk/sig have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	blob, off := packMsgs(msgs)
+	stride := C.size_t(EdDilithium3PrivateKeySize)
+	if shared {
+		stride = 0
+	}
+	return call(func() C.int {
+		return C.cb200_eddilithium3_sign(u8(sk), stride, u8(blob), (*C.uint64_t)(unsafe.Pointer(&off[0])), u8(sig), nil,
+			C.size_t(n))
+	})
+}
+
+// EdDilithium3VerifyBatch: eddilithium3.Verify (eddilithium.go:96-110): both halves must verify.
+func EdDilithium3VerifyBatch(pk []byte, shared bool, msgs [][]byte, sig []byte, ok []bool) error {
+	n := len(msgs)
+	if (shared && len(pk) != EdDilithium3PublicKeySize) || (!shared && len(pk) != n*EdDilithium3PublicKeySize) ||
+		len(sig) != n*EdDilithium3SignatureSize || len(ok) != n {
+		panic("cb200: pk/sig/ok have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return verifyBatch(n, msgs, ok, func(blob []byte, off []uint64, res []byte) C.int {
+		stride := C.size_t(EdDilithium3PublicKeySize)
+		if shared {
+			stride = 0
+		}
+		return C.cb200_eddilithium3_verify(u8(pk), stride, u8(blob), (*C.uint64_t)(unsafe.Pointer(&off[0])), u8(sig),
+			u8(res), C.size_t(n))
+	})
+}
+
 // Hybrid scheme identifiers of include/circl_b200.h (kem/hybrid/hybrid.go:34-93).
 const (
 	HybridX25519MLKEM768 = 0

@@ -313,6 +313,44 @@ size_t cb200_eddilithium2_private_key_size(void); /* 2560 */
 size_t cb200_eddilithium2_signature_size(void);   /* 2484 */
 size_t cb200_eddilithium2_seed_size(void);        /* 32 */
 
+/* ---- Ed448 (sign/ed448, RFC 8032 pure Ed448) ----
+ * keygen = NewKeyFromSeed (ed448.go:191-205): seeds n x 57 -> pk n x 57, sk n x 114 (= seed || pk; may be NULL).
+ * sign = Sign (ed448.go:207-271): sk rows of 114 bytes at sk + i*sk_stride (0 = one key for the batch); A is read from
+ * bytes 57..113 of the key as given, as the reference does; sig n x 114.
+ * verify = Verify (ed448.go:294-339): ok[i] = 1 iff S < l with byte 113 = 0, pk decodes and encode(Q) == R for the
+ * reference's Q = [S]G - [4 ((k / 4) mod l)]A, which drops the 4-torsion component of A.
+ * context: one host string of ctxlen bytes for the whole batch (may be NULL when ctxlen = 0).  ctxlen > 255: sign
+ * returns CB200_ERR_ARG (the reference panics), verify sets every ok[i] = 0 and returns 0 (the reference returns false).
+ * Messages as in cb200_ed25519_sign, with the same read rule around msgs[0] and behind the last message.
+ * Device pointers: msg_off 8-byte aligned; seeds, keys and signatures may start at any byte. */
+int cb200_ed448_keygen(const uint8_t *seeds, uint8_t *pk, uint8_t *sk, size_t n);
+int cb200_ed448_sign(const uint8_t *sk, size_t sk_stride, const uint8_t *msgs, const uint64_t *msg_off,
+                     const uint8_t *context, size_t ctxlen, uint8_t *sig, size_t n);
+int cb200_ed448_verify(const uint8_t *pk, size_t pk_stride, const uint8_t *msgs, const uint64_t *msg_off,
+                       const uint8_t *context, size_t ctxlen, const uint8_t *sig, uint8_t *ok, size_t n);
+size_t cb200_ed448_public_key_size(void);  /* 57 */
+size_t cb200_ed448_private_key_size(void); /* 114 */
+size_t cb200_ed448_signature_size(void);   /* 114 */
+size_t cb200_ed448_seed_size(void);        /* 57 */
+
+/* ---- Ed448-Dilithium3 (sign/eddilithium3): pk = Dilithium3 pk (1952) || Ed448 pk (57) = 2009, sk = Dilithium3
+ * packed sk (4000) || Ed448 seed (57) = 4057, sig = Dilithium3 sig (3293) || Ed448 sig (114) = 3407, seed 57.
+ * keygen = NewKeyFromSeed (eddilithium.go:59-78, SHAKE256(seed) -> Dilithium3 seed (32) || Ed448 seed (57)); sign =
+ * SignTo (:82-93; Ed448 with an empty context, its public key re-derived from the seed as PrivateKey.Unpack does);
+ * verify = Verify (:96-110, both halves).  status (optional): 1 = Dilithium3's 576-attempt cap (CB200_ERR_SIGN_ATTEMPTS
+ * for host pointers).  No context string (sign.ErrContextNotSupported).  Device pointers: msg_off 16-byte aligned
+ * (the Dilithium3 flows read it); seeds, keys, signatures and strides may be at any byte, since every row size is odd
+ * and the Dilithium3 halves are staged through aligned scratch. */
+int cb200_eddilithium3_keygen(const uint8_t *seeds, uint8_t *pk, uint8_t *sk, size_t n);
+int cb200_eddilithium3_sign(const uint8_t *sk, size_t sk_stride, const uint8_t *msgs, const uint64_t *msg_off, uint8_t *sig,
+                            uint8_t *status, size_t n);
+int cb200_eddilithium3_verify(const uint8_t *pk, size_t pk_stride, const uint8_t *msgs, const uint64_t *msg_off,
+                              const uint8_t *sig, uint8_t *ok, size_t n);
+size_t cb200_eddilithium3_public_key_size(void);  /* 2009 */
+size_t cb200_eddilithium3_private_key_size(void); /* 4057 */
+size_t cb200_eddilithium3_signature_size(void);   /* 3407 */
+size_t cb200_eddilithium3_seed_size(void);        /* 57 */
+
 /* ---- ML-DSA-65 ---- */
 /* sign.Scheme.Sign / SignTo    sign/mldsa/mldsa65/dilithium.go:282-303,56-84  ->
  * internal.SignTo (ML-DSA.Sign_internal)  sign/mldsa/mldsa65/internal/dilithium.go:340-470,

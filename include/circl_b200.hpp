@@ -310,26 +310,33 @@ class PrivateKey {
 };
 
 class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 44, 65, 87), round-3 Dilithium2/3/5 (2, 3, 5),
-                // Ed25519 (sign/ed25519/signapi.go) and Ed25519-Dilithium2 (sign/eddilithium2/signapi.go)
+                // Ed25519 (sign/ed25519/signapi.go), Ed25519-Dilithium2 (sign/eddilithium2/signapi.go), Ed448
+                // (sign/ed448/signapi.go) and Ed448-Dilithium3 (sign/eddilithium3/signapi.go)
  public:
-  enum Family { kMLDSA, kEd25519, kEdDilithium2 };
+  enum Family { kMLDSA, kEd25519, kEdDilithium2, kEd448, kEdDilithium3 };
   Scheme(std::string name, int mode, Family family = kMLDSA) : name_(std::move(name)), mode_(mode), family_(family) {}
   const std::string& Name() const { return name_; }
   size_t PublicKeySize() const {
     return family_ == kEd25519 ? cb200_ed25519_public_key_size()
-           : family_ == kEdDilithium2 ? cb200_eddilithium2_public_key_size() : cb200_mldsa_public_key_size(mode_);
+           : family_ == kEdDilithium2 ? cb200_eddilithium2_public_key_size()
+           : family_ == kEd448 ? cb200_ed448_public_key_size()
+           : family_ == kEdDilithium3 ? cb200_eddilithium3_public_key_size() : cb200_mldsa_public_key_size(mode_);
   }
   size_t PrivateKeySize() const {
     return family_ == kEd25519 ? cb200_ed25519_private_key_size()
-           : family_ == kEdDilithium2 ? cb200_eddilithium2_private_key_size() : cb200_mldsa_private_key_size(mode_);
+           : family_ == kEdDilithium2 ? cb200_eddilithium2_private_key_size()
+           : family_ == kEd448 ? cb200_ed448_private_key_size()
+           : family_ == kEdDilithium3 ? cb200_eddilithium3_private_key_size() : cb200_mldsa_private_key_size(mode_);
   }
   size_t SignatureSize() const {
     return family_ == kEd25519 ? cb200_ed25519_signature_size()
-           : family_ == kEdDilithium2 ? cb200_eddilithium2_signature_size() : cb200_mldsa_signature_size(mode_);
+           : family_ == kEdDilithium2 ? cb200_eddilithium2_signature_size()
+           : family_ == kEd448 ? cb200_ed448_signature_size()
+           : family_ == kEdDilithium3 ? cb200_eddilithium3_signature_size() : cb200_mldsa_signature_size(mode_);
   }
-  size_t SeedSize() const { return 32; }
-  // round 3, Ed25519 and Ed25519-Dilithium2: sign.ErrContextNotSupported
-  bool SupportsContext() const { return family_ == kMLDSA && mode_ > 10; }
+  size_t SeedSize() const { return family_ == kEd448 || family_ == kEdDilithium3 ? 57 : 32; }
+  // round 3, Ed25519, Ed25519-Dilithium2 and Ed448-Dilithium3: sign.ErrContextNotSupported; Ed448 takes a context
+  bool SupportsContext() const { return (family_ == kMLDSA && mode_ > 10) || family_ == kEd448; }
 
   std::pair<PublicKey, PrivateKey> DeriveKey(const Bytes& seed) const {  // dilithium.go:266-276, ed25519 signapi.go
     if (seed.size() != SeedSize()) throw std::logic_error("sign: invalid seed size");  // Go panics here
@@ -350,12 +357,13 @@ class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 4
     if (b.size() != PrivateKeySize()) throw ErrPrivKeySize();
     return PrivateKey(this, b);
   }
-  // PrivateKey.Public() of Ed25519 (ed25519.go: the second half of the private key).  The ML-DSA and composite
-  // private keys do not hold their public key; their Public() needs the seed (DeriveKey).
+  // PrivateKey.Public() of Ed25519 and Ed448 (ed25519.go, ed448.go: the second half of the private key).  The ML-DSA
+  // and composite private keys do not hold their public key; their Public() needs the seed (DeriveKey).
   PublicKey Public(const PrivateKey& sk) const {
-    if (family_ != kEd25519) throw std::logic_error("sign: Public() from a packed private key is served for Ed25519 only");
+    if (family_ != kEd25519 && family_ != kEd448)
+      throw std::logic_error("sign: Public() from a packed private key is served for Ed25519 and Ed448 only");
     const Bytes& b = sk.MarshalBinary();
-    return PublicKey(this, Bytes(b.begin() + 32, b.end()));
+    return PublicKey(this, Bytes(b.begin() + PublicKeySize(), b.end()));
   }
   // deterministic signing, as sign.Scheme.Sign does (dilithium.go:282-303, ed25519 signapi.go)
   Bytes Sign(const PrivateKey& sk, const Bytes& msg, const SignatureOpts* opts = nullptr) const {
@@ -366,7 +374,7 @@ class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 4
   }
   bool Verify(const PublicKey& pk, const Bytes& msg, const Bytes& sig, const SignatureOpts* opts = nullptr) const {
     const std::string ctx = opts ? opts->Context : std::string();
-    if (!ctx.empty() && family_ != kMLDSA) throw ErrContextNotSupported();
+    if (!ctx.empty() && family_ != kMLDSA && family_ != kEd448) throw ErrContextNotSupported();
     if (ctx.size() > 255 || sig.size() != SignatureSize()) return false;  // dilithium.go:116-118, ed25519.go:330-334
     uint8_t ok = 0;
     const uint64_t off[2] = {0, msg.size()};
@@ -376,6 +384,11 @@ class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 4
       check(cb200_ed25519_verify(pk.MarshalBinary().data(), 0, padded.data(), off, sig.data(), &ok, 1));
     else if (family_ == kEdDilithium2)
       check(cb200_eddilithium2_verify(pk.MarshalBinary().data(), 0, padded.data(), off, sig.data(), &ok, 1));
+    else if (family_ == kEd448)
+      check(cb200_ed448_verify(pk.MarshalBinary().data(), 0, padded.data(), off, (const uint8_t*)ctx.data(), ctx.size(),
+                               sig.data(), &ok, 1));
+    else if (family_ == kEdDilithium3)
+      check(cb200_eddilithium3_verify(pk.MarshalBinary().data(), 0, padded.data(), off, sig.data(), &ok, 1));
     else
       check(cb200_mldsa_verify(mode_, pk.MarshalBinary().data(), 0, padded.data(), off, (const uint8_t*)ctx.data(), ctx.size(),
                                sig.data(), &ok, 1, 0));
@@ -396,6 +409,11 @@ class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 4
       check(cb200_ed25519_sign(sks.data(), stride, padded.data(), off.data(), sigs.data(), n));
     else if (family_ == kEdDilithium2)
       check(cb200_eddilithium2_sign(sks.data(), stride, padded.data(), off.data(), sigs.data(), nullptr, n));
+    else if (family_ == kEd448)
+      check(cb200_ed448_sign(sks.data(), stride, padded.data(), off.data(), (const uint8_t*)ctx.data(), ctx.size(), sigs.data(),
+                             n));
+    else if (family_ == kEdDilithium3)
+      check(cb200_eddilithium3_sign(sks.data(), stride, padded.data(), off.data(), sigs.data(), nullptr, n));
     else
       check(cb200_mldsa_sign(mode_, sks.data(), stride, padded.data(), off.data(), (const uint8_t*)ctx.data(), ctx.size(), nullptr,
                              sigs.data(), nullptr, n, 0, nullptr));
@@ -416,6 +434,11 @@ class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 4
       check(cb200_ed25519_verify(pks.data(), stride, padded.data(), off.data(), sigs.data(), ok.data(), n));
     else if (family_ == kEdDilithium2)
       check(cb200_eddilithium2_verify(pks.data(), stride, padded.data(), off.data(), sigs.data(), ok.data(), n));
+    else if (family_ == kEd448)
+      check(cb200_ed448_verify(pks.data(), stride, padded.data(), off.data(), (const uint8_t*)ctx.data(), ctx.size(), sigs.data(),
+                               ok.data(), n));
+    else if (family_ == kEdDilithium3)
+      check(cb200_eddilithium3_verify(pks.data(), stride, padded.data(), off.data(), sigs.data(), ok.data(), n));
     else
       check(cb200_mldsa_verify(mode_, pks.data(), stride, padded.data(), off.data(), (const uint8_t*)ctx.data(), ctx.size(),
                                sigs.data(), ok.data(), n, 0));
@@ -429,6 +452,10 @@ class Scheme {  // sign.Scheme (sign/sign.go:48-94) for ML-DSA-44/65/87 (modes 4
       check(cb200_ed25519_keygen(seeds.data(), pks.data(), sks.data(), n));
     else if (family_ == kEdDilithium2)
       check(cb200_eddilithium2_keygen(seeds.data(), pks.data(), sks.data(), n));
+    else if (family_ == kEd448)
+      check(cb200_ed448_keygen(seeds.data(), pks.data(), sks.data(), n));
+    else if (family_ == kEdDilithium3)
+      check(cb200_eddilithium3_keygen(seeds.data(), pks.data(), sks.data(), n));
     else
       check(cb200_mldsa_keygen(mode_, seeds.data(), pks.data(), sks.data(), n));
   }
@@ -457,6 +484,21 @@ inline const Scheme* ByName(const std::string& name) {  // sign/schemes/schemes.
     if (kem::lower(s->Name()) == kem::lower(name)) return s;
   return nullptr;
 }
+
+// Ed448 and Ed448-Dilithium3 (sign/schemes/schemes.go:31-54 lists them second and fourth).  They have a registry of
+// their own so that All() above keeps its eight schemes.
+namespace ed448 {
+inline const std::vector<const Scheme*>& All() {
+  static const Scheme e448("Ed448", 0, Scheme::kEd448), ed3("Ed448-Dilithium3", 3, Scheme::kEdDilithium3);
+  static const std::vector<const Scheme*> all = {&e448, &ed3};
+  return all;
+}
+inline const Scheme* ByName(const std::string& name) {  // case-insensitive; nullptr = no such scheme
+  for (const Scheme* s : All())
+    if (kem::lower(s->Name()) == kem::lower(name)) return s;
+  return nullptr;
+}
+}  // namespace ed448
 
 }  // namespace sign
 }  // namespace circl

@@ -82,6 +82,66 @@ def eddsa_lines(res):
     torch.cuda.empty_cache()
 
 
+def ed448_lines(res):
+    """Ed448 and Ed448-Dilithium3 through the C ABI, device-resident, 2^18 operations, per-op keys, 32-byte and 1 KiB
+    messages, empty context, with X448 KeyGen / Shared of the same run for comparison."""
+    from circl_b200 import x448
+    from circl_b200._ffi import check, lib
+    L = lib()
+    check(L.cb200_set_stream(torch.cuda.current_stream().cuda_stream))
+    n = 1 << 18
+    g = torch.Generator(device="cuda").manual_seed(12)
+    k56 = torch.randint(0, 256, (n, 56), generator=g, device="cuda", dtype=torch.uint8)
+    t = timed(lambda: x448.x448_keygen(k56), steps=3)
+    pub = x448.x448_keygen(k56)
+    res["X448 KeyGen"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+    t = timed(lambda: x448.x448_shared(k56, pub), steps=3)
+    res["X448 Shared"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+    del k56, pub
+    k57 = torch.randint(0, 256, (n, 57), generator=g, device="cuda", dtype=torch.uint8)
+    for mlen in (32, 1024):
+        msg = torch.randint(0, 256, (n * mlen + 8,), generator=g, device="cuda", dtype=torch.uint8)
+        off = (torch.arange(n + 1, device="cuda", dtype=torch.int64) * mlen).contiguous()
+        pk = torch.empty((n, 57), dtype=torch.uint8, device="cuda")
+        sk = torch.empty((n, 114), dtype=torch.uint8, device="cuda")
+        sig = torch.empty((n, 114), dtype=torch.uint8, device="cuda")
+        ok = torch.zeros((n,), dtype=torch.uint8, device="cuda")
+        tag = "" if mlen == 32 else " (1 KiB messages)"
+        t = timed(lambda: check(L.cb200_ed448_keygen(k57.data_ptr(), pk.data_ptr(), sk.data_ptr(), n)), steps=3)
+        if mlen == 32:
+            res["Ed448 KeyGen"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+        t = timed(lambda: check(L.cb200_ed448_sign(sk.data_ptr(), 114, msg.data_ptr(), off.data_ptr(), None, 0,
+                                                   sig.data_ptr(), n)), steps=3)
+        res["Ed448 Sign" + tag] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+        t = timed(lambda: check(L.cb200_ed448_verify(pk.data_ptr(), 57, msg.data_ptr(), off.data_ptr(), None, 0,
+                                                     sig.data_ptr(), ok.data_ptr(), n)), steps=3)
+        res["Ed448 Verify" + tag] = {"n": n, "ms": t, "per_s": n / (t * 1e-3), "all_valid": bool(ok.all().item())}
+        del msg, off, pk, sk, sig, ok
+    msg = torch.randint(0, 256, (n * 32 + 8,), generator=g, device="cuda", dtype=torch.uint8)
+    off = (torch.arange(n + 1, device="cuda", dtype=torch.int64) * 32).contiguous()
+    pk = torch.empty((n, 2009), dtype=torch.uint8, device="cuda")
+    sk = torch.empty((n, 4057), dtype=torch.uint8, device="cuda")
+    sig = torch.empty((n, 3407), dtype=torch.uint8, device="cuda")
+    st = torch.zeros((n,), dtype=torch.uint8, device="cuda")
+    ok = torch.zeros((n,), dtype=torch.uint8, device="cuda")
+    t = timed(lambda: check(L.cb200_eddilithium3_keygen(k57.data_ptr(), pk.data_ptr(), sk.data_ptr(), n)), steps=3)
+    res["Ed448-Dilithium3 KeyGen"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+    t = timed(lambda: check(L.cb200_eddilithium3_sign(sk.data_ptr(), 4057, msg.data_ptr(), off.data_ptr(), sig.data_ptr(),
+                                                      st.data_ptr(), n)), steps=2, warm=2)
+    res["Ed448-Dilithium3 Sign"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+    t = timed(lambda: check(L.cb200_eddilithium3_verify(pk.data_ptr(), 2009, msg.data_ptr(), off.data_ptr(), sig.data_ptr(),
+                                                        ok.data_ptr(), n)), steps=3)
+    res["Ed448-Dilithium3 Verify"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3), "all_valid": bool(ok.all().item())}
+    del msg, off, pk, sk, sig, st, ok, k57
+    torch.cuda.empty_cache()
+
+
+if "--ed448" in sys.argv:  # only the Ed448 lines above and the X448 lines they are compared with
+    ed448_lines(res)
+    print(json.dumps(res, indent=1))
+    sys.exit(0)
+
+
 if "--eddsa" in sys.argv:  # only the signature lines above and the X25519 lines they are compared with
     eddsa_lines(res)
     print(json.dumps(res, indent=1))
