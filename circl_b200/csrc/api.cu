@@ -11,6 +11,7 @@
 #include "../../include/circl_b200.h"
 #include "common.cuh"
 #include "context.h"
+#include "flow_internal.h"
 
 #include <sys/mman.h>
 
@@ -505,6 +506,7 @@ int run_staged(std::vector<Buf>& bufs, size_t first0, size_t n, size_t chunk,
 int HostCall::run(size_t n) {
   bit0 = 0;
   bit1 = 0;
+  nonzero = 0;
   return for_each_shard(n, min_shard, [&](size_t first0, size_t cnt) -> int {
     std::vector<Buf> b = bufs;
     uint8_t* pin = nullptr;
@@ -518,27 +520,19 @@ int HostCall::run(size_t n) {
     int rc = run_staged(b, first0, cnt, chunk, body);
     if (rc) return rc;
     if (pin) {
-      size_t c0 = 0, c1 = 0;
+      size_t c0 = 0, c1 = 0, cz = 0;
       for (size_t i = 0; i < cnt; i++) {
         c0 += (pin[i] & 1) != 0;
         c1 += (pin[i] & 2) != 0;
+        cz += pin[i] != 0;
       }
       bit0 += c0;
       bit1 += c1;
+      nonzero += cz;
       if (user_status) memcpy(user_status + first0, pin, cnt);
     }
     return 0;
   });
-}
-
-int run_host(const std::vector<Buf>& bufs, size_t n, size_t chunk, size_t min_shard,
-             const std::function<int(void** dev, size_t count, size_t first, cudaStream_t st, int slot)>& body) {
-  HostCall hc;
-  hc.bufs = bufs;
-  hc.chunk = chunk;
-  hc.min_shard = min_shard;
-  hc.body = body;
-  return hc.run(n);
 }
 
 // number of polynomials per staging chunk: 64 MiB of int16 polys keeps three
@@ -798,23 +792,11 @@ int cb200_kyber_ntt(int16_t* polys, size_t n, int inverse) {
     set_error("cb200_kyber_ntt: null pointer");
     return CB200_ERR_ARG;
   }
-  if (is_device_ptr(polys)) {
-    if ((uintptr_t)polys & 15) {
-      set_error("cb200_kyber_ntt: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(polys);
-    if (call.rc) return call.rc;
-    return launch_kyber_ntt(polys, n, inverse, ctx().kyber_tw, call.st);
-  }
-  HostCall hc;
-  hc.bufs = {Buf{polys, polys, 512, false, 0}};
-  hc.chunk = kPolyChunk;
-  hc.min_shard = 1u << 15;
-  hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return launch_kyber_ntt((int16_t*)d[0], cnt, inverse, ctx().kyber_tw, st);
-  };
-  return hc.run(n);
+  Batch b{"cb200_kyber_ntt", n, polys, kPolyChunk, 1u << 15, {{polys, 512, 512, kInOut}},
+          {{!aligned({polys}, {}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return launch_kyber_ntt((int16_t*)r[0].p, cnt, inverse, ctx().kyber_tw, st);
+  });
 }
 
 int cb200_kyber_dot(int16_t* out, const int16_t* a, const int16_t* b, int k, size_t n) {
@@ -825,29 +807,12 @@ int cb200_kyber_dot(int16_t* out, const int16_t* a, const int16_t* b, int k, siz
     set_error("cb200_kyber_dot: bad argument");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(out);
-  if (dev != is_device_ptr(a) || dev != is_device_ptr(b)) {
-    set_error("cb200_kyber_dot: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (((uintptr_t)out | (uintptr_t)a | (uintptr_t)b) & 15) {
-      set_error("cb200_kyber_dot: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(out);
-    if (call.rc) return call.rc;
-    return launch_kyber_dot(out, a, b, k, n, ctx().kyber_tw, call.st);
-  }
-  HostCall hc;
-  hc.bufs = {Buf{nullptr, out, 512, false, 0}, Buf{a, nullptr, 512 * (size_t)k, false, 0},
-             Buf{b, nullptr, 512 * (size_t)k, false, 0}};
-  hc.chunk = kPolyChunk / k;
-  hc.min_shard = (1u << 15) / k;
-  hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return launch_kyber_dot((int16_t*)d[0], (const int16_t*)d[1], (const int16_t*)d[2], k, cnt, ctx().kyber_tw, st);
-  };
-  return hc.run(n);
+  const size_t ku = 512 * (size_t)k;
+  Batch bt{"cb200_kyber_dot", n, out, kPolyChunk / k, (1u << 15) / k, {{out, 512, 512, kOut}, {a, ku, ku, kIn}, {b, ku, ku, kIn}},
+           {{!aligned({out, a, b}, {}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  return run_batch(bt, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return launch_kyber_dot((int16_t*)r[0].p, (const int16_t*)r[1].p, (const int16_t*)r[2].p, k, cnt, ctx().kyber_tw, st);
+  });
 }
 
 int cb200_kyber_mulhat(int16_t* out, const int16_t* a, const int16_t* b, size_t n) {
@@ -863,29 +828,12 @@ int cb200_kyber_poly_op(int op, int16_t* out, const int16_t* a, const int16_t* b
     set_error("cb200_kyber_poly_op: bad argument");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(out);
-  if (dev != is_device_ptr(a) || (binary && dev != is_device_ptr(b))) {
-    set_error("cb200_kyber_poly_op: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (((uintptr_t)out | (uintptr_t)a | (uintptr_t)(binary ? b : nullptr)) & 15) {
-      set_error("cb200_kyber_poly_op: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(out);
-    if (call.rc) return call.rc;
-    return launch_kyber_poly_op(op, out, a, b, n, call.st);
-  }
-  HostCall hc;
-  hc.bufs = {Buf{nullptr, out, 512, false, 0}, Buf{a, nullptr, 512, false, 0},
-             Buf{binary ? b : nullptr, nullptr, 512, false, 0}};
-  hc.chunk = kPolyChunk;
-  hc.min_shard = 1u << 15;
-  hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return launch_kyber_poly_op(op, (int16_t*)d[0], (const int16_t*)d[1], (const int16_t*)d[2], cnt, st);
-  };
-  return hc.run(n);
+  if (!binary) b = nullptr;
+  Batch bt{"cb200_kyber_poly_op", n, out, kPolyChunk, 1u << 15, {{out, 512, 512, kOut}, {a, 512, 512, kIn}, {b, 512, 512, kIn}},
+           {{!aligned({out, a, b}, {}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  return run_batch(bt, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return launch_kyber_poly_op(op, (int16_t*)r[0].p, (const int16_t*)r[1].p, (const int16_t*)r[2].p, cnt, st);
+  });
 }
 
 }  // extern "C"

@@ -178,17 +178,13 @@ struct HostCall {
   size_t chunk = 1u << 15;
   size_t min_shard = 1u << 13;
   // index in bufs of the per-op status bytes (unit 1, no host pointers); they return through pinned memory, are
-  // counted (bit 0 / bit 1 set) and copied to user_status if that is not null
+  // counted (bit 0 / bit 1 / any bit set) and copied to user_status if that is not null
   int status_buf = -1;
   uint8_t* user_status = nullptr;
   std::function<int(void** dev, size_t count, size_t first, cudaStream_t st, int slot)> body;
-  std::atomic<size_t> bit0{0}, bit1{0};
+  std::atomic<size_t> bit0{0}, bit1{0}, nonzero{0};
   int run(size_t n);
 };
-
-// A HostCall without status bytes.
-int run_host(const std::vector<Buf>& bufs, size_t n, size_t chunk, size_t min_shard,
-             const std::function<int(void** dev, size_t count, size_t first, cudaStream_t st, int slot)>& body);
 
 // Runs fn(first, count) for one contiguous range per GPU, each on that GPU's worker thread (ctx() is that GPU);
 // returns the first non-zero result and carries its error text over to the caller's thread.

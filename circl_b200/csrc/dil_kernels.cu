@@ -8,6 +8,7 @@
 #include "../../include/circl_b200.h"
 #include "context.h"
 #include "dilithium.cuh"
+#include "flow_internal.h"
 
 namespace cb200 {
 namespace dil {
@@ -252,19 +253,10 @@ int cb200_dil_ntt(uint32_t* polys, size_t n, int inverse) {
     set_error("cb200_dil_ntt: null pointer");
     return CB200_ERR_ARG;
   }
-  if (is_device_ptr(polys)) {
-    if ((uintptr_t)polys & 15) {
-      set_error("cb200_dil_ntt: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(polys);
-    if (call.rc) return call.rc;
-    return launch_dil_ntt(polys, n, inverse, ctx().dil_tw, call.st);
-  }
-  std::vector<Buf> bufs(1);
-  bufs[0] = Buf{polys, polys, 1024, false, 0};
-  return run_host(bufs, n, 1u << 16, 1u << 14, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return launch_dil_ntt((uint32_t*)d[0], cnt, inverse, ctx().dil_tw, st);
+  Batch b{"cb200_dil_ntt", n, polys, 1u << 16, 1u << 14, {{polys, 1024, 1024, kInOut}},
+          {{!aligned({polys}, {}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return launch_dil_ntt((uint32_t*)r[0].p, cnt, inverse, ctx().dil_tw, st);
   });
 }
 
@@ -276,26 +268,12 @@ int cb200_dil_dot(uint32_t* out, const uint32_t* a, const uint32_t* b, int k, si
     set_error("cb200_dil_dot: bad argument");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(out);
-  if (dev != is_device_ptr(a) || dev != is_device_ptr(b)) {
-    set_error("cb200_dil_dot: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (((uintptr_t)out | (uintptr_t)a | (uintptr_t)b) & 15) {
-      set_error("cb200_dil_dot: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(out);
-    if (call.rc) return call.rc;
-    return launch_dil_dot(out, a, b, k, n, call.st);
-  }
-  std::vector<Buf> bufs(3);
-  bufs[0] = Buf{nullptr, out, 1024, false, 0};
-  bufs[1] = Buf{a, nullptr, 1024 * (size_t)k, false, 0};
-  bufs[2] = Buf{b, nullptr, 1024 * (size_t)k, false, 0};
-  return run_host(bufs, n, (1u << 16) / k, (1u << 14) / k, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return launch_dil_dot((uint32_t*)d[0], (const uint32_t*)d[1], (const uint32_t*)d[2], k, cnt, st);
+  const size_t ku = 1024 * (size_t)k;
+  Batch bt{"cb200_dil_dot", n, out, (1u << 16) / k, (1u << 14) / k,
+           {{out, 1024, 1024, kOut}, {a, ku, ku, kIn}, {b, ku, ku, kIn}},
+           {{!aligned({out, a, b}, {}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  return run_batch(bt, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return launch_dil_dot((uint32_t*)r[0].p, (const uint32_t*)r[1].p, (const uint32_t*)r[2].p, k, cnt, st);
   });
 }
 
@@ -312,26 +290,12 @@ int cb200_dil_poly_op(int op, uint32_t* out, const uint32_t* a, const uint32_t* 
     set_error("cb200_dil_poly_op: bad argument");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(out);
-  if (dev != is_device_ptr(a) || (binary && dev != is_device_ptr(b))) {
-    set_error("cb200_dil_poly_op: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (((uintptr_t)out | (uintptr_t)a | (uintptr_t)(binary ? b : nullptr)) & 15) {
-      set_error("cb200_dil_poly_op: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(out);
-    if (call.rc) return call.rc;
-    return launch_dil_poly_op(op, out, a, b, n, call.st);
-  }
-  std::vector<Buf> bufs(3);
-  bufs[0] = Buf{nullptr, out, 1024, false, 0};
-  bufs[1] = Buf{a, nullptr, 1024, false, 0};
-  bufs[2] = Buf{binary ? b : nullptr, nullptr, 1024, false, 0};
-  return run_host(bufs, n, 1u << 16, 1u << 14, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return launch_dil_poly_op(op, (uint32_t*)d[0], (const uint32_t*)d[1], (const uint32_t*)d[2], cnt, st);
+  if (!binary) b = nullptr;
+  Batch bt{"cb200_dil_poly_op", n, out, 1u << 16, 1u << 14,
+           {{out, 1024, 1024, kOut}, {a, 1024, 1024, kIn}, {b, 1024, 1024, kIn}},
+           {{!aligned({out, a, b}, {}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  return run_batch(bt, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return launch_dil_poly_op(op, (uint32_t*)r[0].p, (const uint32_t*)r[1].p, (const uint32_t*)r[2].p, cnt, st);
   });
 }
 
@@ -343,25 +307,10 @@ int cb200_dil_exceeds(const uint32_t* polys, uint32_t bound, uint8_t* flags, siz
     set_error("cb200_dil_exceeds: null pointer");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(polys);
-  if (dev != is_device_ptr(flags)) {
-    set_error("cb200_dil_exceeds: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if ((uintptr_t)polys & 15) {
-      set_error("cb200_dil_exceeds: device polynomials must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(polys);
-    if (call.rc) return call.rc;
-    return launch_dil_exceeds(polys, bound, n, flags, call.st);
-  }
-  std::vector<Buf> bufs(2);
-  bufs[0] = Buf{polys, nullptr, 1024, false, 0};
-  bufs[1] = Buf{nullptr, flags, 1, false, 0};
-  return run_host(bufs, n, 1u << 16, 1u << 14, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return launch_dil_exceeds((const uint32_t*)d[0], bound, cnt, (uint8_t*)d[1], st);
+  Batch b{"cb200_dil_exceeds", n, polys, 1u << 16, 1u << 14, {{polys, 1024, 1024, kIn}, {flags, 1, 1, kOut}},
+          {{!aligned({polys}, {}, 16), "%s: device polynomials must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return launch_dil_exceeds((const uint32_t*)r[0].p, bound, cnt, r[1].p, st);
   });
 }
 
@@ -373,24 +322,11 @@ int cb200_dil_power2round(uint32_t* a0plusq, uint32_t* a1, const uint32_t* a, si
     set_error("cb200_dil_power2round: null pointer");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(a);
-  if (dev != is_device_ptr(a0plusq) || dev != is_device_ptr(a1)) {
-    set_error("cb200_dil_power2round: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (((uintptr_t)a0plusq | (uintptr_t)a1 | (uintptr_t)a) & 15) {
-      set_error("cb200_dil_power2round: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(a);
-    if (call.rc) return call.rc;
-    return launch_dil_power2round(a0plusq, a1, a, n, call.st);
-  }
-  std::vector<Buf> bufs = {Buf{a, nullptr, 1024, false, 0}, Buf{nullptr, a0plusq, 1024, false, 0},
-                           Buf{nullptr, a1, 1024, false, 0}};
-  return run_host(bufs, n, 1u << 16, 1u << 14, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return launch_dil_power2round((uint32_t*)d[1], (uint32_t*)d[2], (const uint32_t*)d[0], cnt, st);
+  Batch b{"cb200_dil_power2round", n, a, 1u << 16, 1u << 14,
+          {{a, 1024, 1024, kIn}, {a0plusq, 1024, 1024, kOut}, {a1, 1024, 1024, kOut}},
+          {{!aligned({a0plusq, a1, a}, {}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return launch_dil_power2round((uint32_t*)r[1].p, (uint32_t*)r[2].p, (const uint32_t*)r[0].p, cnt, st);
   });
 }
 
@@ -402,23 +338,11 @@ int cb200_dil_pack_le16(uint8_t* out, const uint32_t* polys, size_t n) {
     set_error("cb200_dil_pack_le16: null pointer");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(out);
-  if (dev != is_device_ptr(polys)) {
-    set_error("cb200_dil_pack_le16: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (((uintptr_t)out & 3) || ((uintptr_t)polys & 15)) {
-      set_error("cb200_dil_pack_le16: device buffers must be aligned (polynomials 16, output 4 bytes)");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(out);
-    if (call.rc) return call.rc;
-    return launch_dil_pack_le16(out, polys, n, call.st);
-  }
-  std::vector<Buf> bufs = {Buf{polys, nullptr, 1024, false, 0}, Buf{nullptr, out, 128, false, 0}};
-  return run_host(bufs, n, 1u << 16, 1u << 14, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return launch_dil_pack_le16((uint8_t*)d[1], (const uint32_t*)d[0], cnt, st);
+  Batch b{"cb200_dil_pack_le16", n, out, 1u << 16, 1u << 14, {{polys, 1024, 1024, kIn}, {out, 128, 128, kOut}},
+          {{!aligned({out}, {}, 4) || !aligned({polys}, {}, 16),
+            "%s: device buffers must be aligned (polynomials 16, output 4 bytes)"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return launch_dil_pack_le16(r[1].p, (const uint32_t*)r[0].p, cnt, st);
   });
 }
 

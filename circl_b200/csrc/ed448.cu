@@ -26,7 +26,6 @@ int init_ed448_table(Dev& c) {  // device c.device is current
 }
 
 namespace ed448k {
-using namespace sigio;
 
 // Rows of 57 and 114 bytes sit at any byte offset (every row size of Ed448-Dilithium3 is odd): all row accesses are
 // byte loads and stores.
@@ -240,20 +239,9 @@ int cb200_ed448_keygen(const uint8_t* seeds, uint8_t* pk, uint8_t* sk, size_t n)
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({seeds, pk, sk}, &dev)) {
-    set_error("cb200_ed448_keygen: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    DeviceCall call(pk);
-    if (call.rc) return call.rc;
-    return keygen_dev(seeds, 57, pk, 57, sk, n, call.st);
-  }
-  std::vector<Buf> bufs = {Buf{seeds, nullptr, 57, false, 0}, Buf{nullptr, pk, 57, false, 0}};
-  if (sk) bufs.push_back(Buf{nullptr, sk, 114, false, 0});
-  return run_host(bufs, n, 1u << 16, 1u << 13, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return keygen_dev((const uint8_t*)d[0], 57, (uint8_t*)d[1], 57, sk ? (uint8_t*)d[2] : nullptr, cnt, st);
+  Batch b{"cb200_ed448_keygen", n, pk, 1u << 16, 1u << 13, {{seeds, 57, 57, kIn}, {pk, 57, 57, kOut}, {sk, 114, 114, kOut}}, {}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return keygen_dev(r[0].p, 57, r[1].p, 57, r[2].p, cnt, st);
   });
 }
 
@@ -270,29 +258,10 @@ int cb200_ed448_sign(const uint8_t* sk, size_t sk_stride, const uint8_t* msgs, c
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({sk, msgs, msg_off, sig}, &dev)) {
-    set_error("cb200_ed448_sign: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned({msg_off}, {}, 8)) {
-      set_error("cb200_ed448_sign: device msg_off must be 8-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(sig);
-    if (call.rc) return call.rc;
-    const uint8_t* dctx = nullptr;
-    if (ctxlen) {  // the context is a host pointer of at most 255 bytes: stage it
-      CB200_CUDA(cudaMemcpyAsync(call.ws->small, context, ctxlen, cudaMemcpyHostToDevice, call.st));
-      dctx = (const uint8_t*)call.ws->small;
-    }
-    return sign_dev(sk, sk_stride, 0, dctx, (int)ctxlen, msgs, msg_off, sig, 114, n, call.st);
-  }
-  std::vector<Row> rows = {Row{sk, nullptr, 114, sk_stride, sk_stride == 0}, Row{nullptr, sig, 114, 0, false}};
-  if (ctxlen) rows.push_back(Row{context, nullptr, ctxlen, 0, true});
-  return run_msgs(n, rows, msgs, msg_off, [&](uint8_t** d, const uint8_t* m, const uint64_t* o, size_t cnt, cudaStream_t st) {
-    return sign_dev(d[0], sk_stride ? 114 : 0, 0, ctxlen ? d[2] : nullptr, (int)ctxlen, m, o, d[1], 114, cnt, st);
+  Batch b{"cb200_ed448_sign", n, sig, 1u << 15, 1u << 12, {{sk, 114, sk_stride, kIn}, {sig, 114, 114, kOut}},
+          {{!aligned({msg_off}, {}, 8), "%s: device msg_off must be 8-byte aligned"}}, msgs, msg_off, context, ctxlen};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return sign_dev(r[0].p, r[0].stride, 0, r.ctx, (int)ctxlen, r.msgs, r.msg_off, r[1].p, 114, cnt, st);
   });
 }
 
@@ -305,38 +274,16 @@ int cb200_ed448_verify(const uint8_t* pk, size_t pk_stride, const uint8_t* msgs,
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({pk, msgs, msg_off, sig, ok}, &dev)) {
-    set_error("cb200_ed448_verify: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned({msg_off}, {}, 8)) {
-      set_error("cb200_ed448_verify: device msg_off must be 8-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(ok);
-    if (call.rc) return call.rc;
-    if (ctxlen > ed448::kMaxContext) {  // verify returns false
-      CB200_CUDA(cudaMemsetAsync(ok, 0, n, call.st));
+  const bool long_ctx = ctxlen > ed448::kMaxContext;  // verify returns false
+  Batch b{"cb200_ed448_verify", n, ok, 1u << 15, 1u << 12, {{pk, 57, pk_stride, kIn}, {sig, 114, 114, kIn}, {ok, 1, 1, kOut}},
+          {{!aligned({msg_off}, {}, 8), "%s: device msg_off must be 8-byte aligned"}}, msgs, msg_off, context,
+          long_ctx ? 0 : ctxlen};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) -> int {
+    if (long_ctx) {
+      CB200_CUDA(cudaMemsetAsync(r[2].p, 0, cnt, st));
       return 0;
     }
-    const uint8_t* dctx = nullptr;
-    if (ctxlen) {
-      CB200_CUDA(cudaMemcpyAsync(call.ws->small, context, ctxlen, cudaMemcpyHostToDevice, call.st));
-      dctx = (const uint8_t*)call.ws->small;
-    }
-    return verify_dev(pk, pk_stride, dctx, (int)ctxlen, msgs, msg_off, sig, 114, ok, 0, n, call.st);
-  }
-  if (ctxlen > ed448::kMaxContext) {
-    memset(ok, 0, n);
-    return 0;
-  }
-  std::vector<Row> rows = {Row{pk, nullptr, 57, pk_stride, pk_stride == 0}, Row{sig, nullptr, 114, 0, false},
-                           Row{nullptr, ok, 1, 0, false}};
-  if (ctxlen) rows.push_back(Row{context, nullptr, ctxlen, 0, true});
-  return run_msgs(n, rows, msgs, msg_off, [&](uint8_t** d, const uint8_t* m, const uint64_t* o, size_t cnt, cudaStream_t st) {
-    return verify_dev(d[0], pk_stride ? 57 : 0, ctxlen ? d[3] : nullptr, (int)ctxlen, m, o, d[1], 114, d[2], 0, cnt, st);
+    return verify_dev(r[0].p, r[0].stride, r.ctx, (int)ctxlen, r.msgs, r.msg_off, r[1].p, 114, r[2].p, 0, cnt, st);
   });
 }
 
@@ -348,20 +295,10 @@ int cb200_eddilithium3_keygen(const uint8_t* seeds, uint8_t* pk, uint8_t* sk, si
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({seeds, pk, sk}, &dev)) {
-    set_error("cb200_eddilithium3_keygen: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    DeviceCall call(pk);
-    if (call.rc) return call.rc;
-    return edd3_keygen_dev(seeds, pk, sk, n, call.st, kDevSlot);
-  }
-  std::vector<Buf> bufs = {Buf{seeds, nullptr, 57, false, 0}, Buf{nullptr, pk, kEdPk, false, 0},
-                           Buf{nullptr, sk, kEdSk, false, 0}};
-  return run_host(bufs, n, 1u << 14, 1u << 12, [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-    return edd3_keygen_dev((const uint8_t*)d[0], (uint8_t*)d[1], (uint8_t*)d[2], cnt, st, slot);
+  Batch b{"cb200_eddilithium3_keygen", n, pk, 1u << 14, 1u << 12,
+          {{seeds, 57, 57, kIn}, {pk, kEdPk, kEdPk, kOut}, {sk, kEdSk, kEdSk, kOut}}, {}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return edd3_keygen_dev(r[0].p, r[1].p, r[2].p, cnt, st, slot);
   });
 }
 
@@ -374,42 +311,18 @@ int cb200_eddilithium3_sign(const uint8_t* sk, size_t sk_stride, const uint8_t* 
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({sk, msgs, msg_off, sig, status}, &dev)) {
-    set_error("cb200_eddilithium3_sign: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned({msg_off}, {}, 16)) {
-      set_error("cb200_eddilithium3_sign: device msg_off must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    if (n >= (1u << 24)) {  // the limit of the Dilithium3 signing flow
-      set_error("cb200_eddilithium3_sign: a device-pointer batch is limited to 2^24 - 1 signatures per call (got %zu)", n);
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(sig);
-    if (call.rc) return call.rc;
-    return edd3_sign_dev(sk, sk_stride, msgs, msg_off, sig, status, n, call.st, kDevSlot);
-  }
-  std::vector<uint8_t> own;
-  if (!status) {
-    own.resize(n);
-    status = own.data();
-  }
-  std::vector<Row> rows = {Row{sk, nullptr, kEdSk, sk_stride, sk_stride == 0}, Row{nullptr, sig, kEdSig, 0, false},
-                           Row{nullptr, status, 1, 0, false}};
-  rc = run_msgs(n, rows, msgs, msg_off, [&](uint8_t** d, const uint8_t* m, const uint64_t* o, size_t cnt, cudaStream_t st) {
-    return edd3_sign_dev(d[0], sk_stride ? kEdSk : 0, m, o, d[1], d[2], cnt, st, 0);
-  });
+  Batch b{"cb200_eddilithium3_sign", n, sig, 1u << 15, 1u << 12,
+          {{sk, kEdSk, sk_stride, kIn}, {sig, kEdSig, kEdSig, kOut}, {status, 1, 1, kStatus}},
+          {{!aligned({msg_off}, {}, 16), "%s: device msg_off must be 16-byte aligned"},
+           // the limit of the Dilithium3 signing flow
+           {n >= (1u << 24), "%s: a device-pointer batch is limited to 2^24 - 1 signatures per call (got %zu)"}},
+          msgs, msg_off};
+  Counts c;
+  rc = run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return edd3_sign_dev(r[0].p, r[0].stride, r.msgs, r.msg_off, r[1].p, r[2].p, cnt, st, slot);
+  }, &c);
   if (rc) return rc;
-  size_t bad = 0;
-  for (size_t i = 0; i < n; i++) bad += status[i] != 0;
-  if (bad) {
-    set_error("cb200_eddilithium3_sign: %zu of %zu signatures exhausted 576 attempts", bad, n);
-    return CB200_ERR_SIGN_ATTEMPTS;
-  }
-  return 0;
+  return sign_attempts_result("cb200_eddilithium3_sign", c.nonzero, n);
 }
 
 int cb200_eddilithium3_verify(const uint8_t* pk, size_t pk_stride, const uint8_t* msgs, const uint64_t* msg_off,
@@ -421,24 +334,11 @@ int cb200_eddilithium3_verify(const uint8_t* pk, size_t pk_stride, const uint8_t
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({pk, msgs, msg_off, sig, ok}, &dev)) {
-    set_error("cb200_eddilithium3_verify: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned({msg_off}, {}, 16)) {
-      set_error("cb200_eddilithium3_verify: device msg_off must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(ok);
-    if (call.rc) return call.rc;
-    return edd3_verify_dev(pk, pk_stride, msgs, msg_off, sig, ok, n, call.st, kDevSlot);
-  }
-  std::vector<Row> rows = {Row{pk, nullptr, kEdPk, pk_stride, pk_stride == 0}, Row{sig, nullptr, kEdSig, 0, false},
-                           Row{nullptr, ok, 1, 0, false}};
-  return run_msgs(n, rows, msgs, msg_off, [&](uint8_t** d, const uint8_t* m, const uint64_t* o, size_t cnt, cudaStream_t st) {
-    return edd3_verify_dev(d[0], pk_stride ? kEdPk : 0, m, o, d[1], d[2], cnt, st, 0);
+  Batch b{"cb200_eddilithium3_verify", n, ok, 1u << 15, 1u << 12,
+          {{pk, kEdPk, pk_stride, kIn}, {sig, kEdSig, kEdSig, kIn}, {ok, 1, 1, kOut}},
+          {{!aligned({msg_off}, {}, 16), "%s: device msg_off must be 16-byte aligned"}}, msgs, msg_off};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return edd3_verify_dev(r[0].p, r[0].stride, r.msgs, r.msg_off, r[1].p, r[2].p, cnt, st, slot);
   });
 }
 

@@ -16,7 +16,6 @@
 
 namespace cb200 {
 namespace eddsa {
-using namespace sigio;
 
 template <int N>
 __device__ __forceinline__ void ldw(uint32_t (&w)[N], const uint8_t* p) {
@@ -195,24 +194,10 @@ int cb200_ed25519_keygen(const uint8_t* seeds, uint8_t* pk, uint8_t* sk, size_t 
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({seeds, pk, sk}, &dev)) {
-    set_error("cb200_ed25519_keygen: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned({seeds, pk, sk}, {}, 4)) {
-      set_error("cb200_ed25519_keygen: device buffers must be 4-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(pk);
-    if (call.rc) return call.rc;
-    return ed_keygen_dev(seeds, 32, pk, 32, sk, n, call.st);
-  }
-  std::vector<Buf> bufs = {Buf{seeds, nullptr, 32, false, 0}, Buf{nullptr, pk, 32, false, 0}};
-  if (sk) bufs.push_back(Buf{nullptr, sk, 64, false, 0});
-  return run_host(bufs, n, 1u << 16, 1u << 13, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return ed_keygen_dev((const uint8_t*)d[0], 32, (uint8_t*)d[1], 32, sk ? (uint8_t*)d[2] : nullptr, cnt, st);
+  Batch b{"cb200_ed25519_keygen", n, pk, 1u << 16, 1u << 13, {{seeds, 32, 32, kIn}, {pk, 32, 32, kOut}, {sk, 64, 64, kOut}},
+          {{!aligned({seeds, pk, sk}, {}, 4), "%s: device buffers must be 4-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return ed_keygen_dev(r[0].p, 32, r[1].p, 32, r[2].p, cnt, st);
   });
 }
 
@@ -225,23 +210,12 @@ int cb200_ed25519_sign(const uint8_t* sk, size_t sk_stride, const uint8_t* msgs,
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({sk, msgs, msg_off, sig}, &dev)) {
-    set_error("cb200_ed25519_sign: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned({sk, sig}, {sk_stride}, 4) || !aligned({msg_off}, {}, 8)) {
-      set_error("cb200_ed25519_sign: device sk, sk_stride and sig must be 4-byte aligned, msg_off 8-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(sig);
-    if (call.rc) return call.rc;
-    return ed_sign_dev(sk, sk_stride, 0, msgs, msg_off, sig, 64, n, call.st);
-  }
-  std::vector<Row> rows = {Row{sk, nullptr, 64, sk_stride, sk_stride == 0}, Row{nullptr, sig, 64, 0, false}};
-  return run_msgs(n, rows, msgs, msg_off, [&](uint8_t** d, const uint8_t* m, const uint64_t* o, size_t cnt, cudaStream_t st) {
-    return ed_sign_dev(d[0], sk_stride ? 64 : 0, 0, m, o, d[1], 64, cnt, st);
+  Batch b{"cb200_ed25519_sign", n, sig, 1u << 15, 1u << 12, {{sk, 64, sk_stride, kIn}, {sig, 64, 64, kOut}},
+          {{!aligned({sk, sig}, {sk_stride}, 4) || !aligned({msg_off}, {}, 8),
+            "%s: device sk, sk_stride and sig must be 4-byte aligned, msg_off 8-byte aligned"}},
+          msgs, msg_off};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return ed_sign_dev(r[0].p, r[0].stride, 0, r.msgs, r.msg_off, r[1].p, 64, cnt, st);
   });
 }
 
@@ -254,24 +228,13 @@ int cb200_ed25519_verify(const uint8_t* pk, size_t pk_stride, const uint8_t* msg
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({pk, msgs, msg_off, sig, ok}, &dev)) {
-    set_error("cb200_ed25519_verify: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned({pk, sig}, {pk_stride}, 4) || !aligned({msg_off}, {}, 8)) {
-      set_error("cb200_ed25519_verify: device pk, pk_stride and sig must be 4-byte aligned, msg_off 8-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(ok);
-    if (call.rc) return call.rc;
-    return ed_verify_dev(pk, pk_stride, msgs, msg_off, sig, 64, ok, 0, n, call.st);
-  }
-  std::vector<Row> rows = {Row{pk, nullptr, 32, pk_stride, pk_stride == 0}, Row{sig, nullptr, 64, 0, false},
-                           Row{nullptr, ok, 1, 0, false}};
-  return run_msgs(n, rows, msgs, msg_off, [&](uint8_t** d, const uint8_t* m, const uint64_t* o, size_t cnt, cudaStream_t st) {
-    return ed_verify_dev(d[0], pk_stride ? 32 : 0, m, o, d[1], 64, d[2], 0, cnt, st);
+  Batch b{"cb200_ed25519_verify", n, ok, 1u << 15, 1u << 12,
+          {{pk, 32, pk_stride, kIn}, {sig, 64, 64, kIn}, {ok, 1, 1, kOut}},
+          {{!aligned({pk, sig}, {pk_stride}, 4) || !aligned({msg_off}, {}, 8),
+            "%s: device pk, pk_stride and sig must be 4-byte aligned, msg_off 8-byte aligned"}},
+          msgs, msg_off};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return ed_verify_dev(r[0].p, r[0].stride, r.msgs, r.msg_off, r[1].p, 64, r[2].p, 0, cnt, st);
   });
 }
 
@@ -283,24 +246,11 @@ int cb200_eddilithium2_keygen(const uint8_t* seeds, uint8_t* pk, uint8_t* sk, si
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({seeds, pk, sk}, &dev)) {
-    set_error("cb200_eddilithium2_keygen: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned({seeds, pk, sk}, {}, 16)) {
-      set_error("cb200_eddilithium2_keygen: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(pk);
-    if (call.rc) return call.rc;
-    return edd2_keygen_dev(seeds, pk, sk, n, call.st, kDevSlot);
-  }
-  std::vector<Buf> bufs = {Buf{seeds, nullptr, 32, false, 0}, Buf{nullptr, pk, kEdPk, false, 0},
-                           Buf{nullptr, sk, kEdSk, false, 0}};
-  return run_host(bufs, n, 1u << 14, 1u << 12, [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-    return edd2_keygen_dev((const uint8_t*)d[0], (uint8_t*)d[1], (uint8_t*)d[2], cnt, st, slot);
+  Batch b{"cb200_eddilithium2_keygen", n, pk, 1u << 14, 1u << 12,
+          {{seeds, 32, 32, kIn}, {pk, kEdPk, kEdPk, kOut}, {sk, kEdSk, kEdSk, kOut}},
+          {{!aligned({seeds, pk, sk}, {}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return edd2_keygen_dev(r[0].p, r[1].p, r[2].p, cnt, st, slot);
   });
 }
 
@@ -313,42 +263,19 @@ int cb200_eddilithium2_sign(const uint8_t* sk, size_t sk_stride, const uint8_t* 
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({sk, msgs, msg_off, sig, status}, &dev)) {
-    set_error("cb200_eddilithium2_sign: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned({sk, msg_off}, {sk_stride}, 16) || !aligned({sig}, {}, 4)) {
-      set_error("cb200_eddilithium2_sign: device sk, sk_stride and msg_off must be 16-byte aligned, sig 4-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    if (n >= (1u << 24)) {  // the limit of the Dilithium2 signing flow
-      set_error("cb200_eddilithium2_sign: a device-pointer batch is limited to 2^24 - 1 signatures per call (got %zu)", n);
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(sig);
-    if (call.rc) return call.rc;
-    return edd2_sign_dev(sk, sk_stride, msgs, msg_off, sig, status, n, call.st, kDevSlot);
-  }
-  std::vector<uint8_t> own;
-  if (!status) {
-    own.resize(n);
-    status = own.data();
-  }
-  std::vector<Row> rows = {Row{sk, nullptr, kEdSk, sk_stride, sk_stride == 0}, Row{nullptr, sig, kEdSig, 0, false},
-                           Row{nullptr, status, 1, 0, false}};
-  rc = run_msgs(n, rows, msgs, msg_off, [&](uint8_t** d, const uint8_t* m, const uint64_t* o, size_t cnt, cudaStream_t st) {
-    return edd2_sign_dev(d[0], sk_stride ? kEdSk : 0, m, o, d[1], d[2], cnt, st, 0);
-  });
+  Batch b{"cb200_eddilithium2_sign", n, sig, 1u << 15, 1u << 12,
+          {{sk, kEdSk, sk_stride, kIn}, {sig, kEdSig, kEdSig, kOut}, {status, 1, 1, kStatus}},
+          {{!aligned({sk, msg_off}, {sk_stride}, 16) || !aligned({sig}, {}, 4),
+            "%s: device sk, sk_stride and msg_off must be 16-byte aligned, sig 4-byte aligned"},
+           // the limit of the Dilithium2 signing flow
+           {n >= (1u << 24), "%s: a device-pointer batch is limited to 2^24 - 1 signatures per call (got %zu)"}},
+          msgs, msg_off};
+  Counts c;
+  rc = run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return edd2_sign_dev(r[0].p, r[0].stride, r.msgs, r.msg_off, r[1].p, r[2].p, cnt, st, slot);
+  }, &c);
   if (rc) return rc;
-  size_t bad = 0;
-  for (size_t i = 0; i < n; i++) bad += status[i] != 0;
-  if (bad) {
-    set_error("cb200_eddilithium2_sign: %zu of %zu signatures exhausted 576 attempts", bad, n);
-    return CB200_ERR_SIGN_ATTEMPTS;
-  }
-  return 0;
+  return sign_attempts_result("cb200_eddilithium2_sign", c.nonzero, n);
 }
 
 int cb200_eddilithium2_verify(const uint8_t* pk, size_t pk_stride, const uint8_t* msgs, const uint64_t* msg_off,
@@ -360,24 +287,13 @@ int cb200_eddilithium2_verify(const uint8_t* pk, size_t pk_stride, const uint8_t
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({pk, msgs, msg_off, sig, ok}, &dev)) {
-    set_error("cb200_eddilithium2_verify: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned({pk, msg_off}, {pk_stride}, 16) || !aligned({sig}, {}, 4)) {
-      set_error("cb200_eddilithium2_verify: device pk, pk_stride and msg_off must be 16-byte aligned, sig 4-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(ok);
-    if (call.rc) return call.rc;
-    return edd2_verify_dev(pk, pk_stride, msgs, msg_off, sig, ok, n, call.st, kDevSlot);
-  }
-  std::vector<Row> rows = {Row{pk, nullptr, kEdPk, pk_stride, pk_stride == 0}, Row{sig, nullptr, kEdSig, 0, false},
-                           Row{nullptr, ok, 1, 0, false}};
-  return run_msgs(n, rows, msgs, msg_off, [&](uint8_t** d, const uint8_t* m, const uint64_t* o, size_t cnt, cudaStream_t st) {
-    return edd2_verify_dev(d[0], pk_stride ? kEdPk : 0, m, o, d[1], d[2], cnt, st, 0);
+  Batch b{"cb200_eddilithium2_verify", n, ok, 1u << 15, 1u << 12,
+          {{pk, kEdPk, pk_stride, kIn}, {sig, kEdSig, kEdSig, kIn}, {ok, 1, 1, kOut}},
+          {{!aligned({pk, msg_off}, {pk_stride}, 16) || !aligned({sig}, {}, 4),
+            "%s: device pk, pk_stride and msg_off must be 16-byte aligned, sig 4-byte aligned"}},
+          msgs, msg_off};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return edd2_verify_dev(r[0].p, r[0].stride, r.msgs, r.msg_off, r[1].p, r[2].p, cnt, st, slot);
   });
 }
 

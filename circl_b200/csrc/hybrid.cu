@@ -418,21 +418,6 @@ static int hybrid448_decaps_dev(const Hyb& H, const uint8_t* sk, size_t sk_strid
   return 0;
 }
 
-// Every buffer of a call lives on the same side.  Host calls go through the staging pipeline in chunks.
-static bool same_side(std::initializer_list<const void*> ps, bool* dev) {
-  bool first = true;
-  for (const void* p : ps) {
-    if (!p) continue;
-    const bool d = is_device_ptr(p);
-    if (first) {
-      *dev = d;
-      first = false;
-    } else if (d != *dev) {
-      return false;
-    }
-  }
-  return true;
-}
 // the first error class found among the per-op status bytes of a host-pointer call (counted by HostCall)
 static int status_result(size_t pub, size_t priv, size_t n, const char* fn) {
   if (pub) {
@@ -445,19 +430,37 @@ static int status_result(size_t pub, size_t priv, size_t n, const char* fn) {
   }
   return 0;
 }
-// device-pointer calls read their buffers with 32-, 64- and 128-bit accesses
-static bool aligned16(std::initializer_list<const void*> ps, std::initializer_list<size_t> strides) {
-  uintptr_t acc = 0;
-  for (const void* p : ps) acc |= (uintptr_t)p;
-  for (size_t v : strides) acc |= v;
-  return (acc & 15) == 0;
+// Device-pointer calls read their buffers with 32-, 64- and 128-bit accesses; the X448 entry points and hybrids read
+// and write their rows in 32- and 64-bit units.
+static const char* align_text(size_t xs) {
+  return xs == 56 ? "%s: device buffers must be 8-byte aligned" : "%s: device buffers must be 16-byte aligned";
 }
-// the X448 entry points and hybrids read and write their rows in 32- and 64-bit units
-static bool aligned8(std::initializer_list<const void*> ps, std::initializer_list<size_t> strides) {
-  uintptr_t acc = 0;
-  for (const void* p : ps) acc |= (uintptr_t)p;
-  for (size_t v : strides) acc |= v;
-  return (acc & 7) == 0;
+
+// cb200_x25519 and cb200_x448: w = 32 or 56 bytes per scalar, point and output
+static int x_entry(const char* fn, size_t w, const uint8_t* scalars, const uint8_t* points, uint8_t* out, uint8_t* status,
+                   size_t n) {
+  int rc = require_ready();
+  if (rc) return rc;
+  if (!scalars || !out) {
+    set_error("%s: null pointer", fn);
+    return CB200_ERR_ARG;
+  }
+  if (n == 0) return 0;
+  Batch b{fn, n, out, 1u << 17, 1u << 14,
+          {{scalars, w, w, kIn}, {out, w, w, kOut}, {status, 1, 1, kStatus}, {points, w, w, kIn}},
+          {{!aligned({scalars, points, out}, {}, w == 56 ? 8 : 16), align_text(w)}}};
+  Counts c;
+  rc = run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) -> int {
+    if (r[2].p) CB200_CUDA(cudaMemsetAsync(r[2].p, 0, cnt, st));
+    if (w == 56)
+      x448_launch(r[0].p, w, r[3].p, w, r[1].p, w, r[2].p, cnt, st);
+    else
+      x25519_launch(r[0].p, w, r[3].p, w, r[1].p, w, r[2].p, cnt, st);
+    CB200_CUDA(cudaGetLastError());
+    return 0;
+  }, &c);
+  if (rc) return rc;
+  return status_result(c.bit0, c.bit1, n, fn);
 }
 
 }  // namespace hybrid
@@ -469,91 +472,11 @@ using namespace cb200::hybrid;
 extern "C" {
 
 int cb200_x25519(const uint8_t* scalars, const uint8_t* points, uint8_t* out, uint8_t* status, size_t n) {
-  int rc = require_ready();
-  if (rc) return rc;
-  if (!scalars || !out) {
-    set_error("cb200_x25519: null pointer");
-    return CB200_ERR_ARG;
-  }
-  if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({scalars, points, out, status}, &dev)) {
-    set_error("cb200_x25519: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned16({scalars, points, out}, {})) {
-      set_error("cb200_x25519: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(out);
-    if (call.rc) return call.rc;
-    if (status) CB200_CUDA(cudaMemsetAsync(status, 0, n, call.st));
-    x25519_launch(scalars, 32, points, 32, out, 32, status, n, call.st);
-    CB200_CUDA(cudaGetLastError());
-    return 0;
-  }
-  HostCall hc;
-  hc.bufs = {Buf{scalars, nullptr, 32, false, 0}, Buf{nullptr, out, 32, false, 0}, Buf{nullptr, nullptr, 1, false, 0}};
-  if (points) hc.bufs.push_back(Buf{points, nullptr, 32, false, 0});
-  hc.chunk = 1u << 17;
-  hc.min_shard = 1u << 14;
-  hc.status_buf = 2;
-  hc.user_status = status;
-  hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int) -> int {
-    CB200_CUDA(cudaMemsetAsync(d[2], 0, cnt, st));
-    x25519_launch((const uint8_t*)d[0], 32, points ? (const uint8_t*)d[3] : nullptr, 32, (uint8_t*)d[1], 32, (uint8_t*)d[2],
-                  cnt, st);
-    CB200_CUDA(cudaGetLastError());
-    return 0;
-  };
-  rc = hc.run(n);
-  if (rc) return rc;
-  return status_result(hc.bit0, hc.bit1, n, "cb200_x25519");
+  return x_entry("cb200_x25519", 32, scalars, points, out, status, n);
 }
 
 int cb200_x448(const uint8_t* scalars, const uint8_t* points, uint8_t* out, uint8_t* status, size_t n) {
-  int rc = require_ready();
-  if (rc) return rc;
-  if (!scalars || !out) {
-    set_error("cb200_x448: null pointer");
-    return CB200_ERR_ARG;
-  }
-  if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({scalars, points, out, status}, &dev)) {
-    set_error("cb200_x448: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned8({scalars, points, out}, {})) {
-      set_error("cb200_x448: device buffers must be 8-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(out);
-    if (call.rc) return call.rc;
-    if (status) CB200_CUDA(cudaMemsetAsync(status, 0, n, call.st));
-    x448_launch(scalars, 56, points, 56, out, 56, status, n, call.st);
-    CB200_CUDA(cudaGetLastError());
-    return 0;
-  }
-  HostCall hc;
-  hc.bufs = {Buf{scalars, nullptr, 56, false, 0}, Buf{nullptr, out, 56, false, 0}, Buf{nullptr, nullptr, 1, false, 0}};
-  if (points) hc.bufs.push_back(Buf{points, nullptr, 56, false, 0});
-  hc.chunk = 1u << 17;
-  hc.min_shard = 1u << 14;
-  hc.status_buf = 2;
-  hc.user_status = status;
-  hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int) -> int {
-    CB200_CUDA(cudaMemsetAsync(d[2], 0, cnt, st));
-    x448_launch((const uint8_t*)d[0], 56, points ? (const uint8_t*)d[3] : nullptr, 56, (uint8_t*)d[1], 56, (uint8_t*)d[2],
-                cnt, st);
-    CB200_CUDA(cudaGetLastError());
-    return 0;
-  };
-  rc = hc.run(n);
-  if (rc) return rc;
-  return status_result(hc.bit0, hc.bit1, n, "cb200_x448");
+  return x_entry("cb200_x448", 56, scalars, points, out, status, n);
 }
 
 int cb200_xwing_keygen(const uint8_t* seeds, uint8_t* pk, size_t n) {
@@ -564,23 +487,10 @@ int cb200_xwing_keygen(const uint8_t* seeds, uint8_t* pk, size_t n) {
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({seeds, pk}, &dev)) {
-    set_error("cb200_xwing_keygen: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned16({seeds, pk}, {})) {
-      set_error("cb200_xwing_keygen: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(pk);
-    if (call.rc) return call.rc;
-    return xwing_keygen_dev(seeds, pk, n, call.st, kDevSlot);
-  }
-  std::vector<Buf> bufs = {Buf{seeds, nullptr, 32, false, 0}, Buf{nullptr, pk, 1216, false, 0}};
-  return run_host(bufs, n, 1u << 15, 1u << 13, [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-    return xwing_keygen_dev((const uint8_t*)d[0], (uint8_t*)d[1], cnt, st, slot);
+  Batch b{"cb200_xwing_keygen", n, pk, 1u << 15, 1u << 13, {{seeds, 32, 32, kIn}, {pk, 1216, 1216, kOut}},
+          {{!aligned({seeds, pk}, {}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return xwing_keygen_dev(r[0].p, r[1].p, cnt, st, slot);
   });
 }
 
@@ -593,34 +503,16 @@ int cb200_xwing_encaps(const uint8_t* pk, size_t pk_stride, const uint8_t* eseed
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({pk, eseeds, ct, ss, status}, &dev)) {
-    set_error("cb200_xwing_encaps: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned16({pk, eseeds, ct, ss}, {pk_stride})) {
-      set_error("cb200_xwing_encaps: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(ct);
-    if (call.rc) return call.rc;
-    return xwing_encaps_dev(pk, pk_stride, eseeds, ct, ss, status, n, call.st, kDevSlot);
-  }
-  HostCall hc;
-  hc.bufs = {Buf{pk, nullptr, 1216, pk_stride == 0, pk_stride}, Buf{eseeds, nullptr, 64, false, 0},
-             Buf{nullptr, ct, 1120, false, 0}, Buf{nullptr, ss, 32, false, 0}, Buf{nullptr, nullptr, 1, false, 0}};
-  hc.chunk = 1u << 15;
-  hc.min_shard = 1u << 13;
-  hc.status_buf = 4;
-  hc.user_status = status;
-  hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-    return xwing_encaps_dev((const uint8_t*)d[0], pk_stride == 0 ? 0 : 1216, (const uint8_t*)d[1], (uint8_t*)d[2],
-                            (uint8_t*)d[3], (uint8_t*)d[4], cnt, st, slot);
-  };
-  rc = hc.run(n);
+  Batch b{"cb200_xwing_encaps", n, ct, 1u << 15, 1u << 13,
+          {{pk, 1216, pk_stride, kIn}, {eseeds, 64, 64, kIn}, {ct, 1120, 1120, kOut}, {ss, 32, 32, kOut},
+           {status, 1, 1, kStatus}},
+          {{!aligned({pk, eseeds, ct, ss}, {pk_stride}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  Counts c;
+  rc = run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return xwing_encaps_dev(r[0].p, r[0].stride, r[1].p, r[2].p, r[3].p, r[4].p, cnt, st, slot);
+  }, &c);
   if (rc) return rc;
-  return status_result(hc.bit0, hc.bit1, n, "cb200_xwing_encaps");
+  return status_result(c.bit0, c.bit1, n, "cb200_xwing_encaps");
 }
 
 int cb200_xwing_decaps(const uint8_t* sk, size_t sk_stride, const uint8_t* ct, uint8_t* ss, size_t n) {
@@ -631,24 +523,11 @@ int cb200_xwing_decaps(const uint8_t* sk, size_t sk_stride, const uint8_t* ct, u
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({sk, ct, ss}, &dev)) {
-    set_error("cb200_xwing_decaps: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!aligned16({sk, ct, ss}, {sk_stride})) {
-      set_error("cb200_xwing_decaps: device buffers and sk_stride must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(ss);
-    if (call.rc) return call.rc;
-    return xwing_decaps_dev(sk, sk_stride, ct, ss, n, call.st, kDevSlot);
-  }
-  std::vector<Buf> bufs = {Buf{sk, nullptr, 32, sk_stride == 0, sk_stride}, Buf{ct, nullptr, 1120, false, 0},
-                           Buf{nullptr, ss, 32, false, 0}};
-  return run_host(bufs, n, 1u << 15, 1u << 13, [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-    return xwing_decaps_dev((const uint8_t*)d[0], sk_stride == 0 ? 0 : 32, (const uint8_t*)d[1], (uint8_t*)d[2], cnt, st, slot);
+  Batch b{"cb200_xwing_decaps", n, ss, 1u << 15, 1u << 13,
+          {{sk, 32, sk_stride, kIn}, {ct, 1120, 1120, kIn}, {ss, 32, 32, kOut}},
+          {{!aligned({sk, ct, ss}, {sk_stride}, 16), "%s: device buffers and sk_stride must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return xwing_decaps_dev(r[0].p, r[0].stride, r[1].p, r[2].p, cnt, st, slot);
   });
 }
 
@@ -686,40 +565,12 @@ int cb200_hybrid_keygen(int id, const uint8_t* seeds, uint8_t* pk, uint8_t* sk, 
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({seeds, pk, sk}, &dev)) {
-    set_error("cb200_hybrid_keygen: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (H.xs == 56) {
-    if (dev) {
-      if (!aligned8({seeds, pk, sk}, {})) {
-        set_error("cb200_hybrid_keygen: device buffers must be 8-byte aligned");
-        return CB200_ERR_ARG;
-      }
-      DeviceCall call(pk);
-      if (call.rc) return call.rc;
-      return hybrid448_keygen_dev(H, seeds, pk, sk, n, call.st, kDevSlot);
-    }
-    std::vector<Buf> bufs = {Buf{seeds, nullptr, 64, false, 0}, Buf{nullptr, pk, H.ek + 56, false, 0},
-                             Buf{nullptr, sk, H.dk + 56, false, 0}};
-    return run_host(bufs, n, 1u << 15, 1u << 13, [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-      return hybrid448_keygen_dev(H, (const uint8_t*)d[0], (uint8_t*)d[1], (uint8_t*)d[2], cnt, st, slot);
-    });
-  }
-  if (dev) {
-    if (!aligned16({seeds, pk, sk}, {})) {
-      set_error("cb200_hybrid_keygen: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(pk);
-    if (call.rc) return call.rc;
-    return hybrid_keygen_dev(H, seeds, pk, sk, n, call.st, kDevSlot);
-  }
-  std::vector<Buf> bufs = {Buf{seeds, nullptr, 64, false, 0}, Buf{nullptr, pk, H.ek + 32, false, 0},
-                           Buf{nullptr, sk, H.dk + 32, false, 0}};
-  return run_host(bufs, n, 1u << 15, 1u << 13, [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-    return hybrid_keygen_dev(H, (const uint8_t*)d[0], (uint8_t*)d[1], (uint8_t*)d[2], cnt, st, slot);
+  const size_t pks = H.ek + H.xs, sks = H.dk + H.xs;
+  Batch b{"cb200_hybrid_keygen", n, pk, 1u << 15, 1u << 13, {{seeds, 64, 64, kIn}, {pk, pks, pks, kOut}, {sk, sks, sks, kOut}},
+          {{!aligned({seeds, pk, sk}, {}, H.xs == 56 ? 8 : 16), align_text(H.xs)}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return H.xs == 56 ? hybrid448_keygen_dev(H, r[0].p, r[1].p, r[2].p, cnt, st, slot)
+                      : hybrid_keygen_dev(H, r[0].p, r[1].p, r[2].p, cnt, st, slot);
   });
 }
 
@@ -735,65 +586,19 @@ int cb200_hybrid_encaps(int id, const uint8_t* pk, size_t pk_stride, const uint8
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({pk, seeds, ct, ss, status}, &dev)) {
-    set_error("cb200_hybrid_encaps: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!status) {
-      set_error("cb200_hybrid_encaps: device-pointer calls need a status array (it carries kem.ErrPubKey)");
-      return CB200_ERR_ARG;
-    }
-    if (H.xs == 56) {
-      if (!aligned8({pk, seeds, ct, ss}, {pk_stride})) {
-        set_error("cb200_hybrid_encaps: device buffers must be 8-byte aligned");
-        return CB200_ERR_ARG;
-      }
-      DeviceCall call(ct);
-      if (call.rc) return call.rc;
-      return hybrid448_encaps_dev(H, pk, pk_stride, seeds, ct, ss, status, n, call.st, kDevSlot);
-    }
-    if (!aligned16({pk, seeds, ct, ss}, {pk_stride})) {
-      set_error("cb200_hybrid_encaps: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(ct);
-    if (call.rc) return call.rc;
-    return hybrid_encaps_dev(H, pk, pk_stride, seeds, ct, ss, status, n, call.st, kDevSlot);
-  }
-  if (H.xs == 56) {
-    const size_t pks = H.ek + 56;
-    HostCall hc;
-    hc.bufs = {Buf{pk, nullptr, pks, pk_stride == 0, pk_stride}, Buf{seeds, nullptr, 56, false, 0},
-               Buf{nullptr, ct, H.ct + 56, false, 0}, Buf{nullptr, ss, 88, false, 0}, Buf{nullptr, nullptr, 1, false, 0}};
-    hc.chunk = 1u << 15;
-    hc.min_shard = 1u << 13;
-    hc.status_buf = 4;
-    hc.user_status = status;
-    hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-      return hybrid448_encaps_dev(H, (const uint8_t*)d[0], pk_stride == 0 ? 0 : pks, (const uint8_t*)d[1], (uint8_t*)d[2],
-                                  (uint8_t*)d[3], (uint8_t*)d[4], cnt, st, slot);
-    };
-    rc = hc.run(n);
-    if (rc) return rc;
-    return status_result(hc.bit0, hc.bit1, n, "cb200_hybrid_encaps");
-  }
-  const size_t pks = H.ek + 32;
-  HostCall hc;
-  hc.bufs = {Buf{pk, nullptr, pks, pk_stride == 0, pk_stride}, Buf{seeds, nullptr, 32, false, 0},
-             Buf{nullptr, ct, H.ct + 32, false, 0}, Buf{nullptr, ss, 64, false, 0}, Buf{nullptr, nullptr, 1, false, 0}};
-  hc.chunk = 1u << 15;
-  hc.min_shard = 1u << 13;
-  hc.status_buf = 4;
-  hc.user_status = status;
-  hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-    return hybrid_encaps_dev(H, (const uint8_t*)d[0], pk_stride == 0 ? 0 : pks, (const uint8_t*)d[1], (uint8_t*)d[2],
-                             (uint8_t*)d[3], (uint8_t*)d[4], cnt, st, slot);
-  };
-  rc = hc.run(n);
+  const size_t pks = H.ek + H.xs, cts = H.ct + H.xs, sss = 32 + H.xs;
+  Batch b{"cb200_hybrid_encaps", n, ct, 1u << 15, 1u << 13,
+          {{pk, pks, pk_stride, kIn}, {seeds, H.xs, H.xs, kIn}, {ct, cts, cts, kOut}, {ss, sss, sss, kOut},
+           {status, 1, 1, kStatus}},
+          {{!status, "%s: device-pointer calls need a status array (it carries kem.ErrPubKey)"},
+           {!aligned({pk, seeds, ct, ss}, {pk_stride}, H.xs == 56 ? 8 : 16), align_text(H.xs)}}};
+  Counts c;
+  rc = run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return H.xs == 56 ? hybrid448_encaps_dev(H, r[0].p, r[0].stride, r[1].p, r[2].p, r[3].p, r[4].p, cnt, st, slot)
+                      : hybrid_encaps_dev(H, r[0].p, r[0].stride, r[1].p, r[2].p, r[3].p, r[4].p, cnt, st, slot);
+  }, &c);
   if (rc) return rc;
-  return status_result(hc.bit0, hc.bit1, n, "cb200_hybrid_encaps");
+  return status_result(c.bit0, c.bit1, n, "cb200_hybrid_encaps");
 }
 
 int cb200_hybrid_decaps(int id, const uint8_t* sk, size_t sk_stride, const uint8_t* ct, uint8_t* ss, uint8_t* status, size_t n) {
@@ -805,64 +610,18 @@ int cb200_hybrid_decaps(int id, const uint8_t* sk, size_t sk_stride, const uint8
     return CB200_ERR_ARG;
   }
   if (n == 0) return 0;
-  bool dev = false;
-  if (!same_side({sk, ct, ss, status}, &dev)) {
-    set_error("cb200_hybrid_decaps: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (!status) {
-      set_error("cb200_hybrid_decaps: device-pointer calls need a status array (it carries kem.ErrPubKey / kem.ErrPrivKey)");
-      return CB200_ERR_ARG;
-    }
-    if (H.xs == 56) {
-      if (!aligned8({sk, ct, ss}, {})) {
-        set_error("cb200_hybrid_decaps: device buffers must be 8-byte aligned");
-        return CB200_ERR_ARG;
-      }
-      DeviceCall call(ss);
-      if (call.rc) return call.rc;
-      return hybrid448_decaps_dev(H, sk, sk_stride, ct, ss, status, n, call.st, kDevSlot);
-    }
-    if (!aligned16({sk, ct, ss}, {})) {
-      set_error("cb200_hybrid_decaps: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(ss);
-    if (call.rc) return call.rc;
-    return hybrid_decaps_dev(H, sk, sk_stride, ct, ss, status, n, call.st, kDevSlot);
-  }
-  if (H.xs == 56) {
-    const size_t sks = H.dk + 56;
-    HostCall hc;
-    hc.bufs = {Buf{sk, nullptr, sks, false, sk_stride}, Buf{ct, nullptr, H.ct + 56, false, 0},
-               Buf{nullptr, ss, 88, false, 0}, Buf{nullptr, nullptr, 1, false, 0}};
-    hc.chunk = 1u << 15;
-    hc.min_shard = 1u << 13;
-    hc.status_buf = 3;
-    hc.user_status = status;
-    hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-      return hybrid448_decaps_dev(H, (const uint8_t*)d[0], sks, (const uint8_t*)d[1], (uint8_t*)d[2], (uint8_t*)d[3], cnt, st,
-                                  slot);
-    };
-    rc = hc.run(n);
-    if (rc) return rc;
-    return status_result(hc.bit0, hc.bit1, n, "cb200_hybrid_decaps");
-  }
-  const size_t sks = H.dk + 32;
-  HostCall hc;
-  hc.bufs = {Buf{sk, nullptr, sks, false, sk_stride}, Buf{ct, nullptr, H.ct + 32, false, 0},
-             Buf{nullptr, ss, 64, false, 0}, Buf{nullptr, nullptr, 1, false, 0}};
-  hc.chunk = 1u << 15;
-  hc.min_shard = 1u << 13;
-  hc.status_buf = 3;
-  hc.user_status = status;
-  hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-    return hybrid_decaps_dev(H, (const uint8_t*)d[0], sks, (const uint8_t*)d[1], (uint8_t*)d[2], (uint8_t*)d[3], cnt, st, slot);
-  };
-  rc = hc.run(n);
+  const size_t sks = H.dk + H.xs, cts = H.ct + H.xs, sss = 32 + H.xs;
+  Batch b{"cb200_hybrid_decaps", n, ss, 1u << 15, 1u << 13,
+          {{sk, sks, sk_stride, kIn}, {ct, cts, cts, kIn}, {ss, sss, sss, kOut}, {status, 1, 1, kStatus}},
+          {{!status, "%s: device-pointer calls need a status array (it carries kem.ErrPubKey / kem.ErrPrivKey)"},
+           {!aligned({sk, ct, ss}, {}, H.xs == 56 ? 8 : 16), align_text(H.xs)}}};
+  Counts c;
+  rc = run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return H.xs == 56 ? hybrid448_decaps_dev(H, r[0].p, r[0].stride, r[1].p, r[2].p, r[3].p, cnt, st, slot)
+                      : hybrid_decaps_dev(H, r[0].p, r[0].stride, r[1].p, r[2].p, r[3].p, cnt, st, slot);
+  }, &c);
   if (rc) return rc;
-  return status_result(hc.bit0, hc.bit1, n, "cb200_hybrid_decaps");
+  return status_result(c.bit0, c.bit1, n, "cb200_hybrid_decaps");
 }
 
 }  // extern "C"

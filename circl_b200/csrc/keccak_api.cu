@@ -9,6 +9,7 @@
 // that global accesses are whole 128-byte lines (a state is 200 bytes: thread-private rows would touch 7 sectors each).
 #include "../../include/circl_b200.h"
 #include "context.h"
+#include "flow_internal.h"
 #include "keccak.cuh"
 
 namespace cb200 {
@@ -123,18 +124,10 @@ int cb200_keccak_f1600(uint64_t* states, size_t n, int turbo) {
     set_error("cb200_keccak_f1600: null pointer");
     return CB200_ERR_ARG;
   }
-  if (is_device_ptr(states)) {
-    if ((uintptr_t)states & 7) {
-      set_error("cb200_keccak_f1600: device states must be 8-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(states);
-    if (call.rc) return call.rc;
-    return keccakapi::launch_f1600(states, n, turbo, call.st);
-  }
-  std::vector<Buf> bufs = {Buf{states, states, 200, false, 0}};
-  return run_host(bufs, n, 1u << 18, 1u << 16, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return keccakapi::launch_f1600((uint64_t*)d[0], cnt, turbo, st);
+  Batch b{"cb200_keccak_f1600", n, states, 1u << 18, 1u << 16, {{states, 200, 200, kInOut}},
+          {{!aligned({states}, {}, 8), "%s: device states must be 8-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return keccakapi::launch_f1600((uint64_t*)r[0].p, cnt, turbo, st);
   });
 }
 
@@ -161,21 +154,11 @@ int cb200_sha3(int bits, const uint8_t* in, size_t in_stride, size_t inlen, uint
     set_error("cb200_sha3: bad argument");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(out);
-  if (in && dev != is_device_ptr(in)) {
-    set_error("cb200_sha3: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    DeviceCall call(out);
-    if (call.rc) return call.rc;
-    return keccakapi::launch_sponge(rw, in, in_stride, inlen, out, outlen, n, ds, call.st);
-  }
-  const size_t unit = inlen ? inlen : 1;
-  std::vector<Buf> bufs = {Buf{inlen ? in : nullptr, nullptr, unit, in_stride == 0, in_stride}, Buf{nullptr, out, outlen, false, 0}};
-  return run_host(bufs, n, 1u << 16, 1u << 14, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return keccakapi::launch_sponge(rw, (const uint8_t*)d[0], in_stride == 0 ? 0 : inlen, inlen, (uint8_t*)d[1], outlen, cnt,
-                                    ds, st);
+  // an empty input is never read: its rows are a device area only (unit 1 keeps the staged image non-empty)
+  Batch b{"cb200_sha3", n, out, 1u << 16, 1u << 14,
+          {{in, inlen ? inlen : 1, in_stride, inlen ? kIn : kScratch}, {out, outlen, outlen, kOut}}, {}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return keccakapi::launch_sponge(rw, r[0].p, r[0].stride, inlen, r[1].p, outlen, cnt, ds, st);
   });
 }
 

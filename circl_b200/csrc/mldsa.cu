@@ -24,6 +24,7 @@
 #include "../../include/circl_b200.h"
 #include "context.h"
 #include "dilithium.cuh"
+#include "flow_internal.h"
 #include "keccak.cuh"
 #include "mldsa_internal.h"
 
@@ -2001,37 +2002,19 @@ int cb200_mldsa_sign(int mode, const uint8_t* sk, size_t sk_stride, const uint8_
     return CB200_ERR_ARG;
   }
   const int internal = flags & CB200_SIGN_INTERNAL;
-  const bool dev = is_device_ptr(sig);
-  if (dev != is_device_ptr(sk) || dev != is_device_ptr(msgs) || dev != is_device_ptr(msg_off) ||
-      (rnd && dev != is_device_ptr(rnd)) || (status && dev != is_device_ptr(status))) {
-    set_error("cb200_mldsa_sign: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (((uintptr_t)sk | sk_stride | (uintptr_t)msg_off) & 15) {
-      set_error("cb200_mldsa_sign: device sk and sk_stride must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    if (n >= (1u << 24)) {  // the attempt bid of the finalize step packs (attempt << 24 | slot)
-      set_error("cb200_mldsa_sign: a device-pointer batch is limited to 2^24 - 1 signatures per call (got %zu)", n);
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(sig);
-    if (call.rc) return call.rc;
-    const uint8_t* dctx = nullptr;
-    if (ctxlen) {  // the context string is at most 255 bytes and always a host pointer: stage it
-      CB200_CUDA(cudaMemcpyAsync(call.ws->small, context, ctxlen, cudaMemcpyHostToDevice, call.st));
-      dctx = (const uint8_t*)call.ws->small;
-    }
-    return dispatch_sign(mode, sk, sk_stride, msgs, msg_off, dctx, (int)ctxlen, rnd, sig, status, n, internal, call.st, kDevSlot,
-                         attempts, (volatile uint32_t*)call.ws->pin);
-  }
+  Batch b{"cb200_mldsa_sign", n, sig, 0, 0,
+          {{sk, ms.sk, sk_stride, kIn}, {sig, ms.sig, ms.sig, kOut}, {status, 1, 1, kStatus}, {rnd, 32, 32, kIn}},
+          {{!aligned({sk, msg_off}, {sk_stride}, 16), "%s: device sk and sk_stride must be 16-byte aligned"},
+           // the attempt bid of the finalize step packs (attempt << 24 | slot)
+           {n >= (1u << 24), "%s: a device-pointer batch is limited to 2^24 - 1 signatures per call (got %zu)"}},
+          msgs, msg_off, context, ctxlen};
   // host pointers: one contiguous range of the batch per GPU; on each GPU chunks of 2^16 signatures go through the three
   // staging slots.  The rejection loop of a chunk keeps the host busy (one counter read per round), so the input of
   // chunk i+1 is put in flight before chunk i starts and the signatures of chunk i travel back while chunk i+1 runs.
   std::atomic<uint64_t> all_attempts{0};
   std::atomic<size_t> all_bad{0};
-  rc = for_each_shard(n, 1u << 12, [&](size_t sh_first, size_t sh_n) -> int {
+  b.host = [&]() -> int {
+  int rc = for_each_shard(n, 1u << 12, [&](size_t sh_first, size_t sh_n) -> int {
   Dev& c = ctx();
   int rc = 0;
   constexpr size_t kChunk = 1u << 16;
@@ -2113,11 +2096,14 @@ int cb200_mldsa_sign(int mode, const uint8_t* sk, size_t sk_stride, const uint8_
   });
   if (rc) return rc;
   if (attempts) *attempts = all_attempts.load();
-  if (all_bad.load()) {
-    set_error("cb200_mldsa_sign: %zu of %zu signatures exhausted 576 attempts", all_bad.load(), n);
-    return CB200_ERR_SIGN_ATTEMPTS;
-  }
   return 0;
+  };
+  rc = run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return dispatch_sign(mode, r[0].p, r[0].stride, r.msgs, r.msg_off, r.ctx, (int)ctxlen, r[3].p, r[1].p, r[2].p, cnt,
+                         internal, st, slot, attempts, (volatile uint32_t*)wset(slot).pin);
+  });
+  if (rc) return rc;
+  return sign_attempts_result("cb200_mldsa_sign", all_bad.load(), n);
 }
 
 int cb200_mldsa_verify(int mode, const uint8_t* pk, size_t pk_stride, const uint8_t* msgs, const uint64_t* msg_off,
@@ -2140,66 +2126,14 @@ int cb200_mldsa_verify(int mode, const uint8_t* pk, size_t pk_stride, const uint
     return CB200_ERR_ARG;
   }
   const int internal = flags & CB200_SIGN_INTERNAL;
-  const bool dev = is_device_ptr(ok);
-  if (dev != is_device_ptr(pk) || dev != is_device_ptr(msgs) || dev != is_device_ptr(msg_off) || dev != is_device_ptr(sig)) {
-    set_error("cb200_mldsa_verify: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (((uintptr_t)pk | pk_stride | (uintptr_t)msg_off) & 15) {
-      set_error("cb200_mldsa_verify: device pk and pk_stride must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(ok);
-    if (call.rc) return call.rc;
-    const uint8_t* dctx = nullptr;
-    if (ctxlen) {
-      CB200_CUDA(cudaMemcpyAsync(call.ws->small, context, ctxlen, cudaMemcpyHostToDevice, call.st));
-      dctx = (const uint8_t*)call.ws->small;
-    }
-    return dispatch_verify(mode, pk, pk_stride, msgs, msg_off, dctx, (int)ctxlen, sig, ok, n, internal, call.st, kDevSlot);
-  }
   // host pointers: one contiguous range per GPU, each in chunks of 2^15 signatures on the first staging slot
-  return for_each_shard(n, 1u << 12, [&](size_t sh_first, size_t sh_n) -> int {
-    Dev& c = ctx();
-    cudaStream_t st = c.pipe[0];
-    constexpr size_t kChunk = 1u << 15;
-    for (size_t first = sh_first; first < sh_first + sh_n; first += kChunk) {
-      const size_t cnt = sh_first + sh_n - first < kChunk ? sh_first + sh_n - first : kChunk;
-      const uint64_t m0 = msg_off[first];
-      const size_t msg_bytes = (size_t)(msg_off[first + cnt] - m0);
-      size_t off = 0;
-      auto take = [&](size_t bytes) {
-        size_t o = off;
-        off += (bytes + 255) & ~(size_t)255;
-        return o;
-      };
-      const size_t nk = pk_stride ? cnt : 1;
-      const size_t oPk = take(nk * ms.pk), oMsg = take(msg_bytes + 8), oOff = take((cnt + 1) * 8), oSig = take(cnt * ms.sig),
-                   oOk = take(cnt), oCtx = take(256);
-      int rc = ensure_scratch(0, off);
-      if (rc) return rc;
-      char* d = (char*)c.scratch[0];
-      if (pk_stride == 0)
-        CB200_CUDA(cudaMemcpyAsync(d + oPk, pk, ms.pk, cudaMemcpyHostToDevice, st));
-      else if (pk_stride == ms.pk)
-        CB200_CUDA(cudaMemcpyAsync(d + oPk, pk + first * ms.pk, nk * ms.pk, cudaMemcpyHostToDevice, st));
-      else
-        CB200_CUDA(cudaMemcpy2DAsync(d + oPk, ms.pk, pk + first * pk_stride, pk_stride, ms.pk, cnt, cudaMemcpyHostToDevice, st));
-      if (msg_bytes) CB200_CUDA(cudaMemcpyAsync(d + oMsg, msgs + m0, msg_bytes, cudaMemcpyHostToDevice, st));
-      std::vector<uint64_t> ro(cnt + 1);
-      for (size_t i = 0; i <= cnt; i++) ro[i] = msg_off[first + i] - m0;
-      CB200_CUDA(cudaMemcpyAsync(d + oOff, ro.data(), (cnt + 1) * 8, cudaMemcpyHostToDevice, st));
-      CB200_CUDA(cudaMemcpyAsync(d + oSig, sig + first * ms.sig, cnt * ms.sig, cudaMemcpyHostToDevice, st));
-      if (ctxlen) CB200_CUDA(cudaMemcpyAsync(d + oCtx, context, ctxlen, cudaMemcpyHostToDevice, st));
-      rc = dispatch_verify(mode, (const uint8_t*)d + oPk, pk_stride ? ms.pk : (size_t)0, (const uint8_t*)d + oMsg,
-                           (const uint64_t*)(d + oOff), ctxlen ? (const uint8_t*)d + oCtx : (const uint8_t*)nullptr,
-                           (int)ctxlen, (const uint8_t*)d + oSig, (uint8_t*)d + oOk, cnt, internal, st, 0);
-      if (rc) return rc;
-      CB200_CUDA(cudaMemcpyAsync(ok + first, d + oOk, cnt, cudaMemcpyDeviceToHost, st));
-      CB200_CUDA(cudaStreamSynchronize(st));  // `ro` and the scratch are reused by the next chunk
-    }
-    return 0;
+  Batch b{"cb200_mldsa_verify", n, ok, 1u << 15, 1u << 12,
+          {{pk, ms.pk, pk_stride, kIn}, {sig, ms.sig, ms.sig, kIn}, {ok, 1, 1, kOut}},
+          {{!aligned({pk, msg_off}, {pk_stride}, 16), "%s: device pk and pk_stride must be 16-byte aligned"}},
+          msgs, msg_off, context, ctxlen};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return dispatch_verify(mode, (const uint8_t*)r[0].p, r[0].stride, (const uint8_t*)r.msgs, r.msg_off, r.ctx, (int)ctxlen,
+                           (const uint8_t*)r[1].p, r[2].p, cnt, internal, st, slot);
   });
 }
 
@@ -2216,26 +2150,10 @@ int cb200_mldsa_keygen(int mode, const uint8_t* seeds, uint8_t* pk, uint8_t* sk,
     set_error("cb200_mldsa_keygen: null pointer");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(pk);
-  if (dev != is_device_ptr(seeds) || dev != is_device_ptr(sk)) {
-    set_error("cb200_mldsa_keygen: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (((uintptr_t)seeds | (uintptr_t)pk | (uintptr_t)sk) & 15) {
-      set_error("cb200_mldsa_keygen: device buffers must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(pk);
-    if (call.rc) return call.rc;
-    return dispatch_keygen(mode, seeds, pk, sk, n, call.st, kDevSlot);
-  }
-  std::vector<Buf> bufs(3);
-  bufs[0] = Buf{seeds, nullptr, 32, false, 0};
-  bufs[1] = Buf{nullptr, pk, ms.pk, false, 0};
-  bufs[2] = Buf{nullptr, sk, ms.sk, false, 0};
-  return run_host(bufs, n, 1u << 14, 1u << 12, [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) -> int {
-    return dispatch_keygen(mode, (const uint8_t*)d[0], (uint8_t*)d[1], (uint8_t*)d[2], cnt, st, slot);
+  Batch b{"cb200_mldsa_keygen", n, pk, 1u << 14, 1u << 12, {{seeds, 32, 32, kIn}, {pk, ms.pk, ms.pk, kOut}, {sk, ms.sk, ms.sk, kOut}},
+          {{!aligned({seeds, pk, sk}, {}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) -> int {
+    return dispatch_keygen(mode, (const uint8_t*)r[0].p, r[1].p, r[2].p, cnt, st, slot);
   });
 }
 
@@ -2270,11 +2188,6 @@ static int sampler_entry(const char* fn, int kind, int mode, uint32_t* polys, co
     set_error("%s: bad argument", fn);
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(polys);
-  if (dev != is_device_ptr(seeds) || (nonces && dev != is_device_ptr(nonces))) {
-    set_error("%s: mixed host/device pointers", fn);
-    return CB200_ERR_ARG;
-  }
   auto launch = [&](const uint8_t* sd, size_t stride, const uint16_t* nn, uint32_t* out, size_t cnt, cudaStream_t st) -> int {
     using namespace mldsa;
     KernelScope ks(KID_SAMPLER, st);
@@ -2307,21 +2220,11 @@ static int sampler_entry(const char* fn, int kind, int mode, uint32_t* polys, co
     CB200_CUDA(cudaGetLastError());
     return 0;
   };
-  if (dev) {
-    if (((uintptr_t)polys & 15) || (nonces && ((uintptr_t)nonces & 1))) {
-      set_error("%s: device polynomials must be 16-byte aligned", fn);
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(polys);
-    if (call.rc) return call.rc;
-    return launch(seeds, seed_stride, nonces, polys, n, call.st);
-  }
-  std::vector<Buf> bufs = {Buf{seeds, nullptr, seed_len, seed_stride == 0, seed_stride},
-                           Buf{nullptr, polys, 1024, false, 0}};
-  if (nonces) bufs.push_back(Buf{nonces, nullptr, 2, false, 0});
-  return run_host(bufs, n, 1u << 15, 1u << 13, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return launch((const uint8_t*)d[0], seed_stride == 0 ? 0 : seed_len, nonces ? (const uint16_t*)d[2] : nullptr,
-                  (uint32_t*)d[1], cnt, st);
+  Batch b{fn, n, polys, 1u << 15, 1u << 13,
+          {{seeds, seed_len, seed_stride, kIn}, {polys, 1024, 1024, kOut}, {nonces, 2, 2, kIn}},
+          {{!aligned({polys}, {}, 16) || !aligned({nonces}, {}, 2), "%s: device polynomials must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return launch(r[0].p, r[0].stride, (const uint16_t*)r[2].p, (uint32_t*)r[1].p, cnt, st);
   });
 }
 int cb200_dil_derive_uniform(uint32_t* polys, const uint8_t* seeds, size_t seed_stride, const uint16_t* nonces, size_t n) {

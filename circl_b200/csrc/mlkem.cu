@@ -22,6 +22,7 @@
 
 #include "../../include/circl_b200.h"
 #include "context.h"
+#include "flow_internal.h"
 #include "mlkem_internal.h"
 #include "keccak.cuh"
 #include "kyber.cuh"
@@ -1881,29 +1882,11 @@ static int keygen_entry(const char* fn, int mlkem_flag, int k, const uint8_t* se
     set_error("%s: null pointer", fn);
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(ek);
-  if (dev != is_device_ptr(seeds) || dev != is_device_ptr(dk)) {
-    set_error("%s: mixed host/device pointers", fn);
-    return CB200_ERR_ARG;
-  }
-  auto run = [&](const uint8_t* s_, uint8_t* e_, uint8_t* d_, size_t cnt, cudaStream_t st, int slot) {
-    return mlkem::dev_keygen(k, mlkem_flag, s_, e_, d_, cnt, st, slot);
-  };
-  if (dev) {
-    if (((uintptr_t)seeds | (uintptr_t)ek | (uintptr_t)dk) & 15) {
-      set_error("%s: device buffers must be 16-byte aligned", fn);
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(ek);
-    if (call.rc) return call.rc;
-    return run(seeds, ek, dk, n, call.st, kDevSlot);
-  }
-  std::vector<Buf> bufs(3);
-  bufs[0] = Buf{seeds, nullptr, 64, false, 0};
-  bufs[1] = Buf{nullptr, ek, cb200_mlkem_public_key_size(k), false, 0};
-  bufs[2] = Buf{nullptr, dk, 768u * k + 96, false, 0};
-  return run_host(bufs, n, 1u << 15, 1u << 13, [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-    return run((const uint8_t*)d[0], (uint8_t*)d[1], (uint8_t*)d[2], cnt, st, slot);
+  const size_t eksz = cb200_mlkem_public_key_size(k), dksz = 768u * k + 96;
+  Batch b{fn, n, ek, 1u << 15, 1u << 13, {{seeds, 64, 64, kIn}, {ek, eksz, eksz, kOut}, {dk, dksz, dksz, kOut}},
+          {{!aligned({seeds, ek, dk}, {}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return mlkem::dev_keygen(k, mlkem_flag, r[0].p, r[1].p, r[2].p, cnt, st, slot);
   });
 }
 
@@ -1931,38 +1914,15 @@ static int kyber_kem_run(int decaps, int k, const uint8_t* key, size_t key_strid
     set_error("%s: bad argument", fn);
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(ss);
-  if (dev != is_device_ptr(key) || dev != is_device_ptr(in) || (ct && dev != is_device_ptr(ct))) {
-    set_error("%s: mixed host/device pointers", fn);
-    return CB200_ERR_ARG;
-  }
-  auto run = [&](const uint8_t* k_, size_t ks_, const uint8_t* i_, uint8_t* c_, uint8_t* s_, size_t cnt, cudaStream_t st,
-                 int slot) {
-    return k == 2   ? mlkem::r3_device<2>(decaps, k_, ks_, i_, c_, s_, cnt, st, slot)
-           : k == 3 ? mlkem::r3_device<3>(decaps, k_, ks_, i_, c_, s_, cnt, st, slot)
-                    : mlkem::r3_device<4>(decaps, k_, ks_, i_, c_, s_, cnt, st, slot);
-  };
-  if (dev) {
-    if (((uintptr_t)key | (uintptr_t)in | (uintptr_t)ct | (uintptr_t)ss | key_stride) & 15) {
-      set_error("%s: device buffers and the key stride must be 16-byte aligned", fn);
-      return CB200_ERR_ARG;
-    }
-    if (key_stride == 0 && decaps) {
-      set_error("%s: a shared dk needs host pointers (the device path expects one dk per op)", fn);
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(ss);
-    if (call.rc) return call.rc;
-    return run(key, key_stride, in, ct, ss, n, call.st, kDevSlot);
-  }
-  std::vector<Buf> bufs;
-  bufs.push_back(Buf{key, nullptr, keysz, key_stride == 0, key_stride});
-  bufs.push_back(Buf{in, nullptr, decaps ? ctsz : (size_t)32, false, 0});
-  bufs.push_back(Buf{nullptr, ss, 32, false, 0});
-  if (!decaps) bufs.push_back(Buf{nullptr, ct, ctsz, false, 0});
-  return run_host(bufs, n, 1u << 15, 1u << 13, [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-    return run((const uint8_t*)d[0], key_stride == 0 ? 0 : keysz, (const uint8_t*)d[1], decaps ? nullptr : (uint8_t*)d[3],
-               (uint8_t*)d[2], cnt, st, slot);
+  const size_t insz = decaps ? ctsz : (size_t)32;
+  Batch b{fn, n, ss, 1u << 15, 1u << 13,
+          {{key, keysz, key_stride, kIn}, {in, insz, insz, kIn}, {ss, 32, 32, kOut}, {ct, ctsz, ctsz, kOut}},
+          {{!aligned({key, in, ct, ss}, {key_stride}, 16), "%s: device buffers and the key stride must be 16-byte aligned"},
+           {key_stride == 0 && decaps, "%s: a shared dk needs host pointers (the device path expects one dk per op)"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return k == 2   ? mlkem::r3_device<2>(decaps, r[0].p, r[0].stride, r[1].p, r[3].p, r[2].p, cnt, st, slot)
+           : k == 3 ? mlkem::r3_device<3>(decaps, r[0].p, r[0].stride, r[1].p, r[3].p, r[2].p, cnt, st, slot)
+                    : mlkem::r3_device<4>(decaps, r[0].p, r[0].stride, r[1].p, r[3].p, r[2].p, cnt, st, slot);
   });
 }
 int cb200_kyber_kem_encaps(int k, const uint8_t* ek, size_t ek_stride, const uint8_t* seeds, uint8_t* ct, uint8_t* ss,
@@ -1989,47 +1949,26 @@ int cb200_mlkem_decaps(int k, const uint8_t* dk, size_t dk_stride, const uint8_t
     set_error("cb200_mlkem_decaps: bad argument");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(ss);
-  if (dev != is_device_ptr(dk) || dev != is_device_ptr(ct) || (status && dev != is_device_ptr(status))) {
-    set_error("cb200_mlkem_decaps: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  auto run = [&](const uint8_t* d_dk, size_t stride, const uint8_t* d_ct, uint8_t* d_ss, uint8_t* d_st, size_t cnt,
-                 cudaStream_t st, int slot) { return mlkem::dev_decaps(k, 1, d_dk, stride, d_ct, d_ss, d_st, cnt, st, slot); };
-  if (dev) {
-    if (((uintptr_t)dk | (uintptr_t)ct | (uintptr_t)ss | dk_stride) & 15) {
-      set_error("cb200_mlkem_decaps: device buffers and dk_stride must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    if (dk_stride == 0) {
-      set_error("cb200_mlkem_decaps: a shared dk needs host pointers (device path expects one dk per op)");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(ss);
-    if (call.rc) return call.rc;
-    return run(dk, dk_stride, ct, ss, status, n, call.st, kDevSlot);
-  }
   // a shared dk is replicated per op on the device inside each staged chunk (the decapsulation pipeline is per-op)
-  HostCall hc;
-  hc.bufs = {Buf{dk, nullptr, dksz, dk_stride == 0, dk_stride}, Buf{ct, nullptr, ctsz, false, 0},
-             Buf{nullptr, ss, 32, false, 0}, Buf{nullptr, nullptr, 1, false, 0}};
-  if (dk_stride == 0) hc.bufs.push_back(Buf{nullptr, nullptr, dksz, false, 0});  // per-op replicas (device only)
-  hc.chunk = 1u << 15;
-  hc.min_shard = 1u << 13;
-  hc.status_buf = 3;
-  hc.user_status = status;
-  hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) -> int {
-    const uint8_t* keys = (const uint8_t*)d[0];
-    if (dk_stride == 0) {
-      int r = mlkem::replicate_rows((const uint8_t*)d[0], (uint8_t*)d[4], dksz, cnt, st);
-      if (r) return r;
-      keys = (const uint8_t*)d[4];
+  Batch b{"cb200_mlkem_decaps", n, ss, 1u << 15, 1u << 13,
+          {{dk, dksz, dk_stride, kIn}, {ct, ctsz, ctsz, kIn}, {ss, 32, 32, kOut}, {status, 1, 1, kStatus},
+           {nullptr, dk_stride ? 0 : dksz, dksz, kScratch}},  // per-op replicas of a shared dk (host path only)
+          {{!aligned({dk, ct, ss}, {dk_stride}, 16), "%s: device buffers and dk_stride must be 16-byte aligned"},
+           {dk_stride == 0, "%s: a shared dk needs host pointers (device path expects one dk per op)"}}};
+  Counts c;
+  rc = run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) -> int {
+    const uint8_t* keys = r[0].p;
+    size_t stride = r[0].stride;
+    if (r[4].p) {
+      int e = mlkem::replicate_rows(r[0].p, r[4].p, dksz, cnt, st);
+      if (e) return e;
+      keys = r[4].p;
+      stride = dksz;
     }
-    return run(keys, dksz, (const uint8_t*)d[1], (uint8_t*)d[2], (uint8_t*)d[3], cnt, st, slot);
-  };
-  rc = hc.run(n);
+    return mlkem::dev_decaps(k, 1, keys, stride, r[1].p, r[2].p, r[3].p, cnt, st, slot);
+  }, &c);
   if (rc) return rc;
-  return status_error("cb200_mlkem_decaps", 0, hc.bit1, n);
+  return status_error("cb200_mlkem_decaps", 0, c.bit1, n);
 }
 
 size_t cb200_mlkem_public_key_size(int k) { return (k >= 2 && k <= 4) ? 384u * k + 32 : 0; }
@@ -2063,38 +2002,18 @@ static int mlkem_encaps_entry(int k, const uint8_t* ek, size_t ek_stride, const 
     set_error("cb200_mlkem_encaps: bad argument");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(ct);
-  if (dev != is_device_ptr(ek) || dev != is_device_ptr(seeds) || dev != is_device_ptr(ss) ||
-      (status && dev != is_device_ptr(status))) {
-    set_error("cb200_mlkem_encaps: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if (((uintptr_t)ek | (uintptr_t)seeds | (uintptr_t)ct | (uintptr_t)ss | ek_stride) & 15) {
-      set_error("cb200_mlkem_encaps: device buffers and ek_stride must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    // status is needed to report kem.ErrPubKey; with device pointers the caller reads it asynchronously
-    DeviceCall call(ct);
-    if (call.rc) return call.rc;
-    return mlkem::encaps_any(k, ek, ek_stride, seeds, ct, ss, status, n, call.st, kDevSlot, push_ct, push_ss);
-  }
   // host pointers: one contiguous index range per GPU, each staged through HBM in chunks on three streams
-  // (H2D | kernels | D2H overlap); the per-op status always comes back (it carries kem.ErrPubKey)
-  HostCall hc;
-  hc.bufs = {Buf{ek, nullptr, eksz, ek_stride == 0, ek_stride}, Buf{seeds, nullptr, 32, false, 0},
-             Buf{nullptr, ct, ctsz, false, 0}, Buf{nullptr, ss, 32, false, 0}, Buf{nullptr, nullptr, 1, false, 0}};
-  hc.chunk = 1u << 16;
-  hc.min_shard = 1u << 13;
-  hc.status_buf = 4;
-  hc.user_status = status;
-  hc.body = [&](void** d, size_t cnt, size_t, cudaStream_t st, int slot) {
-    return mlkem::encaps_any(k, (const uint8_t*)d[0], ek_stride == 0 ? 0 : eksz, (const uint8_t*)d[1],
-                             (uint8_t*)d[2], (uint8_t*)d[3], (uint8_t*)d[4], cnt, st, slot);
-  };
-  rc = hc.run(n);
+  // (H2D | kernels | D2H overlap); the per-op status always comes back (it carries kem.ErrPubKey).  With device
+  // pointers the caller reads status asynchronously.
+  Batch b{"cb200_mlkem_encaps", n, ct, 1u << 16, 1u << 13,
+          {{ek, eksz, ek_stride, kIn}, {seeds, 32, 32, kIn}, {ct, ctsz, ctsz, kOut}, {ss, 32, 32, kOut}, {status, 1, 1, kStatus}},
+          {{!aligned({ek, seeds, ct, ss}, {ek_stride}, 16), "%s: device buffers and ek_stride must be 16-byte aligned"}}};
+  Counts c;
+  rc = run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) {
+    return mlkem::encaps_any(k, r[0].p, r[0].stride, r[1].p, r[2].p, r[3].p, r[4].p, cnt, st, slot, push_ct, push_ss);
+  }, &c);
   if (rc) return rc;
-  return status_error("cb200_mlkem_encaps", hc.bit0, 0, n);
+  return status_error("cb200_mlkem_encaps", c.bit0, 0, n);
 }
 
 int cb200_kyber_derive_uniform(int16_t* polys, const uint8_t* seeds, size_t seed_stride, const uint8_t* xy, size_t n) {
@@ -2105,25 +2024,11 @@ int cb200_kyber_derive_uniform(int16_t* polys, const uint8_t* seeds, size_t seed
     set_error("cb200_kyber_derive_uniform: bad argument");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(polys);
-  if (dev != is_device_ptr(seeds) || dev != is_device_ptr(xy)) {
-    set_error("cb200_kyber_derive_uniform: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if ((uintptr_t)polys & 15) {
-      set_error("cb200_kyber_derive_uniform: device polynomials must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(polys);
-    if (call.rc) return call.rc;
-    return mlkem::launch_derive_uniform(seeds, seed_stride, xy, polys, n, call.st);
-  }
-  std::vector<Buf> bufs = {Buf{seeds, nullptr, 32, seed_stride == 0, seed_stride}, Buf{xy, nullptr, 2, false, 0},
-                           Buf{nullptr, polys, 512, false, 0}};
-  return run_host(bufs, n, 1u << 16, 1u << 14, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return mlkem::launch_derive_uniform((const uint8_t*)d[0], seed_stride == 0 ? 0 : 32, (const uint8_t*)d[1], (int16_t*)d[2],
-                                        cnt, st);
+  Batch b{"cb200_kyber_derive_uniform", n, polys, 1u << 16, 1u << 14,
+          {{seeds, 32, seed_stride, kIn}, {xy, 2, 2, kIn}, {polys, 512, 512, kOut}},
+          {{!aligned({polys}, {}, 16), "%s: device polynomials must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return mlkem::launch_derive_uniform(r[0].p, r[0].stride, r[1].p, (int16_t*)r[2].p, cnt, st);
   });
 }
 
@@ -2140,25 +2045,11 @@ int cb200_kyber_derive_noise(int16_t* polys, int eta, const uint8_t* seeds, size
     set_error("cb200_kyber_derive_noise: bad argument");
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(polys);
-  if (dev != is_device_ptr(seeds) || dev != is_device_ptr(nonces)) {
-    set_error("cb200_kyber_derive_noise: mixed host/device pointers");
-    return CB200_ERR_ARG;
-  }
-  if (dev) {
-    if ((uintptr_t)polys & 15) {
-      set_error("cb200_kyber_derive_noise: device polynomials must be 16-byte aligned");
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(polys);
-    if (call.rc) return call.rc;
-    return mlkem::launch_derive_noise(eta, seeds, seed_stride, nonces, polys, n, call.st);
-  }
-  std::vector<Buf> bufs = {Buf{seeds, nullptr, 32, seed_stride == 0, seed_stride}, Buf{nonces, nullptr, 1, false, 0},
-                           Buf{nullptr, polys, 512, false, 0}};
-  return run_host(bufs, n, 1u << 16, 1u << 14, [&](void** d, size_t cnt, size_t, cudaStream_t st, int) {
-    return mlkem::launch_derive_noise(eta, (const uint8_t*)d[0], seed_stride == 0 ? 0 : 32, (const uint8_t*)d[1],
-                                      (int16_t*)d[2], cnt, st);
+  Batch b{"cb200_kyber_derive_noise", n, polys, 1u << 16, 1u << 14,
+          {{seeds, 32, seed_stride, kIn}, {nonces, 1, 1, kIn}, {polys, 512, 512, kOut}},
+          {{!aligned({polys}, {}, 16), "%s: device polynomials must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return mlkem::launch_derive_noise(eta, r[0].p, r[0].stride, r[1].p, (int16_t*)r[2].p, cnt, st);
   });
 }
 
@@ -2175,25 +2066,12 @@ static int codec_entry(const char* fn, int op, int d, const void* in, void* out,
     set_error("%s: null pointer", fn);
     return CB200_ERR_ARG;
   }
-  const bool dev = is_device_ptr(out);
-  if (dev != is_device_ptr(in)) {
-    set_error("%s: mixed host/device pointers", fn);
-    return CB200_ERR_ARG;
-  }
   const size_t bytes = op < 2 ? 384 : 32 * (size_t)d;
   const size_t in_unit = (op == 0 || op == 2) ? 512 : bytes, out_unit = (op == 0 || op == 2) ? bytes : 512;
-  if (dev) {
-    if (((uintptr_t)in | (uintptr_t)out) & 15) {
-      set_error("%s: device buffers must be 16-byte aligned", fn);
-      return CB200_ERR_ARG;
-    }
-    DeviceCall call(out);
-    if (call.rc) return call.rc;
-    return mlkem::launch_kyber_codec(op, d, in, out, n, call.st);
-  }
-  std::vector<Buf> bufs = {Buf{in, nullptr, in_unit, false, 0}, Buf{nullptr, out, out_unit, false, 0}};
-  return run_host(bufs, n, 1u << 17, 1u << 15, [&](void** dv, size_t cnt, size_t, cudaStream_t st, int) {
-    return mlkem::launch_kyber_codec(op, d, dv[0], dv[1], cnt, st);
+  Batch b{fn, n, out, 1u << 17, 1u << 15, {{in, in_unit, in_unit, kIn}, {out, out_unit, out_unit, kOut}},
+          {{!aligned({in, out}, {}, 16), "%s: device buffers must be 16-byte aligned"}}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int) {
+    return mlkem::launch_kyber_codec(op, d, r[0].p, r[1].p, cnt, st);
   });
 }
 int cb200_kyber_pack(uint8_t* out, const int16_t* polys, size_t n) { return codec_entry("cb200_kyber_pack", 0, 12, polys, out, n); }
