@@ -82,6 +82,20 @@ SYMBOLS = {
     "cb200_hybrid_shared_key_size": (C.c_size_t, [C.c_int]),
     "cb200_hybrid_seed_size": (C.c_size_t, [C.c_int]),
     "cb200_hybrid_encapsulation_seed_size": (C.c_size_t, [C.c_int]),
+    "cb200_hpke_keygen": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_encaps": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_size_t]),
+    "cb200_hpke_decaps": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_auth_encaps": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_auth_decaps": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                         C.c_void_p, C.c_size_t]),
+    "cb200_hpke_public_key_size": (C.c_size_t, [C.c_int]),
+    "cb200_hpke_private_key_size": (C.c_size_t, [C.c_int]),
+    "cb200_hpke_ciphertext_size": (C.c_size_t, [C.c_int]),
+    "cb200_hpke_shared_key_size": (C.c_size_t, [C.c_int]),
+    "cb200_hpke_seed_size": (C.c_size_t, [C.c_int]),
+    "cb200_hpke_encapsulation_seed_size": (C.c_size_t, [C.c_int]),
     "cb200_mldsa_sign": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
     "cb200_mldsa_verify": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,

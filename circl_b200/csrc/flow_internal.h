@@ -275,5 +275,12 @@ namespace hybrid {
 // outlen multiples of 8, rows 4-byte aligned.
 void shake256_rows(const uint8_t* in, size_t in_stride, int inlen, uint8_t* out, size_t out_stride, int outlen, size_t n,
                    cudaStream_t st);
+// out[i] = KeyGen(k[i]) when p is null, else Shared(k[i], p[i]), for X25519 (hybrid.cu x25519_base_kernel /
+// x25519_kernel) and X448 (x448_kernel), timed under KID_X25519 / KID_X448.  status[i] |= 1 where p[i] is of low order
+// (status may be null).  Rows 4-byte aligned; a stride of 0 reads one row for the whole batch.
+void x25519_rows(const uint8_t* k, size_t k_stride, const uint8_t* p, size_t p_stride, uint8_t* out, size_t out_stride,
+                 uint8_t* status, size_t n, cudaStream_t st);
+void x448_rows(const uint8_t* k, size_t k_stride, const uint8_t* p, size_t p_stride, uint8_t* out, size_t out_stride,
+               uint8_t* status, size_t n, cudaStream_t st);
 }  // namespace hybrid
 }  // namespace cb200

@@ -196,6 +196,14 @@ static void shake_launch(const uint8_t* in, size_t is, int inlen, uint8_t* out, 
 void shake256_rows(const uint8_t* in, size_t is, int inlen, uint8_t* out, size_t os, int outlen, size_t n, cudaStream_t st) {
   shake_launch(in, is, inlen, out, os, outlen, n, st);
 }
+void x25519_rows(const uint8_t* k, size_t ks_, const uint8_t* p, size_t ps, uint8_t* o, size_t os, uint8_t* status, size_t n,
+                 cudaStream_t st) {
+  x25519_launch(k, ks_, p, ps, o, os, status, n, st);
+}
+void x448_rows(const uint8_t* k, size_t ks_, const uint8_t* p, size_t ps, uint8_t* o, size_t os, uint8_t* status, size_t n,
+               cudaStream_t st) {
+  x448_launch(k, ks_, p, ps, o, os, status, n, st);
+}
 
 // ---- X-Wing (ML-KEM-768 + X25519): pk = ek || pk_X (1216), sk = seed (32), ct = ct_M || ct_X (1120)
 static int xwing_expand(const uint8_t* seeds, size_t stride, Arena& A, size_t n, cudaStream_t st, int slot, uint8_t** ek,

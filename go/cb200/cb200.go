@@ -597,6 +597,98 @@ func HybridEncaps(id int, pk []byte, shared bool, seeds, ct, ss []byte) error {
 	})
 }
 
+// HPKE DHKEM identifiers of include/circl_b200.h: the HPKE KEM ids themselves (hpke/algs.go:248-277).
+const (
+	HPKEX25519HKDFSHA256 = 0x20
+	HPKEX448HKDFSHA512   = 0x21
+)
+
+// hpkeSizes returns (N, ss) of a DHKEM id: N = key, enc and seed bytes (32 or 56), ss = shared secret bytes (32 or 64).
+func hpkeSizes(id int, fn string) (int, int) {
+	n := int(C.cb200_hpke_public_key_size(C.int(id)))
+	if n == 0 {
+		panic("cb200: " + fn + ": unknown HPKE KEM id")
+	}
+	return n, int(C.cb200_hpke_shared_key_size(C.int(id)))
+}
+
+// hpkeKey checks one key argument: a single key (shared by the batch, stride 0) or n keys back to back.
+func hpkeKey(k []byte, n, size int, fn string) (*C.uint8_t, C.size_t) {
+	switch len(k) {
+	case size:
+		return u8(k), 0
+	case n * size:
+		return u8(k), C.size_t(size)
+	}
+	panic("cb200: " + fn + ": key buffer has the wrong length")
+}
+
+// HPKEKeygen: batched DeriveKeyPair (hpke/xkem.go:55-71) on n seeds of N bytes; pk and sk: n*N bytes (sk unclamped).
+func HPKEKeygen(id int, seeds, pk, sk []byte) error {
+	N, _ := hpkeSizes(id, "HPKEKeygen")
+	n := len(seeds) / N
+	if len(seeds) != n*N || len(pk) != n*N || len(sk) != n*N {
+		panic("cb200: HPKEKeygen buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return call(func() C.int { return C.cb200_hpke_keygen(C.int(id), u8(seeds), u8(pk), u8(sk), C.size_t(n)) })
+}
+
+// HPKEEncaps: batched Encap, or AuthEncap when skS is not nil (hpke/kembase.go:120-183).  pkR and skS: one key or
+// n keys each; seeds and enc: n*N bytes; ss: n*SharedKeySize.  ErrPubKey (hpke.ErrInvalidKEMSharedSecret for the
+// caller) is returned after the whole batch ran if any operation met a low-order point; ok[i] (may be nil) tells which.
+func HPKEEncaps(id int, pkR, skS, seeds, enc, ss []byte, ok []bool) error {
+	N, S := hpkeSizes(id, "HPKEEncaps")
+	n := len(seeds) / N
+	if len(seeds) != n*N || len(enc) != n*N || len(ss) != n*S || (ok != nil && len(ok) != n) {
+		panic("cb200: HPKEEncaps buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	pr, prs := hpkeKey(pkR, n, N, "HPKEEncaps")
+	status := make([]byte, n)
+	err := call(func() C.int {
+		if skS == nil {
+			return C.cb200_hpke_encaps(C.int(id), pr, prs, u8(seeds), u8(enc), u8(ss), u8(status), C.size_t(n))
+		}
+		sp, sps := hpkeKey(skS, n, N, "HPKEEncaps")
+		return C.cb200_hpke_auth_encaps(C.int(id), pr, prs, sp, sps, u8(seeds), u8(enc), u8(ss), u8(status), C.size_t(n))
+	})
+	for i := range ok {
+		ok[i] = status[i] == 0
+	}
+	return err
+}
+
+// HPKEDecaps: batched Decap, or AuthDecap when pkS is not nil (hpke/kembase.go:185-241).  skR and pkS: one key or n
+// keys each (a single skR has its public key computed once); enc: n*N bytes; ss: n*SharedKeySize.  Errors as HPKEEncaps.
+func HPKEDecaps(id int, skR, enc, pkS, ss []byte, ok []bool) error {
+	N, S := hpkeSizes(id, "HPKEDecaps")
+	n := len(enc) / N
+	if len(enc) != n*N || len(ss) != n*S || (ok != nil && len(ok) != n) {
+		panic("cb200: HPKEDecaps buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	sr, srs := hpkeKey(skR, n, N, "HPKEDecaps")
+	status := make([]byte, n)
+	err := call(func() C.int {
+		if pkS == nil {
+			return C.cb200_hpke_decaps(C.int(id), sr, srs, u8(enc), u8(ss), u8(status), C.size_t(n))
+		}
+		pp, pps := hpkeKey(pkS, n, N, "HPKEDecaps")
+		return C.cb200_hpke_auth_decaps(C.int(id), sr, srs, u8(enc), pp, pps, u8(ss), u8(status), C.size_t(n))
+	})
+	for i := range ok {
+		ok[i] = status[i] == 0
+	}
+	return err
+}
+
 // PinnedBytes returns a Go slice over cudaHostAlloc'd memory: large batches should live
 // here so that host<->device copies run at full PCIe speed and overlap with the kernels.
 func PinnedBytes(n int) ([]byte, func()) {

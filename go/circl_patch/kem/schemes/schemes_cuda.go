@@ -1,7 +1,8 @@
 //go:build cuda && cgo
 
 // Drop-in file for github.com/cloudflare/circl/kem/schemes (next to schemes.go): with the `cuda` build tag the registry
-// entries "ML-KEM-768", "ML-KEM-1024" and "X-Wing" (kem/schemes/schemes.go:30-55) are served by the cb200 engine; every
+// entries "ML-KEM-768", "ML-KEM-1024", "X-Wing", "HPKE_KEM_X25519_HKDF_SHA256" and
+// "HPKE_KEM_X448_HKDF_SHA512" (kem/schemes/schemes.go:30-55) are served by the cb200 engine; every
 // other scheme, and every build without the tag, is untouched.  ByName keeps matching on the lower-cased Name()
 // (schemes.go:57-72), which the GPU schemes do not change.
 //
@@ -14,6 +15,7 @@ import (
 	"github.com/cloudflare/circl/kem"
 
 	"example.com/circl_b200/go/cb200"
+	"example.com/circl_b200/go/hpkecuda"
 	"example.com/circl_b200/go/mlkem1024cuda"
 	"example.com/circl_b200/go/mlkem768cuda"
 	"example.com/circl_b200/go/xwingcuda"
@@ -25,7 +27,8 @@ func init() {
 	if cb200.Init() != nil { // no usable H100: keep CIRCL's own schemes (the library itself has no CPU fallback)
 		return
 	}
-	for _, s := range []kem.Scheme{mlkem768cuda.Scheme(), mlkem1024cuda.Scheme(), xwingcuda.Scheme()} {
+	for _, s := range []kem.Scheme{mlkem768cuda.Scheme(), mlkem1024cuda.Scheme(), xwingcuda.Scheme(), hpkecuda.X25519(),
+		hpkecuda.X448()} {
 		name := strings.ToLower(s.Name())
 		allSchemeNames[name] = s
 		for i := range allSchemes {

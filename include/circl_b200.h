@@ -261,6 +261,37 @@ size_t cb200_hybrid_shared_key_size(int id);         /* 64 for ids 0-2, 88 for i
 size_t cb200_hybrid_seed_size(int id);               /* 64 for every id */
 size_t cb200_hybrid_encapsulation_seed_size(int id); /* 32 for ids 0-2, 56 for ids 3-4 */
 
+/* ---- HPKE DHKEMs (RFC 9180 section 4.1; hpke/kembase.go, hpke/xkem.go), as kem/schemes registers them ----
+ * The ids are the HPKE KEM identifiers.  X25519: seed, encapsulation seed, pk, sk and enc 32 bytes, ss 32 (HKDF-SHA256);
+ * X448: all 56 bytes, ss 64 (HKDF-SHA512).
+ * keygen = DeriveKeyPair (xkem.go:55-71): sk = LabeledExpand(LabeledExtract("", "dkp_prk", seed), "sk", "", Nsk),
+ *   stored unclamped; pk = KeyGen(sk).
+ * encaps = Encap with DeriveKeyPair(seed) as the ephemeral key (kembase.go:120-183); decaps = Decap (:185-241), which
+ *   recomputes pkR from skR.  auth_encaps / auth_decaps = AuthEncap / AuthDecap (:133-159,194-217) with the sender's
+ *   skS / pkS.  kem_context holds the key and enc bytes exactly as passed (X25519: bit 255 included).
+ * Strides: 0 = one key for the whole batch (its public key is then computed once per call).
+ * status: status[i] = 1 where a DH step met a low-order point (x25519/x448.Shared returning false); that op's ss is
+ *   all zero.  A host-pointer call finishes the batch and returns CB200_ERR_PUBKEY (the reference's
+ *   hpke.ErrInvalidKEMSharedSecret); a device-pointer call reports only through status, which it requires.
+ * An unknown id is CB200_ERR_ARG.  Device pointers and strides: 16-byte aligned for 0x20, 8-byte aligned for 0x21. */
+#define CB200_HPKE_X25519_HKDF_SHA256 0x20
+#define CB200_HPKE_X448_HKDF_SHA512 0x21
+int cb200_hpke_keygen(int id, const uint8_t *seeds, uint8_t *pk, uint8_t *sk, size_t n);
+int cb200_hpke_encaps(int id, const uint8_t *pkR, size_t pkR_stride, const uint8_t *seeds, uint8_t *enc, uint8_t *ss,
+                      uint8_t *status, size_t n);
+int cb200_hpke_decaps(int id, const uint8_t *skR, size_t skR_stride, const uint8_t *enc, uint8_t *ss, uint8_t *status,
+                      size_t n);
+int cb200_hpke_auth_encaps(int id, const uint8_t *pkR, size_t pkR_stride, const uint8_t *skS, size_t skS_stride,
+                           const uint8_t *seeds, uint8_t *enc, uint8_t *ss, uint8_t *status, size_t n);
+int cb200_hpke_auth_decaps(int id, const uint8_t *skR, size_t skR_stride, const uint8_t *enc, const uint8_t *pkS,
+                           size_t pkS_stride, uint8_t *ss, uint8_t *status, size_t n);
+size_t cb200_hpke_public_key_size(int id);
+size_t cb200_hpke_private_key_size(int id);
+size_t cb200_hpke_ciphertext_size(int id);
+size_t cb200_hpke_shared_key_size(int id);
+size_t cb200_hpke_seed_size(int id);
+size_t cb200_hpke_encapsulation_seed_size(int id);
+
 /* ---- ML-DSA (mode = 44, 65 or 87) and round-3 Dilithium (mode = 2, 3 or 5); sign/dilithium/gen.go:80-162 ----
  * Same contracts as the ML-DSA-65 entry points documented below, with the parameter set as first argument:
  *   ML-DSA-44 / 65 / 87 (sign/mldsa/mldsa{44,65,87}):    sk 2560 / 4032 / 4896, pk 1312 / 1952 / 2592, sig 2420 / 3309 / 4627

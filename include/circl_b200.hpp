@@ -61,6 +61,8 @@ struct ErrCiphertextSize : Error { ErrCiphertextSize() : Error("kem: invalid cip
 struct ErrPrivKeySize : Error { ErrPrivKeySize() : Error("kem: invalid private key size") {} };
 struct ErrPubKey : Error { ErrPubKey() : Error("kem: invalid public key") {} };
 struct ErrPrivKey : Error { ErrPrivKey() : Error("kem: invalid private key") {} };
+// hpke.ErrInvalidKEMSharedSecret (hpke/hpke.go:280): a DH step of an HPKE DHKEM met a low-order point
+struct ErrInvalidKEMSharedSecret : Error { ErrInvalidKEMSharedSecret() : Error("hpke: invalid KEM shared secret") {} };
 
 class Scheme;
 
@@ -95,24 +97,36 @@ class PrivateKey {  // kem.PrivateKey (kem/kem.go:22-30)
 //   XWING   X-Wing                         kem/xwing/scheme.go:1-140
 //   HYBRID  X25519MLKEM768, Kyber768-X25519, Kyber512-X25519,
 //           Kyber768-X448, Kyber1024-X448                      kem/hybrid/hybrid.go:76-315
+//   HPKE    HPKE_KEM_X25519_HKDF_SHA256, HPKE_KEM_X448_HKDF_SHA512   hpke/kembase.go, hpke/xkem.go; these are also
+//           kem.AuthScheme (kem/kem.go:84-90): the Auth* methods below serve them only
 class Scheme {
  public:
-  enum Kind { MLKEM, KYBER3, XWING, HYBRID };
+  enum Kind { MLKEM, KYBER3, XWING, HYBRID, HPKE };
   Scheme(std::string name, int k, bool round3 = false) : name_(std::move(name)), kind_(round3 ? KYBER3 : MLKEM), k_(k) {}
   Scheme(std::string name, Kind kind, int id) : name_(std::move(name)), kind_(kind), k_(id) {}
   const std::string& Name() const { return name_; }
   size_t CiphertextSize() const {
+    if (kind_ == HPKE) return cb200_hpke_ciphertext_size(k_);
     return kind_ == XWING ? 1120 : kind_ == HYBRID ? cb200_hybrid_ciphertext_size(k_) : cb200_mlkem_ciphertext_size(k_);
   }
-  size_t SharedKeySize() const { return kind_ == HYBRID ? cb200_hybrid_shared_key_size(k_) : 32; }
+  size_t SharedKeySize() const {
+    if (kind_ == HPKE) return cb200_hpke_shared_key_size(k_);
+    return kind_ == HYBRID ? cb200_hybrid_shared_key_size(k_) : 32;
+  }
   size_t PrivateKeySize() const {
+    if (kind_ == HPKE) return cb200_hpke_private_key_size(k_);
     return kind_ == XWING ? 32 : kind_ == HYBRID ? cb200_hybrid_private_key_size(k_) : cb200_mlkem_private_key_size(k_);
   }
   size_t PublicKeySize() const {
+    if (kind_ == HPKE) return cb200_hpke_public_key_size(k_);
     return kind_ == XWING ? 1216 : kind_ == HYBRID ? cb200_hybrid_public_key_size(k_) : cb200_mlkem_public_key_size(k_);
   }
-  size_t SeedSize() const { return kind_ == XWING ? 32 : kind_ == HYBRID ? cb200_hybrid_seed_size(k_) : 64; }
+  size_t SeedSize() const {
+    if (kind_ == HPKE) return cb200_hpke_seed_size(k_);
+    return kind_ == XWING ? 32 : kind_ == HYBRID ? cb200_hybrid_seed_size(k_) : 64;
+  }
   size_t EncapsulationSeedSize() const {
+    if (kind_ == HPKE) return cb200_hpke_encapsulation_seed_size(k_);
     return kind_ == XWING ? 64 : kind_ == HYBRID ? cb200_hybrid_encapsulation_seed_size(k_) : 32;
   }
 
@@ -122,7 +136,8 @@ class Scheme {
     DeriveKeyPairBatch(seed, ek, dk);
     return {PublicKey(this, std::move(ek)), PrivateKey(this, std::move(dk))};
   }
-  std::pair<PublicKey, PrivateKey> GenerateKeyPair() const {  // kyber.go:281-283
+  std::pair<PublicKey, PrivateKey> GenerateKeyPair() const;  // kyber.go:281-283; a random sk for HPKE (xkem.go:73-80)
+  std::pair<PublicKey, PrivateKey> GenerateFromSeed() const {
     Bytes seed(SeedSize());
     fill_random(seed.data(), seed.size());
     return DeriveKeyPair(seed);
@@ -137,7 +152,10 @@ class Scheme {
   }
   // (ct, ss)
   std::pair<Bytes, Bytes> EncapsulateDeterministically(const PublicKey& pk, const Bytes& seed) const {  // kyber.go:359-374
-    if (seed.size() != EncapsulationSeedSize()) throw ErrSeedSize();
+    if (seed.size() != EncapsulationSeedSize()) {
+      if (kind_ == HPKE) throw std::logic_error("kem: invalid seed size");  // DeriveKeyPair panics (xkem.go:60-62)
+      throw ErrSeedSize();
+    }
     if (pk.GetScheme() != this) throw ErrTypeMismatch();
     Bytes ct, ss;
     EncapsulateBatch(pk.MarshalBinary(), seed, ct, ss);
@@ -149,6 +167,8 @@ class Scheme {
     return EncapsulateDeterministically(pk, seed);
   }
   Bytes Decapsulate(const PrivateKey& sk, const Bytes& ct) const {  // kyber.go:376-388
+    // HPKE parses ct as a public key before it looks at the key's type (kembase.go:222)
+    if (kind_ == HPKE && ct.size() != CiphertextSize()) throw ErrPubKeySize();
     if (sk.GetScheme() != this) throw ErrTypeMismatch();
     if (ct.size() != CiphertextSize()) throw ErrCiphertextSize();
     Bytes ss;
@@ -170,6 +190,7 @@ class Scheme {
       case KYBER3: check(cb200_kyber_kem_encaps(k_, eks.data(), stride, seeds.data(), cts.data(), sss.data(), n)); break;
       case XWING: check(cb200_xwing_encaps(eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)); break;
       case HYBRID: check(cb200_hybrid_encaps(k_, eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)); break;
+      case HPKE: check(cb200_hpke_encaps(k_, eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)); break;
     }
   }
   void DecapsulateBatch(const Bytes& dks, const Bytes& cts, Bytes& sss) const {
@@ -194,6 +215,7 @@ class Scheme {
         }
         break;
       }
+      case HPKE: check(cb200_hpke_decaps(k_, dks.data(), stride, cts.data(), sss.data(), nullptr, n)); break;
     }
   }
   void DeriveKeyPairBatch(const Bytes& seeds, Bytes& eks, Bytes& dks) const {
@@ -209,14 +231,69 @@ class Scheme {
         dks = seeds;
         break;
       case HYBRID: check(cb200_hybrid_keygen(k_, seeds.data(), eks.data(), dks.data(), n)); break;
+      case HPKE: check(cb200_hpke_keygen(k_, seeds.data(), eks.data(), dks.data(), n)); break;
     }
+  }
+  // ---- kem.AuthScheme (HPKE only): (ct, ss) and ss
+  std::pair<Bytes, Bytes> AuthEncapsulateDeterministically(const PublicKey& pkr, const PrivateKey& sks,
+                                                           const Bytes& seed) const {  // kembase.go:108-112
+    auth_only();
+    if (seed.size() != EncapsulationSeedSize()) throw std::logic_error("kem: invalid seed size");
+    if (pkr.GetScheme() != this || sks.GetScheme() != this) throw ErrTypeMismatch();
+    Bytes ct, ss;
+    AuthEncapsulateBatch(pkr.MarshalBinary(), sks.MarshalBinary(), seed, ct, ss);
+    return {std::move(ct), std::move(ss)};
+  }
+  std::pair<Bytes, Bytes> AuthEncapsulate(const PublicKey& pkr, const PrivateKey& sks) const {
+    Bytes seed(EncapsulationSeedSize());
+    fill_random(seed.data(), seed.size());
+    return AuthEncapsulateDeterministically(pkr, sks, seed);
+  }
+  Bytes AuthDecapsulate(const PrivateKey& skr, const Bytes& ct, const PublicKey& pks) const {  // kembase.go:194-217
+    auth_only();
+    if (ct.size() != CiphertextSize()) throw ErrPubKeySize();
+    if (skr.GetScheme() != this || pks.GetScheme() != this) throw ErrTypeMismatch();
+    Bytes ss;
+    AuthDecapsulateBatch(skr.MarshalBinary(), ct, pks.MarshalBinary(), ss);
+    return ss;
+  }
+  // keys: one key (shared by the batch) or n keys back to back
+  void AuthEncapsulateBatch(const Bytes& pkrs, const Bytes& skss, const Bytes& seeds, Bytes& cts, Bytes& sss) const {
+    auth_only();
+    const size_t n = rows(seeds, EncapsulationSeedSize(), ErrSeedSize());
+    const size_t ps = key_stride(pkrs, n, PublicKeySize(), ErrPubKeySize()), ss = key_stride(skss, n, PrivateKeySize(), ErrPrivKeySize());
+    cts.resize(n * CiphertextSize());
+    sss.resize(n * SharedKeySize());
+    check(cb200_hpke_auth_encaps(k_, pkrs.data(), ps, skss.data(), ss, seeds.data(), cts.data(), sss.data(), nullptr, n));
+  }
+  void AuthDecapsulateBatch(const Bytes& skrs, const Bytes& cts, const Bytes& pkss, Bytes& sss) const {
+    auth_only();
+    const size_t n = rows(cts, CiphertextSize(), ErrPubKeySize());
+    const size_t ss = key_stride(skrs, n, PrivateKeySize(), ErrPrivKeySize()), ps = key_stride(pkss, n, PublicKeySize(), ErrPubKeySize());
+    sss.resize(n * SharedKeySize());
+    check(cb200_hpke_auth_decaps(k_, skrs.data(), ss, cts.data(), pkss.data(), ps, sss.data(), nullptr, n));
   }
   int k() const { return k_; }
   Kind kind() const { return kind_; }
 
  private:
-  static void check(int rc) {
+  void auth_only() const {
+    if (kind_ != HPKE) throw std::logic_error("kem: " + name_ + " is not a kem.AuthScheme");
+  }
+  template <class E>
+  static size_t rows(const Bytes& b, size_t unit, E err) {
+    if (b.size() % unit) throw err;
+    return b.size() / unit;
+  }
+  template <class E>
+  static size_t key_stride(const Bytes& keys, size_t n, size_t unit, E err) {
+    if (keys.size() == unit) return 0;
+    if (keys.size() != n * unit) throw err;
+    return unit;
+  }
+  void check(int rc) const {
     if (rc == 0) return;
+    if (rc == CB200_ERR_PUBKEY && kind_ == HPKE) throw ErrInvalidKEMSharedSecret();
     if (rc == CB200_ERR_PUBKEY) throw ErrPubKey();
     if (rc == CB200_ERR_PRIVKEY) throw ErrPrivKey();
     if (rc == CB200_ERR_ARG) throw std::logic_error(cb200_last_error());
@@ -224,11 +301,17 @@ class Scheme {
   }
   std::string name_;
   Kind kind_;
-  int k_;  // K of the lattice scheme, or the hybrid identifier
+  int k_;  // K of the lattice scheme, or the hybrid / HPKE KEM identifier
 };
 
 inline PublicKey PrivateKey::Public() const {
   const Scheme* s = scheme_;
+  if (s->kind() == Scheme::HPKE) {  // KeyGen of the stored (unclamped) key (xkem.go:146-163)
+    Bytes pk(s->PublicKeySize());
+    if ((pk.size() == 56 ? cb200_x448 : cb200_x25519)(packed_.data(), nullptr, pk.data(), nullptr, 1))
+      throw Error(cb200_last_error());
+    return PublicKey(s, std::move(pk));
+  }
   if (s->kind() == Scheme::XWING) {  // sk is the seed: derive again (xwing.go:278-281)
     Bytes pk, sk;
     s->DeriveKeyPairBatch(packed_, pk, sk);
@@ -248,6 +331,14 @@ inline PublicKey PrivateKey::Public() const {
   }
   const int k = s->k();
   return PublicKey(s, Bytes(packed_.begin() + 384 * k, packed_.begin() + 384 * k + 384 * k + 32));
+}
+
+inline std::pair<PublicKey, PrivateKey> Scheme::GenerateKeyPair() const {
+  if (kind_ != HPKE) return GenerateFromSeed();
+  Bytes sk(PrivateKeySize());
+  fill_random(sk.data(), sk.size());
+  PrivateKey priv(this, std::move(sk));
+  return {priv.Public(), priv};
 }
 
 inline std::string lower(std::string s) {
@@ -270,6 +361,22 @@ inline const Scheme* ByName(const std::string& name) {  // kem/schemes/schemes.g
     if (lower(s->Name()) == lower(name)) return s;
   return nullptr;
 }
+
+// HPKE's two Montgomery-curve DHKEMs (kem/schemes/schemes.go:35-55) are registered on their own so that All()
+// above keeps its twelve schemes.
+namespace hpke {
+inline const std::vector<const Scheme*>& All() {
+  static const Scheme x25519("HPKE_KEM_X25519_HKDF_SHA256", Scheme::HPKE, CB200_HPKE_X25519_HKDF_SHA256),
+      x448("HPKE_KEM_X448_HKDF_SHA512", Scheme::HPKE, CB200_HPKE_X448_HKDF_SHA512);
+  static const std::vector<const Scheme*> all = {&x25519, &x448};
+  return all;
+}
+inline const Scheme* ByName(const std::string& name) {  // case-insensitive; nullptr = no such scheme
+  for (const Scheme* s : All())
+    if (lower(s->Name()) == lower(name)) return s;
+  return nullptr;
+}
+}  // namespace hpke
 
 }  // namespace kem
 

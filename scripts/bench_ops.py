@@ -136,6 +136,88 @@ def ed448_lines(res):
     torch.cuda.empty_cache()
 
 
+def hpke_lines(res):
+    """HPKE DHKEM(X25519, HKDF-SHA256) and DHKEM(X448, HKDF-SHA512) through the C ABI, device-resident, 2^18 operations,
+    per-op and shared receiver keys, with X25519 / X448 KeyGen and Shared of the same run beside them; the time of the
+    KDF kernels alone (profiling class hpke) is read for the per-op Encaps and Decaps lines."""
+    import subprocess
+    from circl_b200 import hybrid, x448
+    from circl_b200._ffi import check, lib
+    L = lib()
+    check(L.cb200_set_stream(torch.cuda.current_stream().cuda_stream))
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                           text=True, timeout=30).stdout.strip().splitlines()
+        res["card"] = q[0] if q else "unknown"
+    except (OSError, subprocess.SubprocessError):
+        res["card"] = "unknown"
+    n = 1 << 18
+    g = torch.Generator(device="cuda").manual_seed(13)
+    names = L.cb200_profile_kernel_count()
+    hpke_kid = [L.cb200_profile_kernel_name(i).decode() for i in range(names)].index("hpke")
+
+    def kdf_ms(fn):
+        """(wall ms, KDF kernel ms) of one call, with per-kernel event timing on."""
+        import ctypes as C
+        check(L.cb200_profile_enable(1))
+        fn()
+        torch.cuda.synchronize()
+        ms = (C.c_double * names)()
+        cnt = (C.c_uint64 * names)()
+        check(L.cb200_profile_read(ms, cnt, names))
+        check(L.cb200_profile_enable(0))
+        return ms[hpke_kid]
+
+    for kid, w, nss, curve in ((0x20, 32, 32, "X25519"), (0x21, 56, 64, "X448")):
+        name = "DHKEM(X25519, HKDF-SHA256)" if kid == 0x20 else "DHKEM(X448, HKDF-SHA512)"
+        k = torch.randint(0, 256, (n, w), generator=g, device="cuda", dtype=torch.uint8)
+        kg, sh = (hybrid.x25519_keygen, hybrid.x25519_shared) if kid == 0x20 else (x448.x448_keygen, x448.x448_shared)
+        t = timed(lambda: kg(k), steps=3)
+        pub = kg(k)
+        res[f"{curve} KeyGen"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+        t = timed(lambda: sh(k, pub), steps=3)
+        res[f"{curve} Shared"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+        del pub
+        seeds = torch.randint(0, 256, (n, w), generator=g, device="cuda", dtype=torch.uint8)
+        pk = torch.empty((n, w), dtype=torch.uint8, device="cuda")
+        sk = torch.empty((n, w), dtype=torch.uint8, device="cuda")
+        enc = torch.empty((n, w), dtype=torch.uint8, device="cuda")
+        ss = torch.empty((n, nss), dtype=torch.uint8, device="cuda")
+        ss2 = torch.empty((n, nss), dtype=torch.uint8, device="cuda")
+        st = torch.zeros((n,), dtype=torch.uint8, device="cuda")
+        P = lambda x: x.data_ptr()  # noqa: E731
+        ops = {
+            "KeyGen": lambda: check(L.cb200_hpke_keygen(kid, P(seeds), P(pk), P(sk), n)),
+            "Encaps": lambda: check(L.cb200_hpke_encaps(kid, P(pk), w, P(k), P(enc), P(ss), P(st), n)),
+            "Decaps": lambda: check(L.cb200_hpke_decaps(kid, P(sk), w, P(enc), P(ss2), P(st), n)),
+            "Encaps (shared pkR)": lambda: check(L.cb200_hpke_encaps(kid, P(pk), 0, P(k), P(enc), P(ss), P(st), n)),
+            "Decaps (shared skR)": lambda: check(L.cb200_hpke_decaps(kid, P(sk), 0, P(enc), P(ss2), P(st), n)),
+            "AuthEncaps": lambda: check(L.cb200_hpke_auth_encaps(kid, P(pk), w, P(sk), w, P(k), P(enc), P(ss), P(st), n)),
+            "AuthDecaps": lambda: check(L.cb200_hpke_auth_decaps(kid, P(sk), w, P(enc), P(pk), w, P(ss2), P(st), n)),
+            "AuthEncaps (shared pkR, skS)": lambda: check(L.cb200_hpke_auth_encaps(kid, P(pk), 0, P(sk), 0, P(k), P(enc),
+                                                                                   P(ss), P(st), n)),
+            "AuthDecaps (shared skR, pkS)": lambda: check(L.cb200_hpke_auth_decaps(kid, P(sk), 0, P(enc), P(pk), 0,
+                                                                                   P(ss2), P(st), n)),
+        }
+        for op, fn in ops.items():
+            t = timed(fn, steps=3)
+            line = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
+            if op in ("KeyGen", "Encaps", "Decaps"):
+                line["kdf_ms"] = kdf_ms(fn)
+            if op.startswith("Decaps") or op.startswith("AuthDecaps"):
+                torch.cuda.synchronize()
+                line["roundtrip_ok"] = bool(torch.equal(ss, ss2)) and st.sum().item() == 0
+            res[f"{name} {op}"] = line
+        del k, seeds, pk, sk, enc, ss, ss2, st
+        torch.cuda.empty_cache()
+
+
+if "--hpke" in sys.argv:  # only the HPKE lines above and the curve lines they are compared with
+    hpke_lines(res)
+    print(json.dumps(res, indent=1))
+    sys.exit(0)
+
+
 if "--ed448" in sys.argv:  # only the Ed448 lines above and the X448 lines they are compared with
     ed448_lines(res)
     print(json.dumps(res, indent=1))
