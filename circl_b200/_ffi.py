@@ -96,6 +96,15 @@ SYMBOLS = {
     "cb200_hpke_shared_key_size": (C.c_size_t, [C.c_int]),
     "cb200_hpke_seed_size": (C.c_size_t, [C.c_int]),
     "cb200_hpke_encapsulation_seed_size": (C.c_size_t, [C.c_int]),
+    "cb200_frodo640shake_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_frodo640shake_encaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_frodo640shake_decaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_frodo640shake_public_key_size": (C.c_size_t, []),
+    "cb200_frodo640shake_private_key_size": (C.c_size_t, []),
+    "cb200_frodo640shake_ciphertext_size": (C.c_size_t, []),
+    "cb200_frodo640shake_shared_key_size": (C.c_size_t, []),
+    "cb200_frodo640shake_seed_size": (C.c_size_t, []),
+    "cb200_frodo640shake_encapsulation_seed_size": (C.c_size_t, []),
     "cb200_mldsa_sign": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]),
     "cb200_mldsa_verify": (C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,

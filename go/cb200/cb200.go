@@ -612,7 +612,8 @@ func hpkeSizes(id int, fn string) (int, int) {
 	return n, int(C.cb200_hpke_shared_key_size(C.int(id)))
 }
 
-// hpkeKey checks one key argument: a single key (shared by the batch, stride 0) or n keys back to back.
+// hpkeKey checks one key argument: a single key (shared by the batch, stride 0) or n keys back to back.  The
+// FrodoKEM calls use it too.
 func hpkeKey(k []byte, n, size int, fn string) (*C.uint8_t, C.size_t) {
 	switch len(k) {
 	case size:
@@ -687,6 +688,59 @@ func HPKEDecaps(id int, skR, enc, pkS, ss []byte, ok []bool) error {
 		ok[i] = status[i] == 0
 	}
 	return err
+}
+
+// FrodoKEM-640-SHAKE sizes (kem/frodo/frodo640shake/frodo.go:32-51).
+const (
+	Frodo640SHAKEPublicKeySize         = 9616
+	Frodo640SHAKEPrivateKeySize        = 19888
+	Frodo640SHAKECiphertextSize        = 9720
+	Frodo640SHAKESharedKeySize         = 16
+	Frodo640SHAKESeedSize              = 48
+	Frodo640SHAKEEncapsulationSeedSize = 16
+)
+
+// Frodo640SHAKEKeygen: batched DeriveKeyPair (frodo.go:84-135) on n seeds of 48 bytes; pk: n*9616, sk: n*19888.
+func Frodo640SHAKEKeygen(seeds, pk, sk []byte) error {
+	n := len(seeds) / Frodo640SHAKESeedSize
+	if len(seeds) != n*Frodo640SHAKESeedSize || len(pk) != n*Frodo640SHAKEPublicKeySize ||
+		len(sk) != n*Frodo640SHAKEPrivateKeySize {
+		panic("cb200: Frodo640SHAKEKeygen buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return call(func() C.int { return C.cb200_frodo640shake_keygen(u8(seeds), u8(pk), u8(sk), C.size_t(n)) })
+}
+
+// Frodo640SHAKEEncaps: batched EncapsulateDeterministically (frodo.go:160-240).  pk: one packed key (shared by the
+// batch: A and H(pk) are computed once and S'A runs as one tensor-core GEMM) or n keys; seeds: n*16 bytes; ct: n*9720;
+// ss: n*16.  FrodoKEM has no failing inputs.
+func Frodo640SHAKEEncaps(pk, seeds, ct, ss []byte) error {
+	n := len(seeds) / Frodo640SHAKEEncapsulationSeedSize
+	if len(seeds) != n*Frodo640SHAKEEncapsulationSeedSize || len(ct) != n*Frodo640SHAKECiphertextSize ||
+		len(ss) != n*Frodo640SHAKESharedKeySize {
+		panic("cb200: Frodo640SHAKEEncaps buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	p, ps := hpkeKey(pk, n, Frodo640SHAKEPublicKeySize, "Frodo640SHAKEEncaps")
+	return call(func() C.int { return C.cb200_frodo640shake_encaps(p, ps, u8(seeds), u8(ct), u8(ss), C.size_t(n)) })
+}
+
+// Frodo640SHAKEDecaps: batched Decapsulate (frodo.go:247-329).  sk: one packed key (shared by the batch) or n keys;
+// ct: n*9720 bytes; ss: n*16.  Never fails: a ciphertext that does not re-encrypt gives F(ct || s).
+func Frodo640SHAKEDecaps(sk, ct, ss []byte) error {
+	n := len(ct) / Frodo640SHAKECiphertextSize
+	if len(ct) != n*Frodo640SHAKECiphertextSize || len(ss) != n*Frodo640SHAKESharedKeySize {
+		panic("cb200: Frodo640SHAKEDecaps buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	k, ks := hpkeKey(sk, n, Frodo640SHAKEPrivateKeySize, "Frodo640SHAKEDecaps")
+	return call(func() C.int { return C.cb200_frodo640shake_decaps(k, ks, u8(ct), u8(ss), C.size_t(n)) })
 }
 
 // PinnedBytes returns a Go slice over cudaHostAlloc'd memory: large batches should live

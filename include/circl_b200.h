@@ -292,6 +292,25 @@ size_t cb200_hpke_shared_key_size(int id);
 size_t cb200_hpke_seed_size(int id);
 size_t cb200_hpke_encapsulation_seed_size(int id);
 
+/* ---- FrodoKEM-640-SHAKE (kem/frodo/frodo640shake), the only parameter set the reference has ----
+ * Sizes: pk 9616, sk 19888, ct 9720, ss 16, seed 48 (s || seedSE || z), encapsulation seed 16 (mu).
+ * keygen = DeriveKeyPair (frodo.go:84-135); encaps = EncapsulateDeterministically (:160-240); decaps = Decapsulate
+ *   (:247-329), which never fails: a ciphertext that does not re-encrypt gives F(ct || s) (implicit rejection), and
+ *   keys are not validated, as in the reference (Unpack reads any bytes).  So there is no status array.
+ * Strides: 0 = one key for the whole batch.  Then A and H(pk) are computed once per call and S'A runs as one
+ *   tensor-core GEMM over the batch; the bytes are the same as with the key repeated at full stride.
+ * Device pointers and strides: 8-byte aligned (a contiguous batch of 9720-byte ciphertexts is not 16-byte aligned). */
+int cb200_frodo640shake_keygen(const uint8_t *seeds, uint8_t *pk, uint8_t *sk, size_t n);
+int cb200_frodo640shake_encaps(const uint8_t *pk, size_t pk_stride, const uint8_t *seeds, uint8_t *ct, uint8_t *ss,
+                               size_t n);
+int cb200_frodo640shake_decaps(const uint8_t *sk, size_t sk_stride, const uint8_t *ct, uint8_t *ss, size_t n);
+size_t cb200_frodo640shake_public_key_size(void);
+size_t cb200_frodo640shake_private_key_size(void);
+size_t cb200_frodo640shake_ciphertext_size(void);
+size_t cb200_frodo640shake_shared_key_size(void);
+size_t cb200_frodo640shake_seed_size(void);
+size_t cb200_frodo640shake_encapsulation_seed_size(void);
+
 /* ---- ML-DSA (mode = 44, 65 or 87) and round-3 Dilithium (mode = 2, 3 or 5); sign/dilithium/gen.go:80-162 ----
  * Same contracts as the ML-DSA-65 entry points documented below, with the parameter set as first argument:
  *   ML-DSA-44 / 65 / 87 (sign/mldsa/mldsa{44,65,87}):    sk 2560 / 4032 / 4896, pk 1312 / 1952 / 2592, sig 2420 / 3309 / 4627

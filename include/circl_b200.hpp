@@ -99,34 +99,41 @@ class PrivateKey {  // kem.PrivateKey (kem/kem.go:22-30)
 //           Kyber768-X448, Kyber1024-X448                      kem/hybrid/hybrid.go:76-315
 //   HPKE    HPKE_KEM_X25519_HKDF_SHA256, HPKE_KEM_X448_HKDF_SHA512   hpke/kembase.go, hpke/xkem.go; these are also
 //           kem.AuthScheme (kem/kem.go:84-90): the Auth* methods below serve them only
+//   FRODO   FrodoKEM-640-SHAKE             kem/frodo/frodo640shake/frodo.go:405-547
 class Scheme {
  public:
-  enum Kind { MLKEM, KYBER3, XWING, HYBRID, HPKE };
+  enum Kind { MLKEM, KYBER3, XWING, HYBRID, HPKE, FRODO };
   Scheme(std::string name, int k, bool round3 = false) : name_(std::move(name)), kind_(round3 ? KYBER3 : MLKEM), k_(k) {}
   Scheme(std::string name, Kind kind, int id) : name_(std::move(name)), kind_(kind), k_(id) {}
   const std::string& Name() const { return name_; }
   size_t CiphertextSize() const {
     if (kind_ == HPKE) return cb200_hpke_ciphertext_size(k_);
+    if (kind_ == FRODO) return cb200_frodo640shake_ciphertext_size();
     return kind_ == XWING ? 1120 : kind_ == HYBRID ? cb200_hybrid_ciphertext_size(k_) : cb200_mlkem_ciphertext_size(k_);
   }
   size_t SharedKeySize() const {
     if (kind_ == HPKE) return cb200_hpke_shared_key_size(k_);
+    if (kind_ == FRODO) return cb200_frodo640shake_shared_key_size();
     return kind_ == HYBRID ? cb200_hybrid_shared_key_size(k_) : 32;
   }
   size_t PrivateKeySize() const {
     if (kind_ == HPKE) return cb200_hpke_private_key_size(k_);
+    if (kind_ == FRODO) return cb200_frodo640shake_private_key_size();
     return kind_ == XWING ? 32 : kind_ == HYBRID ? cb200_hybrid_private_key_size(k_) : cb200_mlkem_private_key_size(k_);
   }
   size_t PublicKeySize() const {
     if (kind_ == HPKE) return cb200_hpke_public_key_size(k_);
+    if (kind_ == FRODO) return cb200_frodo640shake_public_key_size();
     return kind_ == XWING ? 1216 : kind_ == HYBRID ? cb200_hybrid_public_key_size(k_) : cb200_mlkem_public_key_size(k_);
   }
   size_t SeedSize() const {
     if (kind_ == HPKE) return cb200_hpke_seed_size(k_);
+    if (kind_ == FRODO) return cb200_frodo640shake_seed_size();
     return kind_ == XWING ? 32 : kind_ == HYBRID ? cb200_hybrid_seed_size(k_) : 64;
   }
   size_t EncapsulationSeedSize() const {
     if (kind_ == HPKE) return cb200_hpke_encapsulation_seed_size(k_);
+    if (kind_ == FRODO) return cb200_frodo640shake_encapsulation_seed_size();
     return kind_ == XWING ? 64 : kind_ == HYBRID ? cb200_hybrid_encapsulation_seed_size(k_) : 32;
   }
 
@@ -169,6 +176,8 @@ class Scheme {
   Bytes Decapsulate(const PrivateKey& sk, const Bytes& ct) const {  // kyber.go:376-388
     // HPKE parses ct as a public key before it looks at the key's type (kembase.go:222)
     if (kind_ == HPKE && ct.size() != CiphertextSize()) throw ErrPubKeySize();
+    // FrodoKEM checks the ciphertext length before the key's type (frodo.go:517-525)
+    if (kind_ == FRODO && ct.size() != CiphertextSize()) throw ErrCiphertextSize();
     if (sk.GetScheme() != this) throw ErrTypeMismatch();
     if (ct.size() != CiphertextSize()) throw ErrCiphertextSize();
     Bytes ss;
@@ -191,6 +200,7 @@ class Scheme {
       case XWING: check(cb200_xwing_encaps(eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)); break;
       case HYBRID: check(cb200_hybrid_encaps(k_, eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)); break;
       case HPKE: check(cb200_hpke_encaps(k_, eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)); break;
+      case FRODO: check(cb200_frodo640shake_encaps(eks.data(), stride, seeds.data(), cts.data(), sss.data(), n)); break;
     }
   }
   void DecapsulateBatch(const Bytes& dks, const Bytes& cts, Bytes& sss) const {
@@ -216,6 +226,7 @@ class Scheme {
         break;
       }
       case HPKE: check(cb200_hpke_decaps(k_, dks.data(), stride, cts.data(), sss.data(), nullptr, n)); break;
+      case FRODO: check(cb200_frodo640shake_decaps(dks.data(), stride, cts.data(), sss.data(), n)); break;
     }
   }
   void DeriveKeyPairBatch(const Bytes& seeds, Bytes& eks, Bytes& dks) const {
@@ -232,6 +243,7 @@ class Scheme {
         break;
       case HYBRID: check(cb200_hybrid_keygen(k_, seeds.data(), eks.data(), dks.data(), n)); break;
       case HPKE: check(cb200_hpke_keygen(k_, seeds.data(), eks.data(), dks.data(), n)); break;
+      case FRODO: check(cb200_frodo640shake_keygen(seeds.data(), eks.data(), dks.data(), n)); break;
     }
   }
   // ---- kem.AuthScheme (HPKE only): (ct, ss) and ss
@@ -312,6 +324,8 @@ inline PublicKey PrivateKey::Public() const {
       throw Error(cb200_last_error());
     return PublicKey(s, std::move(pk));
   }
+  if (s->kind() == Scheme::FRODO)  // the embedded public key (frodo.go:466-468)
+    return PublicKey(s, Bytes(packed_.begin() + 16, packed_.begin() + 16 + s->PublicKeySize()));
   if (s->kind() == Scheme::XWING) {  // sk is the seed: derive again (xwing.go:278-281)
     Bytes pk, sk;
     s->DeriveKeyPairBatch(packed_, pk, sk);
@@ -377,6 +391,20 @@ inline const Scheme* ByName(const std::string& name) {  // case-insensitive; nul
   return nullptr;
 }
 }  // namespace hpke
+
+// FrodoKEM-640-SHAKE (kem/schemes/schemes.go entry 6), registered on its own like the HPKE DHKEMs.
+namespace frodo {
+inline const std::vector<const Scheme*>& All() {
+  static const Scheme f("FrodoKEM-640-SHAKE", Scheme::FRODO, 0);
+  static const std::vector<const Scheme*> all = {&f};
+  return all;
+}
+inline const Scheme* ByName(const std::string& name) {  // case-insensitive; nullptr = no such scheme
+  for (const Scheme* s : All())
+    if (lower(s->Name()) == lower(name)) return s;
+  return nullptr;
+}
+}  // namespace frodo
 
 }  // namespace kem
 

@@ -212,6 +212,85 @@ def hpke_lines(res):
         torch.cuda.empty_cache()
 
 
+def frodo_lines(res):
+    """FrodoKEM-640-SHAKE through the C ABI, device-resident, 2^16 operations: KeyGen, Encaps and Decaps with per-op
+    keys, Encaps with one shared pk and Decaps with one shared sk (the tensor-core path), each with the time of its
+    frodo and frodo_gemm kernels (profiling classes) read in a separate profiled call; and the oracle's batch function
+    on every host thread over the same 2^16 operations, its outputs compared with the GPU's."""
+    import ctypes as C
+    import subprocess
+    from circl_b200._ffi import check, lib
+    from oracle import frodo as O
+    L = lib()
+    check(L.cb200_set_stream(torch.cuda.current_stream().cuda_stream))
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                           text=True, timeout=30).stdout.strip().splitlines()
+        res["card"] = q[0] if q else "unknown"
+    except (OSError, subprocess.SubprocessError):
+        res["card"] = "unknown"
+    n = 1 << 16
+    g = torch.Generator(device="cuda").manual_seed(17)
+    names = L.cb200_profile_kernel_count()
+    kn = [L.cb200_profile_kernel_name(i).decode() for i in range(names)]
+    fk, gk = kn.index("frodo"), kn.index("frodo_gemm")
+
+    def split_ms(fn):
+        check(L.cb200_profile_enable(1))
+        fn()
+        torch.cuda.synchronize()
+        ms, cnt = (C.c_double * names)(), (C.c_uint64 * names)()
+        check(L.cb200_profile_read(ms, cnt, names))
+        check(L.cb200_profile_enable(0))
+        return ms[fk], ms[gk]
+
+    seeds = torch.randint(0, 256, (n, 48), generator=g, device="cuda", dtype=torch.uint8)
+    es = torch.randint(0, 256, (n, 16), generator=g, device="cuda", dtype=torch.uint8)
+    pk = torch.empty((n, 9616), dtype=torch.uint8, device="cuda")
+    sk = torch.empty((n, 19888), dtype=torch.uint8, device="cuda")
+    ct = torch.empty((n, 9720), dtype=torch.uint8, device="cuda")
+    ct0 = torch.empty((n, 9720), dtype=torch.uint8, device="cuda")
+    ss, ss2 = (torch.empty((n, 16), dtype=torch.uint8, device="cuda") for _ in range(2))
+    ss0, ss02 = (torch.empty((n, 16), dtype=torch.uint8, device="cuda") for _ in range(2))
+    P = lambda x: x.data_ptr()  # noqa: E731
+    ops = {
+        "KeyGen": lambda: check(L.cb200_frodo640shake_keygen(P(seeds), P(pk), P(sk), n)),
+        "Encaps": lambda: check(L.cb200_frodo640shake_encaps(P(pk), 9616, P(es), P(ct), P(ss), n)),
+        "Decaps": lambda: check(L.cb200_frodo640shake_decaps(P(sk), 19888, P(ct), P(ss2), n)),
+        "Encaps (shared pk)": lambda: check(L.cb200_frodo640shake_encaps(P(pk), 0, P(es), P(ct0), P(ss0), n)),
+        "Decaps (shared sk)": lambda: check(L.cb200_frodo640shake_decaps(P(sk), 0, P(ct0), P(ss02), n)),
+    }
+    for op, fn in ops.items():
+        t = timed(fn, steps=3)
+        f_ms, g_ms = split_ms(fn)
+        line = {"n": n, "ms": t, "per_s": n / (t * 1e-3), "frodo_ms": f_ms, "frodo_gemm_ms": g_ms}
+        if op.startswith("Decaps"):
+            torch.cuda.synchronize()
+            line["roundtrip_ok"] = bool(torch.equal(ss, ss2)) if op == "Decaps" else bool(torch.equal(ss0, ss02))
+        res[f"FrodoKEM-640-SHAKE {op}"] = line
+    threads = os.cpu_count() or 1
+    hs, hes, hpk, hsk, hct = (x.cpu().numpy() for x in (seeds, es, pk, sk, ct))
+    import time
+    for op, fn in (("KeyGen", lambda: O.keygen_batch(hs, threads)), ("Encaps", lambda: O.encaps_batch(hpk, hes, threads)),
+                   ("Decaps", lambda: O.decaps_batch(hsk, hct, threads))):
+        t0 = time.perf_counter()
+        out = fn()
+        dt = time.perf_counter() - t0
+        res[f"FrodoKEM-640-SHAKE {op} oracle"] = {"n": n, "threads": threads, "ms": dt * 1e3, "per_s": n / dt}
+        gpu = (pk, sk) if op == "KeyGen" else (ct, ss) if op == "Encaps" else (ss2,)
+        out = out if isinstance(out, tuple) else (out,)
+        res[f"FrodoKEM-640-SHAKE {op} oracle"]["matches_gpu"] = all(
+            bool(np.array_equal(o, g.cpu().numpy())) for o, g in zip(out, gpu))
+    del seeds, es, pk, sk, ct, ct0, ss, ss2, ss0, ss02
+    torch.cuda.empty_cache()
+
+
+if "--frodo" in sys.argv:  # only the FrodoKEM lines above
+    frodo_lines(res)
+    print(json.dumps(res, indent=1))
+    sys.exit(0)
+
+
 if "--hpke" in sys.argv:  # only the HPKE lines above and the curve lines they are compared with
     hpke_lines(res)
     print(json.dumps(res, indent=1))

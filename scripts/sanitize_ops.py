@@ -63,5 +63,24 @@ xpk, xsk = xw.DeriveKeyPairBatch(rng.integers(0, 256, size=(9, 32), dtype=np.uin
 es = rng.integers(0, 256, size=(9, 64), dtype=np.uint8)
 xct, xss = xw.EncapsulateBatch(xpk, es)
 assert np.array_equal(xw.DecapsulateBatch(xsk, xct), xss)
+
+# FrodoKEM-640-SHAKE at n = 33: every kernel of csrc/frodo.cu -- the per-op path (A staged through shared memory, the
+# B' compare folded with __syncthreads_or), the shared-key path (A planes, the GEMM and its cross-CTA atomicOr on the
+# compare flag), implicit rejection in the B' and C parts
+from circl_b200 import frodo  # noqa: E402
+from oracle import frodo as oracle_frodo  # noqa: E402
+fk = frodo.Scheme()
+fpk, fsk = fk.DeriveKeyPairBatch(rng.integers(0, 256, size=(33, 48), dtype=np.uint8))
+fes = rng.integers(0, 256, size=(33, 16), dtype=np.uint8)
+fct, fss = fk.EncapsulateBatch(fpk, fes)
+fbad = fct.copy()
+fbad[::3, 17] ^= 1
+fbad[1::3, 9700] ^= 1
+assert fk.DecapsulateBatch(fsk, fbad)[0].tobytes() == oracle_frodo.decaps(fsk[0].tobytes(), fbad[0].tobytes())
+pk0, sk0 = fk.UnmarshalBinaryPublicKey(fpk[0].tobytes()), fk.UnmarshalBinaryPrivateKey(fsk[0].tobytes())
+sct, sss = fk.EncapsulateBatch(pk0, fes)
+assert (sct[32].tobytes(), sss[32].tobytes()) == oracle_frodo.encaps(fpk[0].tobytes(), fes[32].tobytes())
+sct[::2, 40] ^= 4
+assert fk.DecapsulateBatch(sk0, sct)[2].tobytes() == oracle_frodo.decaps(fsk[0].tobytes(), sct[2].tobytes())
 circl_b200.shutdown()
 print("sanitize_ops ok")
