@@ -494,18 +494,11 @@ __device__ __forceinline__ int32_t dp2a_hi_us(uint32_t a, uint32_t b, int32_t c)
   asm("dp2a.hi.u32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
   return d;
 }
-// montReduce(p) << 16 for a 32-bit signed p (field.go:4-32)
-__device__ __forceinline__ int32_t mont_red_hi(int32_t p) {
+// montReduce(p) of a 32-bit signed p (field.go:4-32) as a plain sign-extended value
+__device__ __forceinline__ int32_t mont_red_lo(int32_t p) {
   const int32_t m = (int32_t)((uint32_t)p * (kyber::QINV << 16)) >> 16;
-  return p - m * Q;
+  return (p - m * Q) >> 16;
 }
-// montReduce(p) as a plain sign-extended value
-__device__ __forceinline__ int32_t mont_red_lo(int32_t p) { return mont_red_hi(p) >> 16; }
-// Compress_q(x, d) (poly.go:248-328) from ANY representative x of the residue with |x| < 2^15, high-half register:
-// round(x 2^d / q) mod 2^d does not change when a multiple of q is added to x, so x + 10 q in [0, 2^16) is compressed
-// directly -- floor((x' 2^d + 1664) / q) as a 32 x 32 -> 64 multiplication by ceil(2^40 / q), exact below 2^28 -- and the
-// Normalize of cpapke.go:176-177 needs no instruction of its own.  Checked exhaustively against the reference's two
-// constant pairs for every 16-bit x' and d in {4, 5, 10, 11} (tests/test_compress_identity.py).
 // hi32(a * b) as a wide multiplication (IMAD.WIDE.U32) rather than the IMAD.HI.U32 __umulhi compiles to; the issue rates
 // of the two are what scripts/ubench_pipes.cu measures
 __device__ __forceinline__ uint32_t umulhi_wide(uint32_t a, uint32_t b) {
@@ -513,25 +506,23 @@ __device__ __forceinline__ uint32_t umulhi_wide(uint32_t a, uint32_t b) {
   asm("{ .reg .b64 t; mul.wide.u32 t, %1, %2; mov.b64 {_, %0}, t; }" : "=r"(hi) : "r"(a), "r"(b));
   return hi;
 }
+// Compress_q(x, d) (poly.go:248-328) from ANY representative x of the residue with |x| < 2^15, low-format register:
+// round(x 2^d / q) mod 2^d does not change when a multiple of q is added to x, so x + 10 q in [0, 2^16) is compressed
+// directly -- floor((x' 2^d + 1664) / q) as a 32 x 32 -> 64 multiplication by ceil(2^40 / q), exact below 2^28 -- and the
+// Normalize of cpapke.go:176-177 needs no instruction of its own.  Checked exhaustively against the reference's two
+// constant pairs for every 16-bit x' and d in {4, 5, 10, 11} (tests/test_compress_identity.py).
 template <int D>
-__device__ __forceinline__ uint32_t compress_any(int32_t x_hi) {
-  const uint32_t xp = ((uint32_t)x_hi + ((10u * Q) << 16)) >> 16;
-  const uint32_t v = (xp << D) + Q / 2;
-  return (umulhi_wide(v, 330282857u) >> 8) & ((1u << D) - 1);
-}
-// the same from a low-format register (plain sign-extended representative)
-template <int D>
-__device__ __forceinline__ uint32_t compress_any_lo(int32_t x) {
+__device__ __forceinline__ uint32_t compress_any(int32_t x) {
   const uint32_t v = ((uint32_t)(x + 10 * Q) << D) + Q / 2;
   return (umulhi_wide(v, 330282857u) >> 8) & ((1u << D) - 1);
 }
-template <int D, bool LOW = false>
+template <int D>
 __device__ __forceinline__ void compress_any_store_C(const int32_t (&r)[32], uint32_t* __restrict__ dst) {
   uint64_t acc = 0;
   int bits = 0, o = 0;
 #pragma unroll
   for (int i = 0; i < 32; i++) {
-    acc |= (uint64_t)(LOW ? compress_any_lo<D>(r[i]) : compress_any<D>(r[i])) << bits;
+    acc |= (uint64_t)compress_any<D>(r[i]) << bits;
     bits += D;
     if (bits >= 32) {
       dst[o++] = (uint32_t)acc;
@@ -559,40 +550,6 @@ __device__ __forceinline__ int32_t normalize_lo(int32_t x) {
   return x + ((x >> 31) & Q);
 }
 
-// 12-bit unpack of 32 coefficients (48 bytes, 16-byte aligned) straight to packed pairs (poly.go:123-129);
-// returns nonzero if any coefficient is >= q (cpapke.go:45-55)
-__device__ __forceinline__ uint32_t unpack12_pairs(const uint8_t* __restrict__ src, uint32_t (&aw)[16]) {
-  const uint4* p = reinterpret_cast<const uint4*>(src);
-  uint32_t w[12];
-#pragma unroll
-  for (int i = 0; i < 3; i++) {
-    const uint4 q4 = __ldg(p + i);
-    w[4 * i] = q4.x;
-    w[4 * i + 1] = q4.y;
-    w[4 * i + 2] = q4.z;
-    w[4 * i + 3] = q4.w;
-  }
-  uint32_t bad = 0;
-#pragma unroll
-  for (int g = 0; g < 4; g++) {  // 3 words -> 8 coefficients -> 4 pairs
-    const uint32_t a = w[3 * g], b = w[3 * g + 1], c = w[3 * g + 2];
-    uint32_t t[8];
-    t[0] = a & 0xfff;
-    t[1] = (a >> 12) & 0xfff;
-    t[2] = ((a >> 24) | (b << 8)) & 0xfff;
-    t[3] = (b >> 4) & 0xfff;
-    t[4] = (b >> 16) & 0xfff;
-    t[5] = ((b >> 28) | (c << 4)) & 0xfff;
-    t[6] = (c >> 8) & 0xfff;
-    t[7] = c >> 20;
-#pragma unroll
-    for (int j = 0; j < 8; j++) bad |= (t[j] >= (uint32_t)Q);
-#pragma unroll
-    for (int j = 0; j < 4; j++) aw[4 * g + j] = t[2 * j] | (t[2 * j + 1] << 16);
-  }
-  return bad;
-}
-
 // 24 bytes (8-byte aligned) of a 12-bit packed polynomial -> 16 coefficients as 8 packed pairs (poly.go:123-129);
 // returns nonzero if any coefficient is >= q (cpapke.go:45-55)
 __device__ __forceinline__ uint32_t unpack12_half(const uint32_t (&w)[8], uint32_t (&aw)[8]) {
@@ -617,6 +574,97 @@ __device__ __forceinline__ uint32_t unpack12_half(const uint32_t (&w)[8], uint32
   return bad;
 }
 
+// What the three IDP.2A kernels (encrypt_dp_kernel, decrypt_dp_kernel, keygen_dp_kernel) share: the octet of a lane
+// with its slices of dynamic shared memory, the byte-split operands and the accumulation of one half-row.
+//
+// The octet set-up: dynamic shared memory holds the operand areas of the THREADS / 8 octets, their transposition tiles
+// and the 128 twiddle pairs, which are staged here (hence the __syncthreads: every thread of the CTA builds one).  base is
+// the first op of this warp; a kernel returns when base >= n and asks for active(n) / op(n) only after that.
+template <int K, int THREADS>
+struct Octet {
+  uint2* ops;  // this lane's column of the octet's operands, [j][block][lane]
+  uint32_t* tile;
+  const volatile kyber::TwLow* tabl;
+  int oct, v;
+  unsigned mask;
+  size_t base;
+  __device__ __forceinline__ explicit Octet(const kyber::TwPair* __restrict__ tw) {
+    using S = EncSmem<K, THREADS>;
+    constexpr int OCTS = THREADS / 8;
+    extern __shared__ __align__(16) uint32_t enc_smem[];
+    uint32_t* tiles = enc_smem + OCTS * S::op_words;
+    kyber::TwPair* tws = reinterpret_cast<kyber::TwPair*>(tiles + OCTS * kyber::kPolyWords);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    oct = lane >> 3;
+    v = lane & 7;
+    mask = 0xffu << (8 * oct);
+    tile = tiles + (warp * 4 + oct) * kyber::kPolyWords;
+    ops = reinterpret_cast<uint2*>(enc_smem + (size_t)(warp * 4 + oct) * S::op_words) + v;
+    for (int i = threadIdx.x; i < 128; i += THREADS) tws[i] = tw[128 + i];  // {zp, kk} pairs in tw_slot order
+    __syncthreads();
+    tabl = reinterpret_cast<const volatile kyber::TwLow*>(tws);
+    base = ((size_t)blockIdx.x * (THREADS / 32) + warp) * 4;
+  }
+  __device__ __forceinline__ bool active(size_t n) const { return base + oct < n; }
+  // this octet's op, clamped to n - 1 so that an inactive octet still reads valid memory
+  __device__ __forceinline__ size_t op(size_t n) const { return active(n) ? base + oct : n - 1; }
+};
+
+// The byte-split operands W0, W1 of column j from a transformed polynomial (this lane's 32 coefficients, C layout), each
+// coefficient first multiplied by the constant of the Shoup pair (zp, kk).  Quad q of the lane has zeta = Zetas[64 + 8 v + q]:
+// +zeta for its first block, -zeta for its second.
+__device__ __forceinline__ void store_operands(uint2* ops, int j, const int32_t (&r)[32], const volatile kyber::TwLow* tabl,
+                                               int v, int32_t zp, int32_t kk) {
+  using namespace kyber;
+#pragma unroll
+  for (int q = 0; q < 8; q++) {
+    const TwLow z = twl_at(tabl, 64 + 8 * q + v);
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int blk = 2 * q + h;
+      const int32_t b0 = mont_mul_lo(r[2 * blk], zp, kk), b1 = mont_mul_lo(r[2 * blk + 1], zp, kk);
+      int32_t zb1 = mont_mul_lo(b1, z.zp, z.kk);
+      if (h) zb1 = -zb1;
+      // bytes 0 (low, unsigned) and 1 (high, signed) of the registers
+      ops[(j * 16 + blk) * 8] = make_uint2(__byte_perm((uint32_t)b0, (uint32_t)zb1, 0x5140),
+                                           __byte_perm((uint32_t)b1, (uint32_t)b0, 0x5140));
+    }
+  }
+}
+
+// The outputs p0, p1 of eight blocks (one half-row), summed over the columns: per column and block four IDP.2A, the
+// products with the low (unsigned) and the high (signed) operand bytes kept apart until the reduction.
+struct DotAcc {
+  int32_t p0l[8], p0h[8], p1l[8], p1h[8];
+  __device__ __forceinline__ DotAcc() {
+#pragma unroll
+    for (int c = 0; c < 8; c++) p0l[c] = p0h[c] = p1l[c] = p1h[c] = 0;
+  }
+  // one column: the eight packed words aw against the operands oj of the same eight blocks
+  __device__ __forceinline__ void add(const uint32_t (&aw)[8], const uint2* oj) {
+#pragma unroll
+    for (int c = 0; c < 8; c++) {
+      const uint2 w = oj[c * 8];
+      p0l[c] = (int32_t)dp2a_lo_uu(aw[c], w.x, (uint32_t)p0l[c]);
+      p0h[c] = dp2a_hi_us(aw[c], w.x, p0h[c]);
+      p1l[c] = (int32_t)dp2a_lo_uu(aw[c], w.y, (uint32_t)p1l[c]);
+      p1h[c] = dp2a_hi_us(aw[c], w.y, p1h[c]);
+    }
+  }
+  // montReduce of the two outputs of block c
+  __device__ __forceinline__ int32_t p0(int c) const { return mont_red_lo(p0l[c] + p0h[c] * 256); }
+  __device__ __forceinline__ int32_t p1(int c) const { return mont_red_lo(p1l[c] + p1h[c] * 256); }
+  // the eight blocks are coefficients r[OFF .. OFF + 16)
+  template <int OFF>
+  __device__ __forceinline__ void reduce_into(int32_t (&r)[32]) const {
+#pragma unroll
+    for (int c = 0; c < 8; c++) {
+      r[OFF + 2 * c] = p0(c);
+      r[OFF + 2 * c + 1] = p1(c);
+    }
+  }
+};
+
 // THREADS / 8 operations per CTA.  Small CTAs (64 threads, 8 operations, ~31 KB of shared memory for K = 3) keep 7 CTAs
 // = 14 warps per SM resident; every global load is issued one step before its data is used (register double buffers),
 // because a warp walks 19 dependent load -> compute phases per operation and L2 latency, not the instruction count,
@@ -629,28 +677,13 @@ __global__ void __launch_bounds__(THREADS, MINB) encrypt_dp_kernel(
   // lenient = 1: re-encryption inside Decapsulate (PublicKey.Unpack, cpapke.go:58-63: no modulus check; the
   // Normalize of t-hat is immaterial here because only residues are used)
   using P = Params<K>;
-  using S = EncSmem<K, THREADS>;
   using namespace kyber;
-  constexpr int OCTS = THREADS / 8;
-  extern __shared__ __align__(16) uint32_t enc_smem[];
-  uint32_t* ops_all = enc_smem;
-  uint32_t* tiles = enc_smem + OCTS * S::op_words;
-  TwPair* tws = reinterpret_cast<TwPair*>(tiles + OCTS * kPolyWords);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, oct = lane >> 3, v = lane & 7;
-  const unsigned octmask = 0xffu << (8 * oct);
-  uint32_t* tile = tiles + (warp * 4 + oct) * kPolyWords;
-  uint2* ops = reinterpret_cast<uint2*>(ops_all + (size_t)(warp * 4 + oct) * S::op_words) + v;  // [j][block][lane]
-
   // every transform of this kernel runs on low-format registers (kyber.cuh): its inputs are bounded by construction
   // (|noise| <= 3, |montReduce(.)| <= q), far inside the range where no int16 of the reference would wrap
-  for (int i = threadIdx.x; i < 128; i += THREADS) tws[i] = tw[128 + i];  // {zp, kk} pairs in tw_slot order
-  __syncthreads();
-  const volatile TwLow* tabl = reinterpret_cast<const volatile TwLow*>(tws);
-  const size_t base = ((size_t)blockIdx.x * (THREADS / 32) + warp) * 4;
-  if (base >= n) return;
-  const size_t op_raw = base + oct;
-  const bool active = op_raw < n;
-  const size_t op = active ? op_raw : n - 1;
+  const Octet<K, THREADS> o(tw);
+  if (o.base >= n) return;
+  const int v = o.v;
+  const size_t op = o.op(n);
   const uint8_t* ekp = ek + op * ek_stride;
   const uint32_t* Ap = reinterpret_cast<const uint32_t*>(A) + (a_shared ? 0 : op * K * K * (N / 2));
   const uint32_t* np = reinterpret_cast<const uint32_t*>(noise) + op * P::n_noise * (N / 2);
@@ -672,27 +705,14 @@ __global__ void __launch_bounds__(THREADS, MINB) encrypt_dp_kernel(
         for (int q = 0; q < 16; q++) nw[q] = ldg_stream32(np + (j + 1) * (N / 2) + 8 * q + v);
       }
       fwd_pass_S_lo(r);
-      store_S_lo(tile, v, r);
+      store_S_lo(o.tile, v, r);
       __syncwarp();
-      load_C_lo(tile, v, r);
-      fwd_pass_C_lo_smem(r, tabl, v);
+      load_C_lo(o.tile, v, r);
+      fwd_pass_C_lo_smem(r, o.tabl, v);
       __syncwarp();
-#pragma unroll
-      for (int q = 0; q < 8; q++) {  // quad q of this lane: zeta = Zetas[64 + 8 v + q], +zeta for its first block, -zeta for its second
-        const TwLow z = twl_at(tabl, 64 + 8 * q + v);
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-          const int blk = 2 * q + h;
-          // x 512 = R / 128: the Montgomery product by 512 R mod q = 1441, i.e. the pair (kScaleZp, kScaleKk) of the
-          // inverse transform (|in| <= 7 q, |out| < q)
-          const int32_t b0 = mont_mul_lo(r[2 * blk], kScaleZp, kScaleKk), b1 = mont_mul_lo(r[2 * blk + 1], kScaleZp, kScaleKk);
-          int32_t zb1 = mont_mul_lo(b1, z.zp, z.kk);
-          if (h) zb1 = -zb1;
-          // bytes 0 (low, unsigned) and 1 (high, signed) of the registers
-          ops[(j * 16 + blk) * 8] = make_uint2(__byte_perm((uint32_t)b0, (uint32_t)zb1, 0x5140),
-                                               __byte_perm((uint32_t)b1, (uint32_t)b0, 0x5140));
-        }
-      }
+      // x 512 = R / 128: the Montgomery product by 512 R mod q = 1441, i.e. the pair (kScaleZp, kScaleKk) of the
+      // inverse transform (|in| <= 7 q, |out| < q)
+      store_operands(o.ops, j, r, o.tabl, v, kScaleZp, kScaleKk);
     }
   }
   __syncwarp();
@@ -721,9 +741,7 @@ __global__ void __launch_bounds__(THREADS, MINB) encrypt_dp_kernel(
     uint32_t ew[16];
 #pragma unroll 1
     for (int h = 0; h < 2; h++) {
-      int32_t p0l[8], p0h[8], p1l[8], p1h[8];
-#pragma unroll
-      for (int c = 0; c < 8; c++) p0l[c] = p0h[c] = p1l[c] = p1h[c] = 0;
+      DotAcc acc;
       const int ni = h ? i + 1 : i, nh = h ^ 1;  // the half-row after this one
 #pragma unroll
       for (int j = 0; j < K; j++) {
@@ -736,38 +754,22 @@ __global__ void __launch_bounds__(THREADS, MINB) encrypt_dp_kernel(
           if (!lenient) bad |= b;
         }
         if (ni <= K) fetch(ni, nh, j, raw[j]);
-        const uint2* oj = ops + (size_t)(j * 16 + 8 * h) * 8;
-#pragma unroll
-        for (int c = 0; c < 8; c++) {
-          const uint2 w = oj[c * 8];
-          p0l[c] = (int32_t)dp2a_lo_uu(aw[c], w.x, (uint32_t)p0l[c]);
-          p0h[c] = dp2a_hi_us(aw[c], w.x, p0h[c]);
-          p1l[c] = (int32_t)dp2a_lo_uu(aw[c], w.y, (uint32_t)p1l[c]);
-          p1h[c] = dp2a_hi_us(aw[c], w.y, p1h[c]);
-        }
+        acc.add(aw, o.ops + (size_t)(j * 16 + 8 * h) * 8);
       }
       if (h == 0) {
-#pragma unroll
-        for (int c = 0; c < 8; c++) {
-          r[2 * c] = mont_red_lo(p0l[c] + p0h[c] * 256);
-          r[2 * c + 1] = mont_red_lo(p1l[c] + p1h[c] * 256);
-        }
+        acc.reduce_into<0>(r);
         // the noise polynomial this row ends with: in flight during the second half and the inverse transform
         const uint32_t* e = np + (K + i) * (N / 2);
 #pragma unroll
         for (int q = 0; q < 16; q++) ew[q] = __ldg(e + 8 * q + v);
       } else {
-#pragma unroll
-        for (int c = 0; c < 8; c++) {
-          r[16 + 2 * c] = mont_red_lo(p0l[c] + p0h[c] * 256);
-          r[16 + 2 * c + 1] = mont_red_lo(p1l[c] + p1h[c] * 256);
-        }
+        acc.reduce_into<16>(r);
       }
     }
-    inv_pass_C_lo(r, tabl, v);
-    store_C_lo(tile, v, r);
+    inv_pass_C_lo(r, o.tabl, v);
+    store_C_lo(o.tile, v, r);
     __syncwarp();
-    load_S_lo(tile, v, r);
+    load_S_lo(o.tile, v, r);
     inv_pass_S_lo<false>(r, v);
     __syncwarp();
     // before the constant the reference bounds the values by 9 q (ntt.go:187-190), so adding e (<= 2) and the message
@@ -788,20 +790,20 @@ __global__ void __launch_bounds__(THREADS, MINB) encrypt_dp_kernel(
         }
       }
     }
-    store_S_lo(tile, v, r);  // Normalize (cpapke.go:176-177) is absorbed by compress_any
+    store_S_lo(o.tile, v, r);  // Normalize (cpapke.go:176-177) is absorbed by compress_any
     __syncwarp();
-    load_C_lo(tile, v, r);
+    load_C_lo(o.tile, v, r);
     __syncwarp();
-    bad = __any_sync(octmask, bad) ? 1u : 0u;  // after row K this holds the modulus check of the whole key
-    if (active) {
+    bad = __any_sync(o.mask, bad) ? 1u : 0u;  // after row K this holds the modulus check of the whole key
+    if (o.active(n)) {
       if (i < K)
-        compress_any_store_C<P::du, true>(r, reinterpret_cast<uint32_t*>(ctp + i * 32 * P::du) + v * P::du);
+        compress_any_store_C<P::du>(r, reinterpret_cast<uint32_t*>(ctp + i * 32 * P::du) + v * P::du);
       else if (!bad)
-        compress_any_store_C<P::dv, true>(r, reinterpret_cast<uint32_t*>(ctp + K * 32 * P::du) + v * P::dv);
+        compress_any_store_C<P::dv>(r, reinterpret_cast<uint32_t*>(ctp + K * 32 * P::du) + v * P::dv);
     }
   }
   // kem.ErrPubKey (cpapke.go:48-54): no output for a non-canonical key
-  if (active) {
+  if (o.active(n)) {
     if (bad) {
       uint32_t* c32 = reinterpret_cast<uint32_t*>(ctp);
       for (int w = v; w < P::ct_bytes / 4; w += 8) c32[w] = 0;
@@ -811,27 +813,66 @@ __global__ void __launch_bounds__(THREADS, MINB) encrypt_dp_kernel(
   }
 }
 
-// the K-PKE.Encrypt launch of the three flows (Encapsulate, the re-encryption of Decapsulate, round-3 Kyber)
-constexpr int kEncDpThreads = 64;
-template <int K, int MINB>
-static int launch_encrypt_v(const uint8_t* ek, size_t ek_stride, const int16_t* A, int a_shared, const int16_t* noise,
-                            const uint8_t* m, size_t n, uint8_t* ct, uint8_t* ss, uint8_t* status, int lenient,
-                            cudaStream_t st) {
-  using S = EncSmem<K, kEncDpThreads>;
-  if (int arc = ensure_smem_attr((const void*)encrypt_dp_kernel<K, kEncDpThreads, MINB>, S::bytes)) return arc;
+// The launch of the three IDP.2A kernels (encrypt_dp_kernel, decrypt_dp_kernel, keygen_dp_kernel) over n ops, all
+// timed under KID_MLKEM_ENCRYPT.  7 CTAs of 64 threads per SM (K = 4: 6, its operands and registers are larger); H100
+// has the register file and shared memory per SM these were sized for.
+constexpr int kDpThreads = 64;
+template <int K>
+constexpr int kDpMinBlocks = K == 4 ? 6 : 7;
+template <int K, typename... P, typename... A>
+static int launch_dp(void (*kernel)(P...), size_t n, cudaStream_t st, A... args) {
+  constexpr int bytes = EncSmem<K, kDpThreads>::bytes, per_cta = kDpThreads / 8;
+  if (int arc = ensure_smem_attr((const void*)kernel, bytes)) return arc;
   KernelScope ks(KID_MLKEM_ENCRYPT, st);
-  constexpr int per_cta = kEncDpThreads / 8;
-  encrypt_dp_kernel<K, kEncDpThreads, MINB><<<(unsigned)((n + per_cta - 1) / per_cta), kEncDpThreads, S::bytes, st>>>(
-      ek, ek_stride, A, a_shared, noise, m, n, ct, ss, status, (const kyber::TwPair*)ctx().kyber_tw, lenient);
+  kernel<<<(unsigned)((n + per_cta - 1) / per_cta), kDpThreads, bytes, st>>>(args...);
   return 0;
 }
+
+// Sub-batches of sub_batch(n) ops alternate between the two lanes of the work set, forked from the caller's stream and
+// joined back to it with events: the tail wave of one sub-batch's kernels overlaps the next sub-batch instead of idling
+// SMs.  launch(first, cnt, lane, stream) enqueues one sub-batch; a nonzero result ends the loop and is returned.
+static size_t sub_batch(size_t n) { return n < kSub ? n : kSub; }
+template <typename F>
+static int for_sub_batches(WorkSet& ws, size_t n, cudaStream_t st, F&& launch) {
+  const size_t sub = sub_batch(n);
+  CB200_CUDA(cudaEventRecord(ws.ev_fork, st));
+  for (int l = 0; l < 2; l++) CB200_CUDA(cudaStreamWaitEvent(ws.lane[l], ws.ev_fork, 0));
+  int l = 0;
+  for (size_t first = 0; first < n; first += sub, l ^= 1) {
+    // per-kernel event timing (cb200_profile_enable) wants true, non-overlapped durations: stay on one stream
+    cudaStream_t ls = profiling_on() ? st : ws.lane[l];
+    const size_t cnt = (n - first < sub) ? n - first : sub;
+    if (int rc = launch(first, cnt, l, ls)) return rc;
+  }
+  for (int l = 0; l < 2; l++) {
+    CB200_CUDA(cudaEventRecord(ws.ev_join[l], ws.lane[l]));
+    CB200_CUDA(cudaStreamWaitEvent(st, ws.ev_join[l], 0));
+  }
+  return 0;
+}
+
+// (K', r) = G(m || h), ct = K-PKE.Encrypt(ek, m, r) with the lenient key parse, per-op keys: the re-encryption of
+// ML-KEM and round-3 Kyber Decapsulate, and the body of round-3 Kyber Encapsulate.  base + o_A[l] / o_n[l] are the
+// matrix and noise buffers of lane l.
 template <int K>
-static int launch_encrypt(const uint8_t* ek, size_t ek_stride, const int16_t* A, int a_shared, const int16_t* noise,
-                          const uint8_t* m, size_t n, uint8_t* ct, uint8_t* ss, uint8_t* status, int lenient,
-                          cudaStream_t st) {
-  // 7 CTAs of 64 threads per SM (K = 4: 6, its operands and registers are larger); H100 has the register file and
-  // shared memory per SM these were sized for
-  return launch_encrypt_v<K, (K == 4 ? 6 : 7)>(ek, ek_stride, A, a_shared, noise, m, n, ct, ss, status, lenient, st);
+static int encrypt_lenient(const uint8_t* ek, size_t ek_stride, const uint8_t* h, size_t h_stride, const uint8_t* m,
+                           uint8_t* ct, uint8_t* kbar, uint64_t* r, char* base, const size_t (&o_A)[2],
+                           const size_t (&o_n)[2], size_t n, cudaStream_t st, int slot) {
+  using P = Params<K>;
+  {
+    KernelScope ks(KID_MLKEM_G, st);
+    g_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(m, h, h_stride, n, kbar, r);
+  }
+  const kyber::TwPair* tw = (const kyber::TwPair*)ctx().kyber_tw;
+  return for_sub_batches(wset(slot), n, st, [&](size_t first, size_t cnt, int l, cudaStream_t ls) {
+    int16_t* A = (int16_t*)(base + o_A[l]);
+    int16_t* noise = (int16_t*)(base + o_n[l]);
+    if (int src = launch_sample<K>(slot, l, ls, ek + 384 * K + first * ek_stride, ek_stride, cnt, r + 4 * first, cnt, A, noise,
+                                   1, P::n_noise, 4, K))
+      return src;
+    return launch_dp<K>(encrypt_dp_kernel<K, kDpThreads, kDpMinBlocks<K>>, cnt, ls, ek + first * ek_stride, ek_stride, A, 0,
+                        noise, m + 32 * first, cnt, ct + first * P::ct_bytes, nullptr, nullptr, tw, 1);
+  });
 }
 
 
@@ -866,103 +907,59 @@ __global__ void __launch_bounds__(THREADS, MINB) decrypt_dp_kernel(const uint8_t
                                                                    uint8_t* __restrict__ mprime,
                                                                    const kyber::TwPair* __restrict__ tw) {
   using P = Params<K>;
-  using S = EncSmem<K, THREADS>;
   using namespace kyber;
-  constexpr int OCTS = THREADS / 8;
-  extern __shared__ __align__(16) uint32_t enc_smem[];
-  uint32_t* ops_all = enc_smem;
-  uint32_t* tiles = enc_smem + OCTS * S::op_words;
-  TwPair* tws = reinterpret_cast<TwPair*>(tiles + OCTS * kPolyWords);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, oct = lane >> 3, v = lane & 7;
-  const unsigned octmask = 0xffu << (8 * oct);
-  uint32_t* tile = tiles + (warp * 4 + oct) * kPolyWords;
-  uint2* ops = reinterpret_cast<uint2*>(ops_all + (size_t)(warp * 4 + oct) * S::op_words) + v;  // [j][block][lane]
-  for (int i = threadIdx.x; i < 128; i += THREADS) tws[i] = tw[128 + i];  // {zp, kk} pairs in tw_slot order
-  __syncthreads();
-  const volatile TwLow* tabl = reinterpret_cast<const volatile TwLow*>(tws);
-  const size_t base = ((size_t)blockIdx.x * (THREADS / 32) + warp) * 4;
-  if (base >= n) return;
-  const bool active = base + oct < n;
-  const size_t op = active ? base + oct : n - 1;
+  const Octet<K, THREADS> o(tw);
+  if (o.base >= n) return;
+  const int v = o.v;
+  const size_t op = o.op(n);
   const uint8_t* dkp = dk + op * dk_stride;
   const uint8_t* ctp = ct + op * P::ct_bytes;
   int32_t r[32];
 #pragma unroll 1
   for (int j = 0; j < K; j++) {  // operands of u-hat[j] = NTT(Decompress(u[j])) x 512
     decompress_C<P::du, true>(reinterpret_cast<const uint32_t*>(ctp + j * 32 * P::du) + v * P::du, r);
-    store_C_lo(tile, v, r);
+    store_C_lo(o.tile, v, r);
     __syncwarp();
-    load_S_lo(tile, v, r);
+    load_S_lo(o.tile, v, r);
     __syncwarp();
     fwd_pass_S_lo(r);
-    store_S_lo(tile, v, r);
+    store_S_lo(o.tile, v, r);
     __syncwarp();
-    load_C_lo(tile, v, r);
-    fwd_pass_C_lo_smem(r, tabl, v);
+    load_C_lo(o.tile, v, r);
+    fwd_pass_C_lo_smem(r, o.tabl, v);
     __syncwarp();
-#pragma unroll
-    for (int q = 0; q < 8; q++) {
-      const TwLow z = twl_at(tabl, 64 + 8 * q + v);
-#pragma unroll
-      for (int h = 0; h < 2; h++) {
-        const int blk = 2 * q + h;
-        const int32_t b0 = mont_mul_lo(r[2 * blk], kScaleZp, kScaleKk), b1 = mont_mul_lo(r[2 * blk + 1], kScaleZp, kScaleKk);
-        int32_t zb1 = mont_mul_lo(b1, z.zp, z.kk);
-        if (h) zb1 = -zb1;
-        ops[(j * 16 + blk) * 8] = make_uint2(__byte_perm((uint32_t)b0, (uint32_t)zb1, 0x5140),
-                                             __byte_perm((uint32_t)b1, (uint32_t)b0, 0x5140));
-      }
-    }
+    store_operands(o.ops, j, r, o.tabl, v, kScaleZp, kScaleKk);
   }
   __syncwarp();
   // PolyDotHat(&m, &sk.sh, &u) (cpapke.go:121): one row over the K columns, in two halves of eight blocks
 #pragma unroll 1
   for (int h = 0; h < 2; h++) {
-    int32_t p0l[8], p0h[8], p1l[8], p1h[8];
-#pragma unroll
-    for (int c = 0; c < 8; c++) p0l[c] = p0h[c] = p1l[c] = p1h[c] = 0;
+    DotAcc acc;
 #pragma unroll
     for (int j = 0; j < K; j++) {
       const uint2* p = reinterpret_cast<const uint2*>(dkp + 384 * j + 48 * v + 24 * h);
       const uint2 x = __ldg(p), y = __ldg(p + 1), zz = __ldg(p + 2);
       uint32_t raw[8] = {x.x, x.y, y.x, y.y, zz.x, zz.y, 0, 0}, aw[8];
       unpack12_half(raw, aw);
-      const uint2* oj = ops + (size_t)(j * 16 + 8 * h) * 8;
-#pragma unroll
-      for (int c = 0; c < 8; c++) {
-        const uint2 w = oj[c * 8];
-        p0l[c] = (int32_t)dp2a_lo_uu(aw[c], w.x, (uint32_t)p0l[c]);
-        p0h[c] = dp2a_hi_us(aw[c], w.x, p0h[c]);
-        p1l[c] = (int32_t)dp2a_lo_uu(aw[c], w.y, (uint32_t)p1l[c]);
-        p1h[c] = dp2a_hi_us(aw[c], w.y, p1h[c]);
-      }
+      acc.add(aw, o.ops + (size_t)(j * 16 + 8 * h) * 8);
     }
-    if (h == 0) {
-#pragma unroll
-      for (int c = 0; c < 8; c++) {
-        r[2 * c] = mont_red_lo(p0l[c] + p0h[c] * 256);
-        r[2 * c + 1] = mont_red_lo(p1l[c] + p1h[c] * 256);
-      }
-    } else {
-#pragma unroll
-      for (int c = 0; c < 8; c++) {
-        r[16 + 2 * c] = mont_red_lo(p0l[c] + p0h[c] * 256);
-        r[16 + 2 * c + 1] = mont_red_lo(p1l[c] + p1h[c] * 256);
-      }
-    }
+    if (h == 0)
+      acc.reduce_into<0>(r);
+    else
+      acc.reduce_into<16>(r);
   }
-  inv_pass_C_lo(r, tabl, v);
-  store_C_lo(tile, v, r);
+  inv_pass_C_lo(r, o.tabl, v);
+  store_C_lo(o.tile, v, r);
   __syncwarp();
-  load_S_lo(tile, v, r);
+  load_S_lo(o.tile, v, r);
   __syncwarp();
   inv_pass_S_lo<false>(r, v);
   // v polynomial: decompress in C layout, bring to S layout
   int32_t vv[32];
   decompress_C<P::dv, true>(reinterpret_cast<const uint32_t*>(ctp + K * 32 * P::du) + v * P::dv, vv);
-  store_C_lo(tile, v, vv);
+  store_C_lo(o.tile, v, vv);
   __syncwarp();
-  load_S_lo(tile, v, vv);
+  load_S_lo(o.tile, v, vv);
   __syncwarp();
   // m = Normalize(v - m); CompressMessageTo (poly.go:150-166); coefficient 16 s + 2 v + b -> bit of m'
   uint32_t words[8];
@@ -983,27 +980,17 @@ __global__ void __launch_bounds__(THREADS, MINB) decrypt_dp_kernel(const uint8_t
 #pragma unroll
   for (int w = 0; w < 8; w++) {
     uint32_t x = words[w];
-    x |= __shfl_xor_sync(octmask, x, 1);
-    x |= __shfl_xor_sync(octmask, x, 2);
-    x |= __shfl_xor_sync(octmask, x, 4);
+    x |= __shfl_xor_sync(o.mask, x, 1);
+    x |= __shfl_xor_sync(o.mask, x, 2);
+    x |= __shfl_xor_sync(o.mask, x, 4);
     words[w] = x;
   }
-  if (active) {
+  if (o.active(n)) {
     uint32_t mine = 0;
 #pragma unroll
     for (int w = 0; w < 8; w++) mine = (v == w) ? words[w] : mine;
     reinterpret_cast<uint32_t*>(mprime + 32 * op)[v] = mine;
   }
-}
-template <int K>
-static int launch_decrypt(const uint8_t* dk, size_t dk_stride, const uint8_t* ct, size_t n, uint8_t* mprime,
-                          const kyber::TwPair* tw, cudaStream_t st) {
-  constexpr int MINB = K == 4 ? 6 : 7, per_cta = kEncDpThreads / 8;
-  using S = EncSmem<K, kEncDpThreads>;
-  if (int arc = ensure_smem_attr((const void*)decrypt_dp_kernel<K, kEncDpThreads, MINB>, S::bytes)) return arc;
-  decrypt_dp_kernel<K, kEncDpThreads, MINB><<<(unsigned)((n + per_cta - 1) / per_cta), kEncDpThreads, S::bytes, st>>>(
-      dk, dk_stride, ct, n, mprime, tw);
-  return 0;
 }
 
 // Implicit rejection (kyber.go:168-183): ss = (ct == ct2) ? K' : SHAKE256(z || ct)[:32]; also checks
@@ -1063,8 +1050,7 @@ static int decaps_device(const uint8_t* dk, size_t dk_stride, const uint8_t* ct,
                          cudaStream_t st, int slot) {
   using P = Params<K>;
   Dev& c = ctx();
-  WorkSet& ws = wset(slot);
-  const size_t sub = n < kSub ? n : kSub;
+  const size_t sub = sub_batch(n);
   size_t off = 0;
   auto take = [&](size_t bytes) {
     size_t o = off;
@@ -1090,37 +1076,15 @@ static int decaps_device(const uint8_t* dk, size_t dk_stride, const uint8_t* ct,
   const uint8_t* ek = dk + 384 * K;  // dk = sk || ek || H(ek) || z (kyber.go:187-201)
   if (int arc = ensure_smem_attr((const void*)sample_kernel<K>, kSampleSmem)) return arc;
   const kyber::TwPair* tw = (const kyber::TwPair*)c.kyber_tw;
-  {
-    KernelScope ks(KID_MLKEM_ENCRYPT, st);
-    if (int drc = launch_decrypt<K>(dk, dk_stride, ct, n, mprime, tw, st)) return drc;
-  }
+  if (int drc = launch_dp<K>(decrypt_dp_kernel<K, kDpThreads, kDpMinBlocks<K>>, n, st, dk, dk_stride, ct, n, mprime, tw))
+    return drc;
   {
     KernelScope ks(KID_MLKEM_HASH_EK, st);
     hash_ek_kernel<K><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(ek, dk_stride, n, h);
   }
-  {  // (K', r') = G(m' || h) with the h stored in dk (kyber.go:160-164)
-    KernelScope ks(KID_MLKEM_G, st);
-    g_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(mprime, dk + 384 * K + P::ek_bytes, dk_stride, n, kbar, r);
-  }
-  CB200_CUDA(cudaEventRecord(ws.ev_fork, st));
-  for (int q = 0; q < 2; q++) CB200_CUDA(cudaStreamWaitEvent(ws.lane[q], ws.ev_fork, 0));
-  int l = 0;
-  for (size_t first = 0; first < n; first += sub, l ^= 1) {
-    cudaStream_t ls = profiling_on() ? st : ws.lane[l];
-    int16_t* A = (int16_t*)(b + o_A[l]);
-    int16_t* noise = (int16_t*)(b + o_n[l]);
-    const size_t cnt = (n - first < sub) ? n - first : sub;
-    if (int src = launch_sample<K>(slot, l, ls, ek + 384 * K + first * dk_stride, dk_stride, cnt, r + 4 * first, cnt, A, noise,
-                                   1, P::n_noise, 4, K))
-      return src;
-    if (int erc = launch_encrypt<K>(ek + first * dk_stride, dk_stride, A, 0, noise, mprime + 32 * first, cnt,
-                                    ct2 + first * P::ct_bytes, nullptr, nullptr, 1, ls))
-      return erc;
-  }
-  for (int q = 0; q < 2; q++) {
-    CB200_CUDA(cudaEventRecord(ws.ev_join[q], ws.lane[q]));
-    CB200_CUDA(cudaStreamWaitEvent(st, ws.ev_join[q], 0));
-  }
+  // (K', r') = G(m' || h) with the h stored in dk (kyber.go:160-164), ct' = K-PKE.Encrypt(ek, m', r')
+  rc = encrypt_lenient<K>(ek, dk_stride, dk + 384 * K + P::ek_bytes, dk_stride, mprime, ct2, kbar, r, b, o_A, o_n, n, st, slot);
+  if (rc) return rc;
   {
     KernelScope ks(KID_MLKEM_G, st);
     select_kernel<K><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(dk, dk_stride, ct, ct2, kbar, h, n, ss, status);
@@ -1187,26 +1151,14 @@ __global__ void __launch_bounds__(THREADS, MINB) keygen_dp_kernel(const int16_t*
                                                                   uint8_t* __restrict__ ek, uint8_t* __restrict__ dk,
                                                                   const kyber::TwPair* __restrict__ tw) {
   using P = Params<K>;
-  using S = EncSmem<K, THREADS>;
   using namespace kyber;
-  constexpr int OCTS = THREADS / 8;
   // R^2 mod q = 1353 (field.go:35-39) as a Shoup pair: zp = R mod q = 2285 - q
   constexpr int32_t kR2Zp = 2285 - Q, kR2Kk = (kR2Zp * 65536 - 1353) / Q;
   static_assert(kR2Zp * 65536 - 1353 == kR2Kk * Q, "ToMont constant");
-  extern __shared__ __align__(16) uint32_t enc_smem[];
-  uint32_t* ops_all = enc_smem;
-  uint32_t* tiles = enc_smem + OCTS * S::op_words;
-  TwPair* tws = reinterpret_cast<TwPair*>(tiles + OCTS * kPolyWords);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, oct = lane >> 3, v = lane & 7;
-  uint32_t* tile = tiles + (warp * 4 + oct) * kPolyWords;
-  uint2* ops = reinterpret_cast<uint2*>(ops_all + (size_t)(warp * 4 + oct) * S::op_words) + v;  // [j][block][lane]
-  for (int i = threadIdx.x; i < 128; i += THREADS) tws[i] = tw[128 + i];  // {zp, kk} pairs in tw_slot order
-  __syncthreads();
-  const volatile TwLow* tabl = reinterpret_cast<const volatile TwLow*>(tws);
-  const size_t base = ((size_t)blockIdx.x * (THREADS / 32) + warp) * 4;
-  if (base >= n) return;
-  const bool active = base + oct < n;
-  const size_t op = active ? base + oct : n - 1;
+  const Octet<K, THREADS> o(tw);
+  if (o.base >= n) return;
+  const int v = o.v;
+  const size_t op = o.op(n);
   const uint32_t* Ap = reinterpret_cast<const uint32_t*>(A) + op * K * K * (N / 2);
   const uint32_t* np = reinterpret_cast<const uint32_t*>(noise) + op * (2 * K) * (N / 2);
   uint8_t* ekp = ek + op * P::ek_bytes;
@@ -1226,29 +1178,17 @@ __global__ void __launch_bounds__(THREADS, MINB) keygen_dp_kernel(const int16_t*
         for (int q = 0; q < 16; q++) nw[q] = ldg_stream32(np + (j + 1) * (N / 2) + 8 * q + v);
       }
       fwd_pass_S_lo(r);
-      store_S_lo(tile, v, r);
+      store_S_lo(o.tile, v, r);
       __syncwarp();
-      load_C_lo(tile, v, r);
-      fwd_pass_C_lo_smem(r, tabl, v);
+      load_C_lo(o.tile, v, r);
+      fwd_pass_C_lo_smem(r, o.tabl, v);
       __syncwarp();
-#pragma unroll
-      for (int q = 0; q < 8; q++) {  // quad q of this lane: zeta = Zetas[64 + 8 v + q], +zeta for its first block, -zeta for its second
-        const TwLow z = twl_at(tabl, 64 + 8 * q + v);
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-          const int blk = 2 * q + h;
-          const int32_t b0 = mont_mul_lo(r[2 * blk], kR2Zp, kR2Kk), b1 = mont_mul_lo(r[2 * blk + 1], kR2Zp, kR2Kk);
-          int32_t zb1 = mont_mul_lo(b1, z.zp, z.kk);
-          if (h) zb1 = -zb1;
-          ops[(j * 16 + blk) * 8] = make_uint2(__byte_perm((uint32_t)b0, (uint32_t)zb1, 0x5140),
-                                               __byte_perm((uint32_t)b1, (uint32_t)b0, 0x5140));
-        }
-      }
+      store_operands(o.ops, j, r, o.tabl, v, kR2Zp, kR2Kk);
 #pragma unroll
       for (int c = 0; c < 32; c++) r[c] = normalize_lo(r[c]);
       uint32_t pw[12];
       pack12_C_lo(r, pw);
-      if (active) {
+      if (o.active(n)) {
         uint32_t* dst = reinterpret_cast<uint32_t*>(dkp + 384 * j) + 12 * v;
 #pragma unroll
         for (int w = 0; w < 12; w++) dst[w] = pw[w];
@@ -1279,16 +1219,14 @@ __global__ void __launch_bounds__(THREADS, MINB) keygen_dp_kernel(const int16_t*
       for (int q = 0; q < 16; q++) ew[q] = __ldg(np + (K + i + 1) * (N / 2) + 8 * q + v);
     }
     fwd_pass_S_lo(r);
-    store_S_lo(tile, v, r);
+    store_S_lo(o.tile, v, r);
     __syncwarp();
-    load_C_lo(tile, v, r);
-    fwd_pass_C_lo_smem(r, tabl, v);
+    load_C_lo(o.tile, v, r);
+    fwd_pass_C_lo_smem(r, o.tabl, v);
     __syncwarp();
 #pragma unroll 1
     for (int h = 0; h < 2; h++) {
-      int32_t p0l[8], p0h[8], p1l[8], p1h[8];
-#pragma unroll
-      for (int c = 0; c < 8; c++) p0l[c] = p0h[c] = p1l[c] = p1h[c] = 0;
+      DotAcc acc;
       const int ni = h ? i + 1 : i, nh = h ^ 1;  // the half-row after this one
 #pragma unroll
       for (int j = 0; j < K; j++) {
@@ -1296,33 +1234,25 @@ __global__ void __launch_bounds__(THREADS, MINB) keygen_dp_kernel(const int16_t*
 #pragma unroll
         for (int c = 0; c < 8; c++) aw[c] = raw[j][c];
         if (ni < K) fetch(ni, nh, j, raw[j]);
-        const uint2* oj = ops + (size_t)(j * 16 + 8 * h) * 8;
-#pragma unroll
-        for (int c = 0; c < 8; c++) {
-          const uint2 w = oj[c * 8];
-          p0l[c] = (int32_t)dp2a_lo_uu(aw[c], w.x, (uint32_t)p0l[c]);
-          p0h[c] = dp2a_hi_us(aw[c], w.x, p0h[c]);
-          p1l[c] = (int32_t)dp2a_lo_uu(aw[c], w.y, (uint32_t)p1l[c]);
-          p1h[c] = dp2a_hi_us(aw[c], w.y, p1h[c]);
-        }
+        acc.add(aw, o.ops + (size_t)(j * 16 + 8 * h) * 8);
       }
       if (h == 0) {
 #pragma unroll
         for (int c = 0; c < 8; c++) {
-          r[2 * c] = normalize_lo(mont_red_lo(p0l[c] + p0h[c] * 256) + r[2 * c]);
-          r[2 * c + 1] = normalize_lo(mont_red_lo(p1l[c] + p1h[c] * 256) + r[2 * c + 1]);
+          r[2 * c] = normalize_lo(acc.p0(c) + r[2 * c]);
+          r[2 * c + 1] = normalize_lo(acc.p1(c) + r[2 * c + 1]);
         }
       } else {
 #pragma unroll
         for (int c = 0; c < 8; c++) {
-          r[16 + 2 * c] = normalize_lo(mont_red_lo(p0l[c] + p0h[c] * 256) + r[16 + 2 * c]);
-          r[16 + 2 * c + 1] = normalize_lo(mont_red_lo(p1l[c] + p1h[c] * 256) + r[16 + 2 * c + 1]);
+          r[16 + 2 * c] = normalize_lo(acc.p0(c) + r[16 + 2 * c]);
+          r[16 + 2 * c + 1] = normalize_lo(acc.p1(c) + r[16 + 2 * c + 1]);
         }
       }
     }
     uint32_t pw[12];
     pack12_C_lo(r, pw);
-    if (active) {
+    if (o.active(n)) {
       uint32_t* d1 = reinterpret_cast<uint32_t*>(ekp + 384 * i) + 12 * v;
       uint32_t* d2 = reinterpret_cast<uint32_t*>(dkp + 384 * K + 384 * i) + 12 * v;
 #pragma unroll
@@ -1339,8 +1269,7 @@ static int keygen_device(const uint8_t* seeds, uint8_t* ek, uint8_t* dk, size_t 
                          int mlkem = 1) {
   using P = Params<K>;
   Dev& c = ctx();
-  WorkSet& ws = wset(slot);
-  const size_t sub = n < kSub ? n : kSub;
+  const size_t sub = sub_batch(n);
   constexpr size_t dksz = 768 * K + 96;
   size_t off = 0;
   auto take = [&](size_t bytes) {
@@ -1365,31 +1294,18 @@ static int keygen_device(const uint8_t* seeds, uint8_t* ek, uint8_t* dk, size_t 
     KernelScope ks(KID_MLKEM_G, st);
     keygen_seed_kernel<K><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(seeds, n, rs, ek, dk, mlkem);
   }
-  CB200_CUDA(cudaEventRecord(ws.ev_fork, st));
-  for (int q = 0; q < 2; q++) CB200_CUDA(cudaStreamWaitEvent(ws.lane[q], ws.ev_fork, 0));
-  int l = 0;
-  for (size_t first = 0; first < n; first += sub, l ^= 1) {
-    cudaStream_t ls = profiling_on() ? st : ws.lane[l];
+  const kyber::TwPair* tw = (const kyber::TwPair*)c.kyber_tw;
+  rc = for_sub_batches(wset(slot), n, st, [&](size_t first, size_t cnt, int l, cudaStream_t ls) {
     int16_t* A = (int16_t*)(b + o_A[l]);
     int16_t* noise = (int16_t*)(b + o_n[l]);
-    const size_t cnt = (n - first < sub) ? n - first : sub;
     // A (not transposed) from rho = rs[0..4), s/e noise from sigma = rs[4..8)
     if (int src = launch_sample<K>(slot, l, ls, (const uint8_t*)(rs + 8 * first), 64, cnt, rs + 8 * first + 4, cnt, A, noise, 0,
                                    2 * K, 8, 2 * K))
       return src;
-    {
-      KernelScope ks(KID_MLKEM_ENCRYPT, ls);
-      constexpr int MINB = K == 4 ? 6 : 7, per_cta = kEncDpThreads / 8;
-      using S = EncSmem<K, kEncDpThreads>;
-      if (int arc = ensure_smem_attr((const void*)keygen_dp_kernel<K, kEncDpThreads, MINB>, S::bytes)) return arc;
-      keygen_dp_kernel<K, kEncDpThreads, MINB><<<(unsigned)((cnt + per_cta - 1) / per_cta), kEncDpThreads, S::bytes, ls>>>(
-          A, noise, cnt, ek + first * P::ek_bytes, dk + first * dksz, (const kyber::TwPair*)c.kyber_tw);
-    }
-  }
-  for (int q = 0; q < 2; q++) {
-    CB200_CUDA(cudaEventRecord(ws.ev_join[q], ws.lane[q]));
-    CB200_CUDA(cudaStreamWaitEvent(st, ws.ev_join[q], 0));
-  }
+    return launch_dp<K>(keygen_dp_kernel<K, kDpThreads, kDpMinBlocks<K>>, cnt, ls, A, noise, cnt, ek + first * P::ek_bytes,
+                        dk + first * dksz, tw);
+  });
+  if (rc) return rc;
   {  // H(ek) into dk (kyber.go:69-75)
     KernelScope ks(KID_MLKEM_HASH_EK, st);
     hash_ek_kernel<K><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(ek, P::ek_bytes, n, h);
@@ -1468,49 +1384,13 @@ __global__ void __launch_bounds__(128) r3_kdf_kernel(const uint8_t* __restrict__
   for (int j = 0; j < 4; j++) reinterpret_cast<uint64_t*>(ss + 32 * i)[j] = a[j];
 }
 
-// shared tail of round-3 encaps / decaps: (Kbar, r) = G(m || h), ct = Enc(ek, m, r) with the lenient key parse
-template <int K>
-static int r3_encrypt(const uint8_t* ek, size_t ek_stride, const uint8_t* h, size_t h_stride, const uint8_t* m, uint8_t* ct,
-                      uint8_t* kbar, uint64_t* r, char* base, const size_t (&o_A)[2], const size_t (&o_n)[2], size_t n,
-                      cudaStream_t st, int slot) {
-  using P = Params<K>;
-  Dev& c = ctx();
-  WorkSet& ws = wset(slot);
-  const size_t sub = n < kSub ? n : kSub;
-  {
-    KernelScope ks(KID_MLKEM_G, st);
-    g_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(m, h, h_stride, n, kbar, r);
-  }
-  CB200_CUDA(cudaEventRecord(ws.ev_fork, st));
-  for (int q = 0; q < 2; q++) CB200_CUDA(cudaStreamWaitEvent(ws.lane[q], ws.ev_fork, 0));
-  int l = 0;
-  for (size_t first = 0; first < n; first += sub, l ^= 1) {
-    cudaStream_t ls = profiling_on() ? st : ws.lane[l];
-    int16_t* A = (int16_t*)(base + o_A[l]);
-    int16_t* noise = (int16_t*)(base + o_n[l]);
-    const size_t cnt = (n - first < sub) ? n - first : sub;
-    if (int src = launch_sample<K>(slot, l, ls, ek + 384 * K + first * ek_stride, ek_stride, cnt, r + 4 * first, cnt, A, noise,
-                                   1, P::n_noise, 4, K))
-      return src;
-    if (int erc = launch_encrypt<K>(ek + first * ek_stride, ek_stride, A, 0, noise, m + 32 * first, cnt,
-                                    ct + first * P::ct_bytes, nullptr, nullptr, 1, ls))
-      return erc;
-  }
-  for (int q = 0; q < 2; q++) {
-    CB200_CUDA(cudaEventRecord(ws.ev_join[q], ws.lane[q]));
-    CB200_CUDA(cudaStreamWaitEvent(st, ws.ev_join[q], 0));
-  }
-  return 0;
-}
-
 // mode 0: encaps (in = seeds, key = ek), mode 1: decaps (in = ct, key = dk); per-op keys
 template <int K>
 static int r3_device(int decaps, const uint8_t* key, size_t key_stride, const uint8_t* in, uint8_t* ct_out, uint8_t* ss, size_t n,
                      cudaStream_t st, int slot) {
   using P = Params<K>;
   Dev& c = ctx();
-  WorkSet& ws = wset(slot);
-  const size_t sub = n < kSub ? n : kSub;
+  const size_t sub = sub_batch(n);
   size_t off = 0;
   auto take = [&](size_t bytes) {
     size_t o = off;
@@ -1543,18 +1423,16 @@ static int r3_device(int decaps, const uint8_t* key, size_t key_stride, const ui
       KernelScope ks(KID_MLKEM_HASH_EK, st);
       hash_ek_kernel<K><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(key, key_stride, n, h);
     }
-    rc = r3_encrypt<K>(key, key_stride, (const uint8_t*)h, 32, m, ct_out, kbar, r, b, o_A, o_n, n, st, slot);
+    rc = encrypt_lenient<K>(key, key_stride, (const uint8_t*)h, 32, m, ct_out, kbar, r, b, o_A, o_n, n, st, slot);
     if (rc) return rc;
     KernelScope ks(KID_MLKEM_G, st);
     r3_kdf_kernel<K><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(ct_out, nullptr, kbar, nullptr, 0, n, ss);
   } else {
     uint8_t* ct2 = (uint8_t*)(b + o_ct2);
     const uint8_t* ek = key + 384 * K;
-    {
-      KernelScope ks(KID_MLKEM_ENCRYPT, st);
-      if (int drc = launch_decrypt<K>(key, key_stride, in, n, m, tw, st)) return drc;
-    }
-    rc = r3_encrypt<K>(ek, key_stride, key + 384 * K + P::ek_bytes, key_stride, m, ct2, kbar, r, b, o_A, o_n, n, st, slot);
+    if (int drc = launch_dp<K>(decrypt_dp_kernel<K, kDpThreads, kDpMinBlocks<K>>, n, st, key, key_stride, in, n, m, tw))
+      return drc;
+    rc = encrypt_lenient<K>(ek, key_stride, key + 384 * K + P::ek_bytes, key_stride, m, ct2, kbar, r, b, o_A, o_n, n, st, slot);
     if (rc) return rc;
     KernelScope ks(KID_MLKEM_G, st);
     r3_kdf_kernel<K><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(in, ct2, kbar, key + 384 * K + P::ek_bytes + 32, key_stride,
@@ -1565,14 +1443,6 @@ static int r3_device(int decaps, const uint8_t* key, size_t key_stride, const ui
 }
 
 // ------------------------------------------------------------------ host side
-struct Work {
-  uint64_t* h;      // nkeys x 4
-  uint64_t* r;      // n x 4
-  int16_t* A;       // nkeys_sub x K*K x 256
-  int16_t* noise;   // sub x (2K+1) x 256
-};
-
-
 // push_ct / push_ss (optional): where the rows of this call belong in a gather destination -- rank 0's buffer mapped
 // through CUDA IPC, or local memory.  Every sub-batch is copied there as soon as its encrypt kernel has run, by the copy
 // engines on the work set's copy stream, while the next sub-batches compute: the result gather of SURVEY.md 8(e)
@@ -1586,7 +1456,7 @@ static int encaps_device(const uint8_t* ek, size_t ek_stride, const uint8_t* see
   WorkSet& ws = wset(slot);
   const bool shared = (ek_stride == 0);
   const size_t nkeys = shared ? 1 : n;
-  const size_t sub = n < kSub ? n : kSub;
+  const size_t sub = sub_batch(n);
   const size_t subkeys = shared ? 1 : sub;
   size_t off = 0;
   auto take = [&](size_t bytes) {
@@ -1619,24 +1489,17 @@ static int encaps_device(const uint8_t* ek, size_t ek_stride, const uint8_t* see
     if (int src = launch_sample<K>(slot, 0, st, ek + 384 * K, 0, 1, r, 0, (int16_t*)((char*)base + o_A[0]),
                                    (int16_t*)((char*)base + o_n[0]), 1, P::n_noise, 4, K))
       return src;
-  // Sub-batches alternate between two internal streams (fork/join on events): the tail wave of one
-  // sub-batch's kernels overlaps the next sub-batch instead of idling SMs.
-  CB200_CUDA(cudaEventRecord(ws.ev_fork, st));
-  for (int l = 0; l < 2; l++) CB200_CUDA(cudaStreamWaitEvent(ws.lane[l], ws.ev_fork, 0));
-  int l = 0;
-  for (size_t first = 0; first < n; first += sub, l ^= 1) {
-    // per-kernel event timing (cb200_profile_enable) wants true, non-overlapped durations: stay on one stream
-    cudaStream_t ls = profiling_on() ? st : ws.lane[l];
+  const kyber::TwPair* tw = (const kyber::TwPair*)c.kyber_tw;
+  rc = for_sub_batches(ws, n, st, [&](size_t first, size_t cnt, int l, cudaStream_t ls) {
     int16_t* A = (int16_t*)((char*)base + o_A[l]);
     int16_t* noise = (int16_t*)((char*)base + o_n[l]);
-    const size_t cnt = (n - first < sub) ? n - first : sub;
     const size_t keys_here = shared ? 0 : cnt;
     if (int src = launch_sample<K>(slot, l, ls, ek + 384 * K + (shared ? 0 : first * ek_stride), ek_stride, keys_here,
                                    r + 4 * first, cnt, A, noise, 1, P::n_noise, 4, K))
       return src;
-    if (int erc = launch_encrypt<K>(ek + (shared ? 0 : first * ek_stride), ek_stride, A, shared ? 1 : 0, noise,
-                                    seeds + 32 * first, cnt, ct + first * P::ct_bytes, ss + 32 * first,
-                                    status ? status + first : nullptr, 0, ls))
+    if (int erc = launch_dp<K>(encrypt_dp_kernel<K, kDpThreads, kDpMinBlocks<K>>, cnt, ls,
+                               ek + (shared ? 0 : first * ek_stride), ek_stride, A, shared ? 1 : 0, noise, seeds + 32 * first,
+                               cnt, ct + first * P::ct_bytes, ss + 32 * first, status ? status + first : nullptr, tw, 0))
       return erc;
     if (push_ct || push_ss) {
       CB200_CUDA(cudaEventRecord(ws.ev_copy, ls));
@@ -1646,14 +1509,12 @@ static int encaps_device(const uint8_t* ek, size_t ek_stride, const uint8_t* see
                                    cudaMemcpyDefault, ws.copy));
       if (push_ss) CB200_CUDA(cudaMemcpyAsync(push_ss + 32 * first, ss + 32 * first, cnt * 32, cudaMemcpyDefault, ws.copy));
     }
-  }
+    return 0;
+  });
+  if (rc) return rc;
   if (push_ct || push_ss) {  // the caller's stream covers the pushes too
     CB200_CUDA(cudaEventRecord(ws.ev_copy, ws.copy));
     CB200_CUDA(cudaStreamWaitEvent(st, ws.ev_copy, 0));
-  }
-  for (int q = 0; q < 2; q++) {
-    CB200_CUDA(cudaEventRecord(ws.ev_join[q], ws.lane[q]));
-    CB200_CUDA(cudaStreamWaitEvent(st, ws.ev_join[q], 0));
   }
   CB200_CUDA(cudaGetLastError());
   return 0;
