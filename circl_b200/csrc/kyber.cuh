@@ -417,6 +417,104 @@ __host__ __device__ __forceinline__ bool words_in_range(const uint32_t (&w)[16],
 #endif
 }
 
+// ---------------------------------------------------------------- noise on the S layout
+// prmt.b32 with the full selector: bit 3 of a nibble replicates the sign of the selected byte (__byte_perm masks it off)
+__host__ __device__ __forceinline__ uint32_t prmt_sx(uint32_t a, uint32_t b, uint32_t sel) {
+#ifdef __CUDA_ARCH__
+  uint32_t d;
+  asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(sel));
+  return d;
+#else
+  const uint64_t x = ((uint64_t)b << 32) | a;
+  uint32_t d = 0;
+  for (int i = 0; i < 4; i++) {
+    const uint32_t s = (sel >> (4 * i)) & 0xf, byte = (uint32_t)(x >> (8 * (s & 7))) & 0xff;
+    d |= ((s & 8) ? ((byte & 0x80) ? 0xffu : 0u) : byte) << (8 * i);
+  }
+  return d;
+#endif
+}
+// CBD_2 (sample.go:80-93) of four PRF bytes: w[q] = the pair (coefficient of the low nibble, of the high nibble) of byte
+// q of t, packed as two int16.  d = (t & 0x55..) + ((t >> 1) & 0x55..) holds, per nibble j, a_j in its low and b_j in its
+// high two bits, and coefficient j = a_j - b_j.  Bytewise: even coefficients sit in the low nibbles of the four bytes, odd
+// ones in the high nibbles; (0x80 | a) - b never borrows across bytes and ^ 0x80 turns it into the signed byte a - b; one
+// PRMT per output word then widens a byte pair to two int16 (selector bit 3 replicates the sign).  19 instructions per
+// eight coefficients instead of ~55 for the field-by-field form.
+__host__ __device__ __forceinline__ void cbd2_words(uint32_t t, uint32_t (&w)[4]) {
+  const uint32_t d = (t & 0x55555555u) + ((t >> 1) & 0x55555555u);
+  const uint32_t ae = d & 0x03030303u, be = (d >> 2) & 0x03030303u;
+  const uint32_t ao = (d >> 4) & 0x03030303u, bo = (d >> 6) & 0x03030303u;
+  const uint32_t ce = ((ae | 0x80808080u) - be) ^ 0x80808080u;  // signed bytes: coefficients 0, 2, 4, 6
+  const uint32_t co = ((ao | 0x80808080u) - bo) ^ 0x80808080u;  // coefficients 1, 3, 5, 7
+  w[0] = prmt_sx(ce, co, 0xc480);
+  w[1] = prmt_sx(ce, co, 0xd591);
+  w[2] = prmt_sx(ce, co, 0xe6a2);
+  w[3] = prmt_sx(ce, co, 0xf7b3);
+}
+
+// CBD_eta (sample.go:31-95) of a PRF output B of 64 eta bytes, lane by lane: coefficient c is nibble c of B (eta = 2)
+// or bits [6 c, 6 c + 6) (eta = 3), so for its S-layout coefficients 16 s + 2 v + b lane v needs, for s = 0..15, byte
+// 8 s + v of B (eta = 2) or the 12 bits at bit 96 s + 12 v (eta = 3).  noise_select gathers them from the 32 / 48
+// little-endian words of B into kNoiseWords words: byte s & 3 of word s >> 2 (eta = 2), the field of s at bit 16 (s & 1)
+// of word s >> 1 (eta = 3).  noise_pairs turns the words of s = 4 k .. 4 k + 3 into the four packed pairs of
+// coefficients 16 s + 2 v + {0, 1}.
+template <int ETA>
+constexpr int kNoiseWords = ETA == 2 ? 4 : 8;
+template <int ETA>
+__host__ __device__ __forceinline__ void noise_select(const uint32_t* w, int v, uint32_t (&x)[kNoiseWords<ETA>]) {
+  if constexpr (ETA == 2) {
+    const int h = v >> 2;
+    const uint32_t sel = (uint32_t)(v & 3) | ((uint32_t)(4 + (v & 3)) << 4);  // byte v & 3 of two words
+#pragma unroll
+    for (int k = 0; k < 4; k++) {  // s = 4 k + q lies in word 2 s + h
+      const uint32_t t01 = prmt_sx(w[8 * k + h], w[8 * k + 2 + h], sel);
+      const uint32_t t23 = prmt_sx(w[8 * k + 4 + h], w[8 * k + 6 + h], sel);
+      x[k] = prmt_sx(t01, t23, 0x5410);
+    }
+  } else {
+    const int wo = (12 * v) >> 5, sh = (12 * v) & 31;
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+      uint32_t f[2];
+#pragma unroll
+      for (int b = 0; b < 2; b++) {
+        const int s = 2 * i + b;
+        const uint64_t lo = w[3 * s + wo], hi = sh > 20 ? w[3 * s + wo + 1] : 0u;  // lanes 2 and 5 straddle two words
+        f[b] = (uint32_t)(((hi << 32) | lo) >> sh) & 0xfffu;
+      }
+      x[i] = f[0] | (f[1] << 16);
+    }
+  }
+}
+template <int ETA>
+__host__ __device__ __forceinline__ void noise_pairs(const uint32_t (&x)[kNoiseWords<ETA>], int k, uint32_t (&p)[4]) {
+  if constexpr (ETA == 2) {
+    cbd2_words(x[k], p);
+  } else {  // per 6-bit half of a field: (sum of its low three bits) - (sum of its high three bits)
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+      const uint32_t t = x[2 * k + i], m = 0x02490249u;
+      const uint32_t d = (t & m) + ((t >> 1) & m) + ((t >> 2) & m);
+#pragma unroll
+      for (int b = 0; b < 2; b++) {
+        const uint32_t e = d >> (16 * b);
+        p[2 * i + b] = pack2_lo((int32_t)(e & 7) - (int32_t)((e >> 3) & 7), (int32_t)((e >> 6) & 7) - (int32_t)((e >> 9) & 7));
+      }
+    }
+  }
+}
+// all 32 coefficients of the lane, S layout
+template <int ETA>
+__host__ __device__ __forceinline__ void noise_cbd(const uint32_t (&x)[kNoiseWords<ETA>], int32_t (&r)[32]) {
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    uint32_t p[4];
+    noise_pairs<ETA>(x, k, p);
+#pragma unroll
+    for (int q = 0; q < 4; q++) unpack2_lo(p[q], r[8 * k + 2 * q], r[8 * k + 2 * q + 1]);
+  }
+}
+
 // The low-format pairs of the C-layout passes are kept lane-transposed (in the device table and therefore in its
 // shared-memory copy): "entry i of lane v" of a layer, Zetas position base + c v + i (c = 2, 4, 8 entries per lane for
 // l = 8, 4, 2), is stored at base + 8 i + v, so the eight lanes of an octet read eight consecutive pairs instead of

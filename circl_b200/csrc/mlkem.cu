@@ -10,11 +10,11 @@
 //     CompressTo                      common/poly.go:248-328
 //
 // Pipeline (all intermediates stay on the device; sub-batches are sized so that
-// A^T and the noise polynomials live in the 126 MB L2 between kernels):
+// A^T lives in the 50 MB L2 between kernels):
 //   1. hash_kernel    one thread per op/key: h = SHA3-256(ek), (K', r) = SHA3-512(m || h)
-//   2. sample_kernel  one thread per Keccak stream: K*K SHAKE128 matrix streams per key,
-//                     2K+1 SHAKE256 noise streams per op (warps are stream-homogeneous)
-//   3. encrypt_dp_kernel one octet (8 lanes) per op: NTT(r), A^T o r, t o r, InvNTT, +e, compress
+//   2. sample_kernel  one thread per Keccak stream: K*K SHAKE128 matrix streams per key
+//   3. encrypt_dp_kernel one octet (8 lanes) per op: the 2K+1 SHAKE256 noise streams (lane p: nonces p, p + 8),
+//                     NTT(r), A^T o r, t o r, InvNTT, +e, compress
 #include <stdlib.h>
 #include <string.h>
 
@@ -130,44 +130,25 @@ __device__ __forceinline__ uint32_t reject_block(const uint64_t (&a)[25], uint32
   return wp;
 }
 
-// CBD_2 of 128 bytes (sample.go:80-93), written as 256 packed int16.  Eight coefficients per 32-bit word t of the
-// PRF output: d = (t & 0x55..) + ((t >> 1) & 0x55..) holds, per nibble j, a_j in its low and b_j in its high two bits, and
-// coefficient j = a_j - b_j.  Bytewise: even coefficients sit in the low nibbles of the four bytes, odd ones in the
-// high nibbles; (0x80 | a) - b never borrows across bytes and ^ 0x80 turns it into the signed byte a - b; one PRMT per
-// output word then widens a byte pair to two int16 (selector bit 3 replicates the sign).  19 instructions per eight
-// coefficients instead of ~55 for the field-by-field form.
-// prmt.b32 with the full selector: bit 3 of a nibble replicates the sign of the selected byte (__byte_perm masks it off)
-__device__ __forceinline__ uint32_t prmt_sx(uint32_t a, uint32_t b, uint32_t sel) {
-  uint32_t d;
-  asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(sel));
-  return d;
-}
-__device__ __forceinline__ void cbd2_words(uint32_t t, uint32_t (&w)[4]) {
-  const uint32_t d = (t & 0x55555555u) + ((t >> 1) & 0x55555555u);
-  const uint32_t ae = d & 0x03030303u, be = (d >> 2) & 0x03030303u;
-  const uint32_t ao = (d >> 4) & 0x03030303u, bo = (d >> 6) & 0x03030303u;
-  const uint32_t ce = ((ae | 0x80808080u) - be) ^ 0x80808080u;  // signed bytes: coefficients 0, 2, 4, 6
-  const uint32_t co = ((ao | 0x80808080u) - bo) ^ 0x80808080u;  // coefficients 1, 3, 5, 7
-  w[0] = prmt_sx(ce, co, 0xc480);
-  w[1] = prmt_sx(ce, co, 0xd591);
-  w[2] = prmt_sx(ce, co, 0xe6a2);
-  w[3] = prmt_sx(ce, co, 0xf7b3);
-}
+// CBD_2 of 128 bytes (sample.go:80-93), written as 256 packed int16 (kyber::cbd2_words: eight coefficients per word)
 __device__ __forceinline__ void cbd2_store(const uint64_t (&a)[25], int16_t* __restrict__ dst) {
   uint4* out = reinterpret_cast<uint4*>(dst);
 #pragma unroll
   for (int i = 0; i < 16; i++) {
     uint32_t lo[4], hi[4];
-    cbd2_words((uint32_t)a[i], lo);
-    cbd2_words((uint32_t)(a[i] >> 32), hi);
+    kyber::cbd2_words((uint32_t)a[i], lo);
+    kyber::cbd2_words((uint32_t)(a[i] >> 32), hi);
     out[2 * i] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
     out[2 * i + 1] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
   }
 }
 
-// sub-batch size: A^T + noise of one sub-batch (8 KiB / op for K=3, 12.5 KiB for K=4) stay in the 50 MB L2
-// (ML-KEM-768, 2^20 per-op keys, H100 SXM at 400 W: 24.7 ms per step at 4096, 25.5 at 8192, 30.0 at 2048)
-constexpr size_t kSub = 4096;
+// sub-batch size.  A sub-batch leaves only A^T in memory (4.5 KiB / op for K=3, 8 KiB for K=4), so two 4096-op
+// sub-batches in flight fit the 50 MB L2 and two of 8192 do not; 8192 still measured faster (ML-KEM-768, 2^20 per-op
+// keys, H100 80GB HBM3 SXM at 700 W: 19.9 ms per step against 20.9 at 4096), as it halves the launches and the tail
+// waves, sample_fix_kernel's most of all (1.8 against 3.5 ms per step).  With the noise still in memory (8 KiB / op)
+// 4096 had been the faster (H100 SXM at 400 W: 24.7 ms per step at 4096, 25.5 at 8192, 30.0 at 2048).
+constexpr size_t kSub = 8192;
 constexpr int kRowWords = 129;  // 256 int16 + 2 slack, odd word stride
 constexpr int kSampleSmem = 128 * kRowWords * 4;
 
@@ -259,72 +240,50 @@ __device__ __forceinline__ void noise_stream(uint64_t (&a)[25], int16_t* __restr
   }
 }
 
-// Stream index space (blockDim-aligned so that warps never mix stream kinds):
-//   [0, nkeys*K*K)               matrix streams, s = (i*K + j) * nkeys + key  -> A^T[key][i][j] = XOF(rho, i, j)
-//   then n*(2K+1) noise streams, s = nonce * n + op                            -> PRF(r_op, nonce)
+// One thread per matrix stream, s = (i*K + j) * nkeys + key -> A^T[key][i][j] = XOF(rho, i, j).  (The noise is made
+// by the K-PKE kernels themselves, octet_prf.)
 template <int K>
 __global__ void __launch_bounds__(128) sample_kernel(const uint8_t* __restrict__ rho0, size_t ek_stride, size_t nkeys,
-                                                     const uint64_t* __restrict__ r, size_t n,
-                                                     int16_t* __restrict__ A, int16_t* __restrict__ noise,
-                                                     size_t mat_blocks, int transpose, int n_noise, int r_words,
-                                                     int n_eta1, FixList* __restrict__ fix) {
+                                                     int16_t* __restrict__ A, int transpose, FixList* __restrict__ fix) {
   // rho0 + key*ek_stride is rho of that key; transpose = 1 derives A^T (encryption), 0 derives A (key
-  // generation, mat.go:13-29); n_noise PRF streams per op, seeded by r[op*r_words .. +4); the first n_eta1
-  // nonces use eta1 (3 for ML-KEM-512), the others eta2 = 2
-  using P = Params<K>;
+  // generation, mat.go:13-29)
   uint64_t a[25];
   keccak::zero(a);
-  if (blockIdx.x < mat_blocks) {
-    // Each thread rejection-samples into its own shared-memory row (129-word stride: conflict-free
-    // while the counters of a warp agree); the CTA then streams the rows out as whole 512-byte polynomials.
-    extern __shared__ __align__(16) uint32_t rows[];
-    const size_t s0 = (size_t)blockIdx.x * blockDim.x;
-    const size_t s = s0 + threadIdx.x;
-    const size_t total = nkeys * K * K;
-    const bool live = s < total;
-    const size_t sc = live ? s : total - 1;
-    const size_t key = sc % nkeys;
-    const int ij = (int)(sc / nkeys), i = ij / K, j = ij % K;
-    const uint8_t* rho = rho0 + key * ek_stride;
+  // Each thread rejection-samples into its own shared-memory row (129-word stride: conflict-free
+  // while the counters of a warp agree); the CTA then streams the rows out as whole 512-byte polynomials.
+  extern __shared__ __align__(16) uint32_t rows[];
+  const size_t s0 = (size_t)blockIdx.x * blockDim.x;
+  const size_t s = s0 + threadIdx.x;
+  const size_t total = nkeys * K * K;
+  const bool live = s < total;
+  const size_t sc = live ? s : total - 1;
+  const size_t key = sc % nkeys;
+  const int ij = (int)(sc / nkeys), i = ij / K, j = ij % K;
+  const uint8_t* rho = rho0 + key * ek_stride;
 #pragma unroll
-    for (int w = 0; w < 4; w++) a[w] = keccak::ld64(rho + 8 * w);
-    // m[i][j] = XOF(rho, x, y) with (x, y) = (i, j) if transpose else (j, i)
-    a[4] = (uint64_t)(transpose ? i : j) | ((uint64_t)(transpose ? j : i) << 8) | (0x1full << 16);
-    a[20] = 0x8000000000000000ull;                               // rate 168
-    const int got = uniform_stream3(a, rows + threadIdx.x * kRowWords);
-    if (live && got < N) {  // ~1 % of the streams: finished by sample_fix_kernel from this state
-      Pending* list = reinterpret_cast<Pending*>(fix + 1);
-      Pending& e = list[atomicAdd(&fix->n, 1u)];
-      e.stream = (uint32_t)s;
-      e.count = (uint32_t)got;
+  for (int w = 0; w < 4; w++) a[w] = keccak::ld64(rho + 8 * w);
+  // m[i][j] = XOF(rho, x, y) with (x, y) = (i, j) if transpose else (j, i)
+  a[4] = (uint64_t)(transpose ? i : j) | ((uint64_t)(transpose ? j : i) << 8) | (0x1full << 16);
+  a[20] = 0x8000000000000000ull;                               // rate 168
+  const int got = uniform_stream3(a, rows + threadIdx.x * kRowWords);
+  if (live && got < N) {  // ~1 % of the streams: finished by sample_fix_kernel from this state
+    Pending* list = reinterpret_cast<Pending*>(fix + 1);
+    Pending& e = list[atomicAdd(&fix->n, 1u)];
+    e.stream = (uint32_t)s;
+    e.count = (uint32_t)got;
 #pragma unroll
-      for (int w = 0; w < 25; w++) e.a[w] = a[w];
-    }
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int p = warp; p < (int)blockDim.x; p += blockDim.x / 32) {
-      const size_t sp = s0 + p;
-      if (sp >= total) break;
-      const size_t pkey = sp % nkeys;
-      const int pij = (int)(sp / nkeys);
-      uint32_t* dst = reinterpret_cast<uint32_t*>(A + (pkey * K * K + pij) * N);
+    for (int w = 0; w < 25; w++) e.a[w] = a[w];
+  }
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int p = warp; p < (int)blockDim.x; p += blockDim.x / 32) {
+    const size_t sp = s0 + p;
+    if (sp >= total) break;
+    const size_t pkey = sp % nkeys;
+    const int pij = (int)(sp / nkeys);
+    uint32_t* dst = reinterpret_cast<uint32_t*>(A + (pkey * K * K + pij) * N);
 #pragma unroll
-      for (int w = 0; w < 4; w++) dst[32 * w + lane] = rows[p * kRowWords + 32 * w + lane];
-    }
-  } else {
-    const size_t s = (size_t)(blockIdx.x - mat_blocks) * blockDim.x + threadIdx.x;
-    if (s >= n * n_noise) return;
-    const size_t op = s % n;
-    const int nonce = (int)(s / n);
-#pragma unroll
-    for (int w = 0; w < 4; w++) a[w] = r[r_words * op + w];
-    a[4] = (uint64_t)nonce | (0x1full << 8);
-    a[16] = 0x8000000000000000ull;  // rate 136
-    int16_t* dst = noise + (op * n_noise + nonce) * N;
-    if (P::eta1 == 3 && nonce < n_eta1)
-      noise_stream<3>(a, dst);
-    else
-      noise_stream<2>(a, dst);
+    for (int w = 0; w < 4; w++) dst[32 * w + lane] = rows[p * kRowWords + 32 * w + lane];
   }
 }
 
@@ -434,19 +393,18 @@ __global__ void __launch_bounds__(64) sample_fix_kernel(FixList* __restrict__ fi
 // sample_kernel + sample_fix_kernel on stream `ls`; `lane` picks the unfinished-stream list of the work set
 template <int K>
 static int launch_sample(int slot, int lane, cudaStream_t ls, const uint8_t* rho0, size_t ek_stride, size_t nkeys,
-                         const uint64_t* r, size_t n, int16_t* A, int16_t* noise, int transpose, int n_noise, int r_words,
-                         int n_eta1) {
+                         int16_t* A, int transpose) {
+  if (nkeys == 0) return 0;
   if (int arc = ensure_smem_attr((const void*)sample_kernel<K>, kSampleSmem)) return arc;
-  const size_t streams = nkeys * K * K, mat_blocks = (streams + 127) / 128, noise_blocks = (n * n_noise + 127) / 128;
+  const size_t streams = nkeys * K * K;
   void* fix = nullptr;
-  if (int frc = ensure_fix(slot, lane, sizeof(FixList) + (streams ? streams : 1) * sizeof(Pending), ls, &fix)) return frc;
-  if (mat_blocks + noise_blocks == 0) return 0;
+  if (int frc = ensure_fix(slot, lane, sizeof(FixList) + streams * sizeof(Pending), ls, &fix)) return frc;
   {
     KernelScope ks(KID_MLKEM_SAMPLE, ls);
-    sample_kernel<K><<<(unsigned)(mat_blocks + noise_blocks), 128, kSampleSmem, ls>>>(
-        rho0, ek_stride, nkeys, r, n, A, noise, mat_blocks, transpose, n_noise, r_words, n_eta1, (FixList*)fix);
+    sample_kernel<K><<<(unsigned)((streams + 127) / 128), 128, kSampleSmem, ls>>>(rho0, ek_stride, nkeys, A, transpose,
+                                                                                 (FixList*)fix);
   }
-  if (streams) {
+  {
     KernelScope ks(KID_MLKEM_SAMPLE_FIX, ls);
     const unsigned grid = (unsigned)std::min<size_t>(64, (streams / 64 + 63) / 64 + 1);  // ~1 % of the streams, 64 per CTA
     sample_fix_kernel<K><<<grid, 64, 0, ls>>>((FixList*)fix, nkeys, A);
@@ -477,9 +435,12 @@ static int launch_sample(int slot, int lane, cudaStream_t ls, const uint8_t* rho
 // 32-bit sum p of 2 K products is below 8 . 4096 . q < 2^27, and |montReduce(p)| <= |p| / 2^16 + q / 2 <= q, which is the
 // input bound of the inverse transform's lazy-Barrett schedule (ntt.go:145-150).
 constexpr int kOpPad = 16;  // words between the operand areas of two ops: half-warps (two octets) hit disjoint banks
+// behind the operands: the lanes' words of e2 (4 each), which encrypt_dp_kernel keeps here until its last row -- in
+// registers they would push the K = 3 kernel past the 128 it may use at 7 CTAs per SM
+constexpr int kE2Words = 32;
 template <int K, int THREADS>
 struct EncSmem {
-  static constexpr int op_words = K * 128 * 2 + kOpPad;
+  static constexpr int op_words = K * 128 * 2 + kE2Words + kOpPad;
   static constexpr int words = (THREADS / 8) * op_words + (THREADS / 8) * kyber::kPolyWords + 256;
   static constexpr int bytes = words * 4;
 };
@@ -608,7 +569,45 @@ struct Octet {
   __device__ __forceinline__ bool active(size_t n) const { return base + oct < n; }
   // this octet's op, clamped to n - 1 so that an inactive octet still reads valid memory
   __device__ __forceinline__ size_t op(size_t n) const { return active(n) ? base + oct : n - 1; }
+  // the octet's whole operand area (op_words words)
+  __device__ __forceinline__ uint32_t* area() const { return reinterpret_cast<uint32_t*>(ops - v); }
 };
+
+// The noise of one op, made by its octet (K-PKE.KeyGen / Encrypt: DeriveNoise, sample.go:31-95).  Lane p runs the PRF
+// streams p, p + 8, ... < S -- SHAKE256(seed || p), the first E1 of them squeezed to 64 ETA1 bytes, the others to 128
+// (eta = 2) -- and stages the output in the octet's operand area, which is free until the first store_operands:
+// stream j at word prf_offset(j), 34 / 50 words apart so that the 64-bit stores of the lanes fall in different banks.
+// After a __syncwarp each lane gathers its words of every stream with kyber::noise_select; the polynomials never
+// exist in global memory.
+template <int ETA1, int E1>
+__host__ __device__ constexpr int prf_offset(int j) {
+  return j < E1 ? j * (ETA1 == 3 ? 50 : 34) : E1 * (ETA1 == 3 ? 50 : 34) + (j - E1) * 34;
+}
+template <int K, int THREADS, int S, int E1, int ETA1>
+__device__ __forceinline__ void octet_prf(uint32_t* area, const uint64_t* __restrict__ seed, int v) {
+  static_assert(prf_offset<ETA1, E1>(S) <= EncSmem<K, THREADS>::op_words, "PRF output must fit in the operand area");
+#pragma unroll 1
+  for (int p = v; p < S; p += 8) {
+    uint64_t a[25];
+    keccak::zero(a);
+#pragma unroll
+    for (int w = 0; w < 4; w++) a[w] = __ldg(seed + w);
+    a[4] = (uint64_t)p | (0x1full << 8);
+    a[16] = 0x8000000000000000ull;  // rate 136
+    keccak::f1600(a);
+    uint64_t* dst = reinterpret_cast<uint64_t*>(area + prf_offset<ETA1, E1>(p));
+    if (ETA1 == 3 && p < E1) {
+#pragma unroll
+      for (int q = 0; q < 17; q++) dst[q] = a[q];
+      keccak::f1600(a);
+#pragma unroll
+      for (int q = 0; q < 7; q++) dst[17 + q] = a[q];
+    } else {
+#pragma unroll
+      for (int q = 0; q < 16; q++) dst[q] = a[q];
+    }
+  }
+}
 
 // The byte-split operands W0, W1 of column j from a transformed polynomial (this lane's 32 coefficients, C layout), each
 // coefficient first multiplied by the constant of the Shoup pair (zp, kk).  Quad q of the lane has zeta = Zetas[64 + 8 v + q]:
@@ -672,10 +671,10 @@ struct DotAcc {
 template <int K, int THREADS, int MINB>
 __global__ void __launch_bounds__(THREADS, MINB) encrypt_dp_kernel(
     const uint8_t* __restrict__ ek, size_t ek_stride, const int16_t* __restrict__ A, int a_shared,
-    const int16_t* __restrict__ noise, const uint8_t* __restrict__ m, size_t n, uint8_t* __restrict__ ct,
+    const uint64_t* __restrict__ rseed, const uint8_t* __restrict__ m, size_t n, uint8_t* __restrict__ ct,
     uint8_t* __restrict__ ss, uint8_t* __restrict__ status, const kyber::TwPair* __restrict__ tw, int lenient) {
   // lenient = 1: re-encryption inside Decapsulate (PublicKey.Unpack, cpapke.go:58-63: no modulus check; the
-  // Normalize of t-hat is immaterial here because only residues are used)
+  // Normalize of t-hat is immaterial here because only residues are used).  rseed: the PRF seed r, 4 words per op.
   using P = Params<K>;
   using namespace kyber;
   // every transform of this kernel runs on low-format registers (kyber.cuh): its inputs are bounded by construction
@@ -686,24 +685,35 @@ __global__ void __launch_bounds__(THREADS, MINB) encrypt_dp_kernel(
   const size_t op = o.op(n);
   const uint8_t* ekp = ek + op * ek_stride;
   const uint32_t* Ap = reinterpret_cast<const uint32_t*>(A) + (a_shared ? 0 : op * K * K * (N / 2));
-  const uint32_t* np = reinterpret_cast<const uint32_t*>(noise) + op * P::n_noise * (N / 2);
   uint8_t* ctp = ct + op * P::ct_bytes;
 
+  // r[0..K) (eta1), e1[0..K), e2 (eta2 = 2) from PRF(r, 0 .. 2K) (cpapke.go:145-159): the lane's words of each, those
+  // of e1 kept in registers until their row (eb[0] is always the next one), those of e2 behind the operands
   int32_t r[32];
-
-  // operands of rh = NTT(r) x 512  (cpapke.go:142-144; the reduction is the multiplication)
+  uint32_t eb[K][4];
+  uint4* const e2s = reinterpret_cast<uint4*>(o.area() + 2 * 128 * K) + v;
   {
-    uint32_t nw[16];
+    uint32_t* const area = o.area();
+    octet_prf<K, THREADS, P::n_noise, K, P::eta1>(area, rseed + 4 * op, v);
+    __syncwarp();
+    uint32_t rb[K][kNoiseWords<P::eta1>], e2[4];
 #pragma unroll
-    for (int q = 0; q < 16; q++) nw[q] = ldg_stream32(np + 8 * q + v);
+    for (int j = 0; j < K; j++) {
+      noise_select<P::eta1>(area + prf_offset<P::eta1, K>(j), v, rb[j]);
+      noise_select<2>(area + prf_offset<P::eta1, K>(K + j), v, eb[j]);
+    }
+    noise_select<2>(area + prf_offset<P::eta1, K>(2 * K), v, e2);
+    *e2s = make_uint4(e2[0], e2[1], e2[2], e2[3]);
+    __syncwarp();  // the operands overwrite the staged PRF output
+
+    // operands of rh = NTT(r) x 512  (cpapke.go:142-144; the reduction is the multiplication)
 #pragma unroll 1
     for (int j = 0; j < K; j++) {
+      noise_cbd<P::eta1>(rb[0], r);
 #pragma unroll
-      for (int q = 0; q < 16; q++) unpack2_lo(nw[q], r[2 * q], r[2 * q + 1]);
-      if (j + 1 < K) {
+      for (int q = 0; q + 1 < K; q++)
 #pragma unroll
-        for (int q = 0; q < 16; q++) nw[q] = ldg_stream32(np + (j + 1) * (N / 2) + 8 * q + v);
-      }
+        for (int w = 0; w < kNoiseWords<P::eta1>; w++) rb[q][w] = rb[q + 1][w];
       fwd_pass_S_lo(r);
       store_S_lo(o.tile, v, r);
       __syncwarp();
@@ -738,7 +748,6 @@ __global__ void __launch_bounds__(THREADS, MINB) encrypt_dp_kernel(
   for (int j = 0; j < K; j++) fetch(0, 0, j, raw[j]);
 #pragma unroll 1
   for (int i = 0; i <= K; i++) {
-    uint32_t ew[16];
 #pragma unroll 1
     for (int h = 0; h < 2; h++) {
       DotAcc acc;
@@ -756,15 +765,10 @@ __global__ void __launch_bounds__(THREADS, MINB) encrypt_dp_kernel(
         if (ni <= K) fetch(ni, nh, j, raw[j]);
         acc.add(aw, o.ops + (size_t)(j * 16 + 8 * h) * 8);
       }
-      if (h == 0) {
+      if (h == 0)
         acc.reduce_into<0>(r);
-        // the noise polynomial this row ends with: in flight during the second half and the inverse transform
-        const uint32_t* e = np + (K + i) * (N / 2);
-#pragma unroll
-        for (int q = 0; q < 16; q++) ew[q] = __ldg(e + 8 * q + v);
-      } else {
+      else
         acc.reduce_into<16>(r);
-      }
     }
     inv_pass_C_lo(r, o.tabl, v);
     store_C_lo(o.tile, v, r);
@@ -776,19 +780,37 @@ __global__ void __launch_bounds__(THREADS, MINB) encrypt_dp_kernel(
     // term (1665) stays inside the int16 range the packed tile below carries
     {  // + e1[i] / + e2 (+ Decompress_q(m, 1)), S layout
       const uint32_t* mw = reinterpret_cast<const uint32_t*>(m + 32 * op);
+      uint32_t ew[4];
+      if (i < K) {
 #pragma unroll
-      for (int s = 0; s < 16; s++) {
-        int32_t e0, e1;
-        unpack2_lo(ew[s], e0, e1);
-        r[2 * s] += e0;
-        r[2 * s + 1] += e1;
-        if (i == K) {  // DecompressMessage, poly.go:134-147: coefficient idx = 16 s + 2 v + b <- bit idx of m
-          const uint32_t word = __ldg(mw + (s >> 1));
-          const uint32_t bits = (word >> (16 * (s & 1) + 2 * v)) & 3;
-          r[2 * s] += (bits & 1) ? (Q + 1) / 2 : 0;
-          r[2 * s + 1] += (bits & 2) ? (Q + 1) / 2 : 0;
+        for (int w = 0; w < 4; w++) ew[w] = eb[0][w];
+      } else {
+        const uint4 t = *e2s;
+        ew[0] = t.x, ew[1] = t.y, ew[2] = t.z, ew[3] = t.w;
+      }
+#pragma unroll
+      for (int k = 0; k < 4; k++) {
+        uint32_t ep[4];
+        noise_pairs<2>(ew, k, ep);
+#pragma unroll
+        for (int q = 0; q < 4; q++) {
+          const int s = 4 * k + q;
+          int32_t e0, e1;
+          unpack2_lo(ep[q], e0, e1);
+          r[2 * s] += e0;
+          r[2 * s + 1] += e1;
+          if (i == K) {  // DecompressMessage, poly.go:134-147: coefficient idx = 16 s + 2 v + b <- bit idx of m
+            const uint32_t word = __ldg(mw + (s >> 1));
+            const uint32_t bits = (word >> (16 * (s & 1) + 2 * v)) & 3;
+            r[2 * s] += (bits & 1) ? (Q + 1) / 2 : 0;
+            r[2 * s + 1] += (bits & 2) ? (Q + 1) / 2 : 0;
+          }
         }
       }
+#pragma unroll
+      for (int q = 0; q + 1 < K; q++)
+#pragma unroll
+        for (int w = 0; w < 4; w++) eb[q][w] = eb[q + 1][w];
     }
     store_S_lo(o.tile, v, r);  // Normalize (cpapke.go:176-177) is absorbed by compress_any
     __syncwarp();
@@ -852,12 +874,12 @@ static int for_sub_batches(WorkSet& ws, size_t n, cudaStream_t st, F&& launch) {
 }
 
 // (K', r) = G(m || h), ct = K-PKE.Encrypt(ek, m, r) with the lenient key parse, per-op keys: the re-encryption of
-// ML-KEM and round-3 Kyber Decapsulate, and the body of round-3 Kyber Encapsulate.  base + o_A[l] / o_n[l] are the
-// matrix and noise buffers of lane l.
+// ML-KEM and round-3 Kyber Decapsulate, and the body of round-3 Kyber Encapsulate.  base + o_A[l] is the matrix buffer
+// of lane l.
 template <int K>
 static int encrypt_lenient(const uint8_t* ek, size_t ek_stride, const uint8_t* h, size_t h_stride, const uint8_t* m,
-                           uint8_t* ct, uint8_t* kbar, uint64_t* r, char* base, const size_t (&o_A)[2],
-                           const size_t (&o_n)[2], size_t n, cudaStream_t st, int slot) {
+                           uint8_t* ct, uint8_t* kbar, uint64_t* r, char* base, const size_t (&o_A)[2], size_t n,
+                           cudaStream_t st, int slot) {
   using P = Params<K>;
   {
     KernelScope ks(KID_MLKEM_G, st);
@@ -866,12 +888,10 @@ static int encrypt_lenient(const uint8_t* ek, size_t ek_stride, const uint8_t* h
   const kyber::TwPair* tw = (const kyber::TwPair*)ctx().kyber_tw;
   return for_sub_batches(wset(slot), n, st, [&](size_t first, size_t cnt, int l, cudaStream_t ls) {
     int16_t* A = (int16_t*)(base + o_A[l]);
-    int16_t* noise = (int16_t*)(base + o_n[l]);
-    if (int src = launch_sample<K>(slot, l, ls, ek + 384 * K + first * ek_stride, ek_stride, cnt, r + 4 * first, cnt, A, noise,
-                                   1, P::n_noise, 4, K))
-      return src;
+    if (int src = launch_sample<K>(slot, l, ls, ek + 384 * K + first * ek_stride, ek_stride, cnt, A, 1)) return src;
     return launch_dp<K>(encrypt_dp_kernel<K, kDpThreads, kDpMinBlocks<K>>, cnt, ls, ek + first * ek_stride, ek_stride, A, 0,
-                        noise, m + 32 * first, cnt, ct + first * P::ct_bytes, nullptr, nullptr, tw, 1);
+                        (const uint64_t*)(r + 4 * first), m + 32 * first, cnt, ct + first * P::ct_bytes, nullptr, nullptr,
+                        tw, 1);
   });
 }
 
@@ -1059,11 +1079,8 @@ static int decaps_device(const uint8_t* dk, size_t dk_stride, const uint8_t* ct,
   };
   const size_t o_h = take(n * 32), o_r = take(n * 32), o_m = take(n * 32), o_k = take(n * 32),
                o_ct2 = take(n * (size_t)P::ct_bytes);
-  size_t o_A[2], o_n[2];
-  for (int q = 0; q < 2; q++) {
-    o_A[q] = take(sub * K * K * 512);
-    o_n[q] = take(sub * P::n_noise * 512);
-  }
+  size_t o_A[2];
+  for (int q = 0; q < 2; q++) o_A[q] = take(sub * K * K * 512);
   void* base = nullptr;
   int rc = ensure_work(slot, off, &base);
   if (rc) return rc;
@@ -1083,7 +1100,7 @@ static int decaps_device(const uint8_t* dk, size_t dk_stride, const uint8_t* ct,
     hash_ek_kernel<K><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(ek, dk_stride, n, h);
   }
   // (K', r') = G(m' || h) with the h stored in dk (kyber.go:160-164), ct' = K-PKE.Encrypt(ek, m', r')
-  rc = encrypt_lenient<K>(ek, dk_stride, dk + 384 * K + P::ek_bytes, dk_stride, mprime, ct2, kbar, r, b, o_A, o_n, n, st, slot);
+  rc = encrypt_lenient<K>(ek, dk_stride, dk + 384 * K + P::ek_bytes, dk_stride, mprime, ct2, kbar, r, b, o_A, n, st, slot);
   if (rc) return rc;
   {
     KernelScope ks(KID_MLKEM_G, st);
@@ -1147,7 +1164,7 @@ __device__ __forceinline__ void pack12_C(const int32_t (&r)[32], uint32_t (&w)[1
 // low-format registers (inputs |c| <= 3).
 template <int K, int THREADS, int MINB>
 __global__ void __launch_bounds__(THREADS, MINB) keygen_dp_kernel(const int16_t* __restrict__ A,
-                                                                  const int16_t* __restrict__ noise, size_t n,
+                                                                  const uint64_t* __restrict__ rs, size_t n,
                                                                   uint8_t* __restrict__ ek, uint8_t* __restrict__ dk,
                                                                   const kyber::TwPair* __restrict__ tw) {
   using P = Params<K>;
@@ -1160,23 +1177,32 @@ __global__ void __launch_bounds__(THREADS, MINB) keygen_dp_kernel(const int16_t*
   const int v = o.v;
   const size_t op = o.op(n);
   const uint32_t* Ap = reinterpret_cast<const uint32_t*>(A) + op * K * K * (N / 2);
-  const uint32_t* np = reinterpret_cast<const uint32_t*>(noise) + op * (2 * K) * (N / 2);
   uint8_t* ekp = ek + op * P::ek_bytes;
   uint8_t* dkp = dk + op * (768 * K + 96);
 
+  // s[0..K), e[0..K) (both eta1) from PRF(sigma, 0 .. 2K) (cpapke.go:81-94), sigma = rs[8 op + 4 ..): the lane's words of
+  // each, the e-words kept until their row (eb[0] is always the next one)
+  constexpr int NW = kNoiseWords<P::eta1>;
   int32_t r[32];
+  uint32_t eb[K][NW];
   {  // s-hat[j]: packed into dk (normalised) and turned into the operands of the products
-    uint32_t nw[16];
+    uint32_t* const area = o.area();
+    octet_prf<K, THREADS, 2 * K, 2 * K, P::eta1>(area, rs + 8 * op + 4, v);
+    __syncwarp();
+    uint32_t sb[K][NW];
 #pragma unroll
-    for (int q = 0; q < 16; q++) nw[q] = ldg_stream32(np + 8 * q + v);
+    for (int j = 0; j < K; j++) {
+      noise_select<P::eta1>(area + prf_offset<P::eta1, 2 * K>(j), v, sb[j]);
+      noise_select<P::eta1>(area + prf_offset<P::eta1, 2 * K>(K + j), v, eb[j]);
+    }
+    __syncwarp();  // the operands overwrite the staged PRF output
 #pragma unroll 1
     for (int j = 0; j < K; j++) {
+      noise_cbd<P::eta1>(sb[0], r);
 #pragma unroll
-      for (int q = 0; q < 16; q++) unpack2_lo(nw[q], r[2 * q], r[2 * q + 1]);
-      if (j + 1 < K) {
+      for (int q = 0; q + 1 < K; q++)
 #pragma unroll
-        for (int q = 0; q < 16; q++) nw[q] = ldg_stream32(np + (j + 1) * (N / 2) + 8 * q + v);
-      }
+        for (int w = 0; w < NW; w++) sb[q][w] = sb[q + 1][w];
       fwd_pass_S_lo(r);
       store_S_lo(o.tile, v, r);
       __syncwarp();
@@ -1207,17 +1233,13 @@ __global__ void __launch_bounds__(THREADS, MINB) keygen_dp_kernel(const int16_t*
   uint32_t raw[K][8];
 #pragma unroll
   for (int j = 0; j < K; j++) fetch(0, 0, j, raw[j]);
-  uint32_t ew[16];
-#pragma unroll
-  for (int q = 0; q < 16; q++) ew[q] = __ldg(np + K * (N / 2) + 8 * q + v);
 #pragma unroll 1
   for (int i = 0; i < K; i++) {
+    noise_cbd<P::eta1>(eb[0], r);  // e-hat[i] = NTT(e[i])
 #pragma unroll
-    for (int q = 0; q < 16; q++) unpack2_lo(ew[q], r[2 * q], r[2 * q + 1]);  // e-hat[i] = NTT(e[i])
-    if (i + 1 < K) {
+    for (int q = 0; q + 1 < K; q++)
 #pragma unroll
-      for (int q = 0; q < 16; q++) ew[q] = __ldg(np + (K + i + 1) * (N / 2) + 8 * q + v);
-    }
+      for (int w = 0; w < NW; w++) eb[q][w] = eb[q + 1][w];
     fwd_pass_S_lo(r);
     store_S_lo(o.tile, v, r);
     __syncwarp();
@@ -1278,11 +1300,8 @@ static int keygen_device(const uint8_t* seeds, uint8_t* ek, uint8_t* dk, size_t 
     return o;
   };
   const size_t o_rs = take(n * 64), o_h = take(n * 32);
-  size_t o_A[2], o_n[2];
-  for (int q = 0; q < 2; q++) {
-    o_A[q] = take(sub * K * K * 512);
-    o_n[q] = take(sub * 2 * K * 512);
-  }
+  size_t o_A[2];
+  for (int q = 0; q < 2; q++) o_A[q] = take(sub * K * K * 512);
   void* base = nullptr;
   int rc = ensure_work(slot, off, &base);
   if (rc) return rc;
@@ -1297,13 +1316,10 @@ static int keygen_device(const uint8_t* seeds, uint8_t* ek, uint8_t* dk, size_t 
   const kyber::TwPair* tw = (const kyber::TwPair*)c.kyber_tw;
   rc = for_sub_batches(wset(slot), n, st, [&](size_t first, size_t cnt, int l, cudaStream_t ls) {
     int16_t* A = (int16_t*)(b + o_A[l]);
-    int16_t* noise = (int16_t*)(b + o_n[l]);
-    // A (not transposed) from rho = rs[0..4), s/e noise from sigma = rs[4..8)
-    if (int src = launch_sample<K>(slot, l, ls, (const uint8_t*)(rs + 8 * first), 64, cnt, rs + 8 * first + 4, cnt, A, noise, 0,
-                                   2 * K, 8, 2 * K))
-      return src;
-    return launch_dp<K>(keygen_dp_kernel<K, kDpThreads, kDpMinBlocks<K>>, cnt, ls, A, noise, cnt, ek + first * P::ek_bytes,
-                        dk + first * dksz, tw);
+    // A (not transposed) from rho = rs[0..4); the kernel derives s and e from sigma = rs[4..8)
+    if (int src = launch_sample<K>(slot, l, ls, (const uint8_t*)(rs + 8 * first), 64, cnt, A, 0)) return src;
+    return launch_dp<K>(keygen_dp_kernel<K, kDpThreads, kDpMinBlocks<K>>, cnt, ls, A, (const uint64_t*)(rs + 8 * first), cnt,
+                        ek + first * P::ek_bytes, dk + first * dksz, tw);
   });
   if (rc) return rc;
   {  // H(ek) into dk (kyber.go:69-75)
@@ -1399,11 +1415,8 @@ static int r3_device(int decaps, const uint8_t* key, size_t key_stride, const ui
   };
   const size_t o_h = take(n * 32), o_r = take(n * 32), o_m = take(n * 32), o_k = take(n * 32),
                o_ct2 = take(decaps ? n * (size_t)P::ct_bytes : 0);
-  size_t o_A[2], o_n[2];
-  for (int q = 0; q < 2; q++) {
-    o_A[q] = take(sub * K * K * 512);
-    o_n[q] = take(sub * P::n_noise * 512);
-  }
+  size_t o_A[2];
+  for (int q = 0; q < 2; q++) o_A[q] = take(sub * K * K * 512);
   void* basev = nullptr;
   int rc = ensure_work(slot, off, &basev);
   if (rc) return rc;
@@ -1423,7 +1436,7 @@ static int r3_device(int decaps, const uint8_t* key, size_t key_stride, const ui
       KernelScope ks(KID_MLKEM_HASH_EK, st);
       hash_ek_kernel<K><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(key, key_stride, n, h);
     }
-    rc = encrypt_lenient<K>(key, key_stride, (const uint8_t*)h, 32, m, ct_out, kbar, r, b, o_A, o_n, n, st, slot);
+    rc = encrypt_lenient<K>(key, key_stride, (const uint8_t*)h, 32, m, ct_out, kbar, r, b, o_A, n, st, slot);
     if (rc) return rc;
     KernelScope ks(KID_MLKEM_G, st);
     r3_kdf_kernel<K><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(ct_out, nullptr, kbar, nullptr, 0, n, ss);
@@ -1432,7 +1445,7 @@ static int r3_device(int decaps, const uint8_t* key, size_t key_stride, const ui
     const uint8_t* ek = key + 384 * K;
     if (int drc = launch_dp<K>(decrypt_dp_kernel<K, kDpThreads, kDpMinBlocks<K>>, n, st, key, key_stride, in, n, m, tw))
       return drc;
-    rc = encrypt_lenient<K>(ek, key_stride, key + 384 * K + P::ek_bytes, key_stride, m, ct2, kbar, r, b, o_A, o_n, n, st, slot);
+    rc = encrypt_lenient<K>(ek, key_stride, key + 384 * K + P::ek_bytes, key_stride, m, ct2, kbar, r, b, o_A, n, st, slot);
     if (rc) return rc;
     KernelScope ks(KID_MLKEM_G, st);
     r3_kdf_kernel<K><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(in, ct2, kbar, key + 384 * K + P::ek_bytes + 32, key_stride,
@@ -1465,11 +1478,9 @@ static int encaps_device(const uint8_t* ek, size_t ek_stride, const uint8_t* see
     return o;
   };
   const size_t o_h = take(nkeys * 32), o_r = take(n * 32);
-  size_t o_A[2], o_n[2];
+  size_t o_A[2];
   o_A[0] = take(subkeys * K * K * 512);
   o_A[1] = shared ? o_A[0] : take(subkeys * K * K * 512);
-  o_n[0] = take(sub * P::n_noise * 512);
-  o_n[1] = take(sub * P::n_noise * 512);
   void* base = nullptr;
   int rc = ensure_work(slot, off, &base);
   if (rc) return rc;
@@ -1485,21 +1496,18 @@ static int encaps_device(const uint8_t* ek, size_t ek_stride, const uint8_t* see
     KernelScope ks(KID_MLKEM_G, st);
     g_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(seeds, (const uint8_t*)h, shared ? 0 : 32, n, ss, r);
   }
-  if (shared)  // one key: A^T is derived once, before the sub-batches fork
-    if (int src = launch_sample<K>(slot, 0, st, ek + 384 * K, 0, 1, r, 0, (int16_t*)((char*)base + o_A[0]),
-                                   (int16_t*)((char*)base + o_n[0]), 1, P::n_noise, 4, K))
-      return src;
+  // one key: A^T is derived once, before the sub-batches fork, and a sub-batch is then a single kernel
+  if (shared)
+    if (int src = launch_sample<K>(slot, 0, st, ek + 384 * K, 0, 1, (int16_t*)((char*)base + o_A[0]), 1)) return src;
   const kyber::TwPair* tw = (const kyber::TwPair*)c.kyber_tw;
   rc = for_sub_batches(ws, n, st, [&](size_t first, size_t cnt, int l, cudaStream_t ls) {
     int16_t* A = (int16_t*)((char*)base + o_A[l]);
-    int16_t* noise = (int16_t*)((char*)base + o_n[l]);
-    const size_t keys_here = shared ? 0 : cnt;
-    if (int src = launch_sample<K>(slot, l, ls, ek + 384 * K + (shared ? 0 : first * ek_stride), ek_stride, keys_here,
-                                   r + 4 * first, cnt, A, noise, 1, P::n_noise, 4, K))
-      return src;
+    if (!shared)
+      if (int src = launch_sample<K>(slot, l, ls, ek + 384 * K + first * ek_stride, ek_stride, cnt, A, 1)) return src;
     if (int erc = launch_dp<K>(encrypt_dp_kernel<K, kDpThreads, kDpMinBlocks<K>>, cnt, ls,
-                               ek + (shared ? 0 : first * ek_stride), ek_stride, A, shared ? 1 : 0, noise, seeds + 32 * first,
-                               cnt, ct + first * P::ct_bytes, ss + 32 * first, status ? status + first : nullptr, tw, 0))
+                               ek + (shared ? 0 : first * ek_stride), ek_stride, A, shared ? 1 : 0,
+                               (const uint64_t*)(r + 4 * first), seeds + 32 * first, cnt, ct + first * P::ct_bytes,
+                               ss + 32 * first, status ? status + first : nullptr, tw, 0))
       return erc;
     if (push_ct || push_ss) {
       CB200_CUDA(cudaEventRecord(ws.ev_copy, ls));
@@ -1529,7 +1537,7 @@ static int encaps_any(int k, const uint8_t* ek, size_t ek_stride, const uint8_t*
 }
 
 // ------------------------------------------------------------------ 7. the sampler and serialisation surface on its own
-// (*Poly).DeriveUniform (sample.go:192-236) for n independent (seed, x, y): the matrix branch of sample_kernel
+// (*Poly).DeriveUniform (sample.go:192-236) for n independent (seed, x, y): the stream of sample_kernel
 __global__ void __launch_bounds__(128) derive_uniform_kernel(const uint8_t* __restrict__ seeds, size_t seed_stride,
                                                              const uint8_t* __restrict__ xy, size_t n,
                                                              int16_t* __restrict__ polys) {
@@ -1557,7 +1565,8 @@ __global__ void __launch_bounds__(128) derive_uniform_kernel(const uint8_t* __re
     for (int w = 0; w < 4; w++) dst[32 * w + lane] = rows[p * kRowWords + 32 * w + lane];
   }
 }
-// (*Poly).DeriveNoise (sample.go:31-95) for n independent (seed, nonce): the noise branch of sample_kernel
+// (*Poly).DeriveNoise (sample.go:31-95) for n independent (seed, nonce), thread per polynomial (the K-PKE kernels
+// sample theirs per octet, octet_prf)
 template <int ETA>
 __global__ void __launch_bounds__(128) derive_noise_kernel(const uint8_t* __restrict__ seeds, size_t seed_stride,
                                                            const uint8_t* __restrict__ nonces, size_t n,
