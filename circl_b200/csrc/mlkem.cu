@@ -9,10 +9,11 @@
 //     DeriveNoise2                    common/sample.go:67-95 (SHAKE256 PRF + CBD_2)
 //     CompressTo                      common/poly.go:248-328
 //
-// Pipeline (all intermediates stay on the device; sub-batches are sized so that
-// A^T lives in the 50 MB L2 between kernels):
+// Pipeline (all intermediates stay on the device; sub-batches of kSub ops alternate between two streams, and A^T is
+// the only intermediate of a sub-batch in memory -- 36 MiB at 8192 ops, K = 3):
 //   1. hash_kernel    one thread per op/key: h = SHA3-256(ek), (K', r) = SHA3-512(m || h)
-//   2. sample_kernel  one thread per Keccak stream: K*K SHAKE128 matrix streams per key
+//   2. sample_kernel  one thread per Keccak stream: K*K SHAKE128 matrix streams per key, staged a block at a time
+//                     and written by each warp itself (uniform_block)
 //   3. encrypt_dp_kernel one octet (8 lanes) per op: the 2K+1 SHAKE256 noise streams (lane p: nonces p, p + 8),
 //                     NTT(r), A^T o r, t o r, InvNTT, +e, compress
 #include <stdlib.h>
@@ -107,9 +108,9 @@ __global__ void __launch_bounds__(128) g_kernel(const uint8_t* __restrict__ m, c
 // ------------------------------------------------------------------ 2. samplers
 // 12-bit rejection sampling of one 168-byte SHAKE128 block (sample.go:203-233): 112 candidates, field f at bit 12 f
 // of the block (d1 = low, d2 = high 12 bits of each 3-byte group, in that order).  `wp` is the 32-bit shared-memory
-// address of the next free int16 of this thread's row: every candidate is stored there (clamped to the slack entry
-// behind the row once 256 are in) and only the advance is predicated -- per candidate a shift/mask pair, a min, a
-// compare, one STS and one predicated add, all on 32-bit registers.  Returns the new address (>= end when full).
+// address of the next free int16 of this thread's staging: every candidate is stored there (clamped to `end`, the
+// entry of coefficient 256, once 256 are in) and only the advance is predicated -- per candidate a shift/mask pair, a
+// min, a compare, one STS and one predicated add, all on 32-bit registers.  Returns the new address (>= end when full).
 template <bool CHECKED>
 __device__ __forceinline__ uint32_t reject_block(const uint64_t (&a)[25], uint32_t wp, uint32_t end) {
 #pragma unroll
@@ -123,7 +124,7 @@ __device__ __forceinline__ uint32_t reject_block(const uint64_t (&a)[25], uint32
       const uint32_t hi = (uint32_t)(a[(wi + 1) >> 1] >> (32 * ((wi + 1) & 1)));
       d = __funnelshift_r(lo, hi, sh) & 0xfff;
     }
-    // the first two blocks hold 224 candidates: they cannot run past the 256-entry row, so only later blocks clamp
+    // the first two blocks hold 224 candidates: they cannot run past coefficient 256, so only later blocks clamp
     asm volatile("st.shared.u16 [%0], %1;" ::"r"(CHECKED ? min(wp, end) : wp), "h"((uint16_t)d) : "memory");
     wp += (d < (uint32_t)Q) ? 2u : 0u;
   }
@@ -147,10 +148,17 @@ __device__ __forceinline__ void cbd2_store(const uint64_t (&a)[25], int16_t* __r
 // sub-batches in flight fit the 50 MB L2 and two of 8192 do not; 8192 still measured faster (ML-KEM-768, 2^20 per-op
 // keys, H100 80GB HBM3 SXM at 700 W: 19.9 ms per step against 20.9 at 4096), as it halves the launches and the tail
 // waves, sample_fix_kernel's most of all (1.8 against 3.5 ms per step).  With the noise still in memory (8 KiB / op)
-// 4096 had been the faster (H100 SXM at 400 W: 24.7 ms per step at 4096, 25.5 at 8192, 30.0 at 2048).
+// 4096 had been the faster (H100 SXM at 400 W: 24.7 ms per step at 4096, 25.5 at 8192, 30.0 at 2048).  Per sub-batch
+// of 8192 ops (K = 3) sample_kernel runs 576 CTAs on 792 resident slots (6 per SM) and encrypt_dp_kernel 1024 on 924.
 constexpr size_t kSub = 8192;
-constexpr int kRowWords = 129;  // 256 int16 + 2 slack, odd word stride
-constexpr int kSampleSmem = 128 * kRowWords * 4;
+// The matrix sampler's staging (uniform_block): per thread 15 chunks of 8 int16 -- up to 7 coefficients carried from
+// the last block, the 112 candidates of this one and the clamp slot -- 240 B, so 30,720 B per 128-thread CTA and
+// registers, not shared memory, set its residency: 80 per thread, 6 CTAs per SM (it had been 3, by a 66,048-byte row
+// per CTA; at 72 registers ptxas spills).
+constexpr int kStageChunks = 15;
+constexpr int kSampleThreads = 128;
+constexpr int kSampleMinBlocks = 6;
+constexpr int kSampleSmem = kSampleThreads * kStageChunks * 16;
 
 // CBD_3 of 192 bytes (sample.go:31-62): 6-byte windows, 8 coefficients each; w = 24 squeezed words
 __device__ __forceinline__ void cbd3_store(const uint64_t (&w)[24], int16_t* __restrict__ dst) {
@@ -181,39 +189,66 @@ __device__ __forceinline__ void cbd3_store(const uint64_t (&w)[24], int16_t* __r
   }
 }
 
-// One SHAKE128 stream of DeriveUniform (sample.go:192-236): `a` holds the absorbed, padded first block; the 256 accepted
-// coefficients land in this thread's shared-memory row (256 int16 + slack, kRowWords words).
-__device__ __forceinline__ void uniform_stream(uint64_t (&a)[25], uint32_t* row_words) {
-  int16_t* row = reinterpret_cast<int16_t*>(row_words);
-  uint32_t wp = smem_u32(row);
-  const uint32_t wend = wp + 2 * N;
-#pragma unroll 1
-  for (int b = 0; b < 2; b++) {
-    keccak::f1600(a);
-    wp = reject_block<false>(a, wp, wend);
-  }
-  do {
-    keccak::f1600(a);
-    wp = reject_block<true>(a, wp, wend);
-  } while (wp < wend);
-}
-// The same with exactly three blocks -- what 99 % of the streams need (SURVEY.md 8(a)) -- so that all lanes of a warp and
-// all warps of a CTA finish together; returns the number of coefficients accepted.  A stream that is short of 256 is
-// handed, with its sponge state, to sample_fix_kernel: a warp no longer squeezes a fourth block for all 32 lanes
-// because one of them needs it (27 % of the warps did), and no CTA waits at its barrier for such a warp.
-__device__ __forceinline__ int uniform_stream3(uint64_t (&a)[25], uint32_t* row_words) {
-  int16_t* row = reinterpret_cast<int16_t*>(row_words);
-  const uint32_t w0 = smem_u32(row);
-  uint32_t wp = w0;
-  const uint32_t wend = wp + 2 * N;
-#pragma unroll 1
-  for (int b = 0; b < 2; b++) {
-    keccak::f1600(a);
-    wp = reject_block<false>(a, wp, wend);
-  }
+// One SHAKE128 block of the 32 streams of a warp (sample.go:203-233), warp-collective.  `wst` is the warp's staging
+// (32 x kStageChunks chunks of 16 B, lane l's at l * kStageChunks); this lane's polynomial is the 32 chunks from
+// out[poly]; `cnt` is the number of coefficients it holds so far.  Returns the new count, clamped to 256 (CHECKED; the
+// first two blocks hold at most 224 candidates and need no clamp).  Staging entry e stands for coefficient base + e,
+// base = cnt rounded down to a multiple of 8, so the entries [0, cnt - base) are the ones carried over from the last
+// block and every chunk of the staging is a 16-byte chunk of the polynomial:
+//   1. permute; parse the 112 candidates into the thread's staging from entry cnt - base on (reject_block);
+//   2. the warp writes the chunks [base / 8, ceil(cnt' / 8)) of every stream (at most 15), two streams per pass --
+//      lanes 0-15 stream 2q, lanes 16-31 stream 2q + 1 -- with one 16-byte load and store per lane: 16 passes of one
+//      shuffle (the stream's first chunk and chunk count, packed), unpacking, a compare, LDS.128 and STG.128;
+//   3. the thread moves its last, partial chunk to the front of its staging for the next block.
+// A partial chunk is written with whatever follows the last coefficient in the staging and rewritten whole by the
+// next block's pass (or, for a stream sample_kernel hands off, from position cnt' on by sample_fix_kernel).
+// Threads past the end of the batch (`live` false) take part and write nothing.  poly must stay below 2^23 - 1, so
+// that (32 poly + 32) << 4 fits the 32-bit job word.
+template <bool CHECKED>
+__device__ __forceinline__ uint32_t uniform_block(uint64_t (&a)[25], uint4* wst, int lane, uint4* __restrict__ out,
+                                                  uint32_t poly, uint32_t cnt, bool live) {
   keccak::f1600(a);
-  wp = reject_block<true>(a, wp, wend);
-  return (int)((min(wp, wend) - w0) >> 1);
+  uint4* own = wst + lane * kStageChunks;
+  const uint32_t base = cnt & ~7u, s0 = smem_u32(own), end = s0 + 2 * (N - base);
+  const uint32_t wp = reject_block<CHECKED>(a, s0 + 2 * (cnt - base), end);
+  cnt = base + ((min(wp, end) - s0) >> 1);
+  // first chunk to write << 4 | chunk count (<= 15)
+  const uint32_t job = live ? ((32 * poly + base / 8) << 4) | ((cnt - base + 7) >> 3) : 0;
+  __syncwarp();
+  const int half = lane >> 4, c = lane & 15;
+  const uint4* rd = wst + half * kStageChunks + c;
+#pragma unroll 4
+  for (int q = 0; q < 16; q++) {
+    const uint32_t jp = __shfl_sync(0xffffffffu, job, 2 * q + half);
+    if (c < (int)(jp & 15)) out[(jp >> 4) + c] = rd[2 * q * kStageChunks];
+  }
+  __syncwarp();
+  if (cnt < N) own[0] = own[(cnt - base) >> 3];
+  return cnt;
+}
+
+// One SHAKE128 stream of DeriveUniform (sample.go:192-236) per lane of a warp: `a` holds the absorbed, padded first
+// block; the 256 accepted coefficients go to out[poly] (uniform_block).  The warp squeezes blocks until all its streams
+// are full.
+__device__ __forceinline__ void uniform_stream(uint64_t (&a)[25], uint4* wst, int lane, uint4* out, uint32_t poly,
+                                               bool live) {
+  uint32_t cnt = 0;
+#pragma unroll 1
+  for (int b = 0; b < 2; b++) cnt = uniform_block<false>(a, wst, lane, out, poly, cnt, live);
+  do {
+    cnt = uniform_block<true>(a, wst, lane, out, poly, cnt, live);
+  } while (__any_sync(0xffffffffu, cnt < N));
+}
+// The same with exactly three blocks -- what 99 % of the streams need (SURVEY.md 8(a)) -- so that all lanes of a warp
+// finish together; returns the number of coefficients accepted, the first that many of which are in the polynomial.
+// A stream that is short of 256 is handed, with its sponge state, to sample_fix_kernel: a warp no longer squeezes a
+// fourth block for all 32 lanes because one of them needs it (27 % of the warps did).
+__device__ __forceinline__ uint32_t uniform_stream3(uint64_t (&a)[25], uint4* wst, int lane, uint4* out, uint32_t poly,
+                                                    bool live) {
+  uint32_t cnt = 0;
+#pragma unroll 1
+  for (int b = 0; b < 2; b++) cnt = uniform_block<false>(a, wst, lane, out, poly, cnt, live);
+  return uniform_block<true>(a, wst, lane, out, poly, cnt, live);
 }
 struct Pending {  // one unfinished SHAKE128 stream
   uint32_t stream, count;
@@ -243,18 +278,19 @@ __device__ __forceinline__ void noise_stream(uint64_t (&a)[25], int16_t* __restr
 // One thread per matrix stream, s = (i*K + j) * nkeys + key -> A^T[key][i][j] = XOF(rho, i, j).  (The noise is made
 // by the K-PKE kernels themselves, octet_prf.)
 template <int K>
-__global__ void __launch_bounds__(128) sample_kernel(const uint8_t* __restrict__ rho0, size_t ek_stride, size_t nkeys,
-                                                     int16_t* __restrict__ A, int transpose, FixList* __restrict__ fix) {
+__global__ void __launch_bounds__(kSampleThreads, kSampleMinBlocks) sample_kernel(const uint8_t* __restrict__ rho0, size_t ek_stride,
+                                                                size_t nkeys, int16_t* __restrict__ A, int transpose,
+                                                                FixList* __restrict__ fix) {
   // rho0 + key*ek_stride is rho of that key; transpose = 1 derives A^T (encryption), 0 derives A (key
   // generation, mat.go:13-29)
+  // Each warp stages its 32 streams a block at a time and writes them to A itself (uniform_block): no CTA barrier.
+  extern __shared__ __align__(16) uint4 stage[];
+  const int lane = threadIdx.x & 31, wbase = threadIdx.x & ~31;
+  const size_t s = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t total = nkeys * K * K;
+  if (s - lane >= total) return;  // a warp with no stream of the batch
   uint64_t a[25];
   keccak::zero(a);
-  // Each thread rejection-samples into its own shared-memory row (129-word stride: conflict-free
-  // while the counters of a warp agree); the CTA then streams the rows out as whole 512-byte polynomials.
-  extern __shared__ __align__(16) uint32_t rows[];
-  const size_t s0 = (size_t)blockIdx.x * blockDim.x;
-  const size_t s = s0 + threadIdx.x;
-  const size_t total = nkeys * K * K;
   const bool live = s < total;
   const size_t sc = live ? s : total - 1;
   const size_t key = sc % nkeys;
@@ -265,25 +301,15 @@ __global__ void __launch_bounds__(128) sample_kernel(const uint8_t* __restrict__
   // m[i][j] = XOF(rho, x, y) with (x, y) = (i, j) if transpose else (j, i)
   a[4] = (uint64_t)(transpose ? i : j) | ((uint64_t)(transpose ? j : i) << 8) | (0x1full << 16);
   a[20] = 0x8000000000000000ull;                               // rate 168
-  const int got = uniform_stream3(a, rows + threadIdx.x * kRowWords);
+  const uint32_t got = uniform_stream3(a, stage + wbase * kStageChunks, lane, reinterpret_cast<uint4*>(A),
+                                       (uint32_t)(key * K * K + ij), live);
   if (live && got < N) {  // ~1 % of the streams: finished by sample_fix_kernel from this state
     Pending* list = reinterpret_cast<Pending*>(fix + 1);
     Pending& e = list[atomicAdd(&fix->n, 1u)];
     e.stream = (uint32_t)s;
-    e.count = (uint32_t)got;
+    e.count = got;
 #pragma unroll
     for (int w = 0; w < 25; w++) e.a[w] = a[w];
-  }
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int p = warp; p < (int)blockDim.x; p += blockDim.x / 32) {
-    const size_t sp = s0 + p;
-    if (sp >= total) break;
-    const size_t pkey = sp % nkeys;
-    const int pij = (int)(sp / nkeys);
-    uint32_t* dst = reinterpret_cast<uint32_t*>(A + (pkey * K * K + pij) * N);
-#pragma unroll
-    for (int w = 0; w < 4; w++) dst[32 * w + lane] = rows[p * kRowWords + 32 * w + lane];
   }
 }
 
@@ -395,14 +421,15 @@ template <int K>
 static int launch_sample(int slot, int lane, cudaStream_t ls, const uint8_t* rho0, size_t ek_stride, size_t nkeys,
                          int16_t* A, int transpose) {
   if (nkeys == 0) return 0;
+  static_assert(kSub * 16 < (1u << 23) - 1, "uniform_block: polynomial index too large");  // nkeys <= kSub
   if (int arc = ensure_smem_attr((const void*)sample_kernel<K>, kSampleSmem)) return arc;
   const size_t streams = nkeys * K * K;
   void* fix = nullptr;
   if (int frc = ensure_fix(slot, lane, sizeof(FixList) + streams * sizeof(Pending), ls, &fix)) return frc;
   {
     KernelScope ks(KID_MLKEM_SAMPLE, ls);
-    sample_kernel<K><<<(unsigned)((streams + 127) / 128), 128, kSampleSmem, ls>>>(rho0, ek_stride, nkeys, A, transpose,
-                                                                                 (FixList*)fix);
+    sample_kernel<K><<<(unsigned)((streams + kSampleThreads - 1) / kSampleThreads), kSampleThreads, kSampleSmem, ls>>>(
+        rho0, ek_stride, nkeys, A, transpose, (FixList*)fix);
   }
   {
     KernelScope ks(KID_MLKEM_SAMPLE_FIX, ls);
@@ -1538,11 +1565,14 @@ static int encaps_any(int k, const uint8_t* ek, size_t ek_stride, const uint8_t*
 
 // ------------------------------------------------------------------ 7. the sampler and serialisation surface on its own
 // (*Poly).DeriveUniform (sample.go:192-236) for n independent (seed, x, y): the stream of sample_kernel
-__global__ void __launch_bounds__(128) derive_uniform_kernel(const uint8_t* __restrict__ seeds, size_t seed_stride,
-                                                             const uint8_t* __restrict__ xy, size_t n,
-                                                             int16_t* __restrict__ polys) {
-  extern __shared__ __align__(16) uint32_t rows[];
-  const size_t s0 = (size_t)blockIdx.x * blockDim.x, s = s0 + threadIdx.x, sc = s < n ? s : n - 1;
+__global__ void __launch_bounds__(kSampleThreads) derive_uniform_kernel(const uint8_t* __restrict__ seeds,
+                                                                        size_t seed_stride,
+                                                                        const uint8_t* __restrict__ xy, size_t n,
+                                                                        int16_t* __restrict__ polys) {
+  extern __shared__ __align__(16) uint4 stage[];
+  const int lane = threadIdx.x & 31, wbase = threadIdx.x & ~31;
+  const size_t s = (size_t)blockIdx.x * blockDim.x + threadIdx.x, sc = s < n ? s : n - 1;
+  if (s - lane >= n) return;  // a warp with no stream of the batch
   const uint8_t* seed = seeds + sc * seed_stride;
   uint64_t a[25];
   keccak::zero(a);
@@ -1555,15 +1585,9 @@ __global__ void __launch_bounds__(128) derive_uniform_kernel(const uint8_t* __re
   }
   a[4] = (uint64_t)xy[2 * sc] | ((uint64_t)xy[2 * sc + 1] << 8) | (0x1full << 16);
   a[20] = 0x8000000000000000ull;
-  uniform_stream(a, rows + threadIdx.x * kRowWords);
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int p = warp; p < (int)blockDim.x; p += blockDim.x / 32) {
-    if (s0 + p >= n) break;
-    uint32_t* dst = reinterpret_cast<uint32_t*>(polys + (s0 + p) * N);
-#pragma unroll
-    for (int w = 0; w < 4; w++) dst[32 * w + lane] = rows[p * kRowWords + 32 * w + lane];
-  }
+  // polynomials relative to the warp's first, so the chunk indices stay small whatever n is
+  uniform_stream(a, stage + wbase * kStageChunks, lane, reinterpret_cast<uint4*>(polys + (s - lane) * N),
+                 (uint32_t)(sc - (s - lane)), s < n);
 }
 // (*Poly).DeriveNoise (sample.go:31-95) for n independent (seed, nonce), thread per polynomial (the K-PKE kernels
 // sample theirs per octet, octet_prf)
@@ -1661,7 +1685,8 @@ int launch_derive_uniform(const uint8_t* seeds, size_t seed_stride, const uint8_
                           cudaStream_t st) {
   if (int arc = ensure_smem_attr((const void*)derive_uniform_kernel, kSampleSmem)) return arc;
   KernelScope ks(KID_SAMPLER, st);
-  derive_uniform_kernel<<<(unsigned)((n + 127) / 128), 128, kSampleSmem, st>>>(seeds, seed_stride, xy, n, polys);
+  derive_uniform_kernel<<<(unsigned)((n + kSampleThreads - 1) / kSampleThreads), kSampleThreads, kSampleSmem, st>>>(
+      seeds, seed_stride, xy, n, polys);
   CB200_CUDA(cudaGetLastError());
   return 0;
 }
