@@ -96,6 +96,21 @@ SYMBOLS = {
     "cb200_hpke_shared_key_size": (C.c_size_t, [C.c_int]),
     "cb200_hpke_seed_size": (C.c_size_t, [C.c_int]),
     "cb200_hpke_encapsulation_seed_size": (C.c_size_t, [C.c_int]),
+    "cb200_p256": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p256_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p256_encaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_size_t]),
+    "cb200_hpke_p256_decaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p256_auth_encaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p256_auth_decaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                              C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p256_public_key_size": (C.c_size_t, []),
+    "cb200_hpke_p256_private_key_size": (C.c_size_t, []),
+    "cb200_hpke_p256_ciphertext_size": (C.c_size_t, []),
+    "cb200_hpke_p256_shared_key_size": (C.c_size_t, []),
+    "cb200_hpke_p256_seed_size": (C.c_size_t, []),
+    "cb200_hpke_p256_encapsulation_seed_size": (C.c_size_t, []),
     "cb200_frodo640shake_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_frodo640shake_encaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_frodo640shake_decaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]),

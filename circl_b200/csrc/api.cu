@@ -60,7 +60,7 @@ static const char* kKernelNames[KID_COUNT] = {
     "dil_ntt", "dil_invntt", "dil_dot", "dil_elementwise",
     "mldsa_expand_key", "mldsa_mu_rhoprime", "mldsa_mask", "mldsa_w", "mldsa_challenge", "mldsa_response",
     "mldsa_compact", "x25519", "hybrid_glue", "keccak_f1600", "sampler", "mlkem_sample_fix", "x448", "ed25519", "ed448",
-    "hpke", "frodo", "frodo_gemm"};
+    "hpke", "frodo", "frodo_gemm", "p256"};
 const char* kernel_name(int id) { return (id >= 0 && id < KID_COUNT) ? kKernelNames[id] : "?"; }
 
 KernelScope::KernelScope(int id_, cudaStream_t st_) : st(st_), id(id_) {
@@ -318,6 +318,7 @@ static void dev_destroy(Dev& d) {
   if (d.dil_tw) cudaFree(d.dil_tw);
   if (d.x25519_table) cudaFree(d.x25519_table);
   if (d.ed448_table) cudaFree(d.ed448_table);
+  if (d.p256_table) cudaFree(d.p256_table);
 }
 static Dev* dev_by_ordinal(int device) {
   for (auto& d : rt().devs)

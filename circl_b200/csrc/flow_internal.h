@@ -282,5 +282,10 @@ void x25519_rows(const uint8_t* k, size_t k_stride, const uint8_t* p, size_t p_s
                  uint8_t* status, size_t n, cudaStream_t st);
 void x448_rows(const uint8_t* k, size_t k_stride, const uint8_t* p, size_t p_stride, uint8_t* out, size_t out_stride,
                uint8_t* status, size_t n, cudaStream_t st);
+// The same for P-256 (p256.cu p256_base_kernel / p256_kernel, timed under KID_P256): scalars of 32 bytes, points and
+// KeyGen outputs of 65 (0x04 || X || Y), Shared outputs of 32 (X), all big-endian and at any byte.  status[i] |= 1
+// where p[i] is not a valid public key and |= 2 where k[i] is not a valid private key; that op's output is all zero.
+void p256_rows(const uint8_t* k, size_t k_stride, const uint8_t* p, size_t p_stride, uint8_t* out, size_t out_stride,
+               uint8_t* status, size_t n, cudaStream_t st);
 }  // namespace hybrid
 }  // namespace cb200

@@ -62,33 +62,45 @@ def _run(call, status):
 
 
 class DHKEM:
-    """One of the two DHKEMs; the sizes follow from the id (xkem.go:20-24, kembase.go:34)."""
+    """One of the two DHKEMs; the sizes follow from the id (xkem.go:20-24, kembase.go:34).  A subclass with other
+    key sizes (_nsk, _npk), its own entry points (_c), key class (_Priv) and errors (_run) is circl_b200.p256's."""
+
+    _Priv = PrivateKey
 
     def __init__(self, name: str, ident: int, n: int, nss: int):
         self._name, self._id, self._n, self._nss = name, ident, n, nss
+        self._nsk = self._npk = n
 
     def Name(self) -> str: return self._name
-    def PublicKeySize(self): return self._n
-    def PrivateKeySize(self): return self._n
-    def CiphertextSize(self): return self._n
-    def SeedSize(self): return self._n
-    def EncapsulationSeedSize(self): return self._n
+    def PublicKeySize(self): return self._npk
+    def PrivateKeySize(self): return self._nsk
+    def CiphertextSize(self): return self._npk
+    def SeedSize(self): return self._nsk
+    def EncapsulationSeedSize(self): return self._nsk
     def SharedKeySize(self): return self._nss
+
+    def _c(self, name, *args):
+        """cb200_hpke_<name>(id, args...)"""
+        return getattr(lib(), "cb200_hpke_" + name)(self._id, *args)
+
+    @staticmethod
+    def _run(call, status):
+        _run(call, status)
 
     # ---------------------------------------------------------------- single operations
     def UnmarshalBinaryPublicKey(self, buf: bytes) -> PublicKey:
-        if len(buf) != self._n:
+        if len(buf) != self._npk:
             raise ErrPubKeySize("kem: invalid public key size")
         return PublicKey(self, buf)
 
     def UnmarshalBinaryPrivateKey(self, buf: bytes) -> PrivateKey:
-        if len(buf) != self._n:
+        if len(buf) != self._nsk:
             raise ErrPrivKeySize("kem: invalid private key size")
-        return PrivateKey(self, buf)
+        return self._Priv(self, buf)
 
     def GenerateKeyPair(self):
         """A random private key, as the reference draws it (xkem.go:73-80)."""
-        sk = PrivateKey(self, os.urandom(self._n))
+        sk = self._Priv(self, os.urandom(self._nsk))
         return sk.Public(), sk
 
     # Argument checks in the reference's order: the seed (DeriveKeyPair of the ephemeral key) or the encapsulation
@@ -96,10 +108,10 @@ class DHKEM:
     def DeriveKeyPair(self, seed: bytes):
         self._seed(seed)  # the reference panics with kem.ErrSeedSize
         pk, sk = self.DeriveKeyPairBatch(self._row(seed))
-        return PublicKey(self, pk[0].tobytes()), PrivateKey(self, sk[0].tobytes())
+        return PublicKey(self, pk[0].tobytes()), self._Priv(self, sk[0].tobytes())
 
     def Encapsulate(self, pk: PublicKey):
-        return self.EncapsulateDeterministically(pk, os.urandom(self._n))
+        return self.EncapsulateDeterministically(pk, os.urandom(self._nsk))
 
     def EncapsulateDeterministically(self, pk: PublicKey, seed: bytes):
         self._seed(seed)
@@ -113,7 +125,7 @@ class DHKEM:
         return self.DecapsulateBatch(sk, self._row(ct))[0].tobytes()
 
     def AuthEncapsulate(self, pkr: PublicKey, sks: PrivateKey):
-        return self.AuthEncapsulateDeterministically(pkr, sks, os.urandom(self._n))
+        return self.AuthEncapsulateDeterministically(pkr, sks, os.urandom(self._nsk))
 
     def AuthEncapsulateDeterministically(self, pkr: PublicKey, sks: PrivateKey, seed: bytes):
         self._seed(seed)
@@ -131,10 +143,10 @@ class DHKEM:
     # ---------------------------------------------------------------- batches
     def DeriveKeyPairBatch(self, seeds):
         """(n, N) seeds -> (pk (n, N), sk (n, N))."""
-        s = _prep(seeds, self._n, ErrSeedSize("kem: invalid seed size"))
+        s = _prep(seeds, self._nsk, ErrSeedSize("kem: invalid seed size"))
         n = s.shape[0]
-        pk, sk = _new(s, (n, self._n)), _new(s, (n, self._n))
-        check(lib().cb200_hpke_keygen(self._id, _ptr(s), _ptr(pk), _ptr(sk), n))
+        pk, sk = _new(s, (n, self._npk)), _new(s, (n, self._nsk))
+        check(self._c("keygen", _ptr(s), _ptr(pk), _ptr(sk), n))
         return pk, sk
 
     def EncapsulateBatch(self, pks, seeds):
@@ -153,30 +165,29 @@ class DHKEM:
         return self._decaps(skrs, encs, pkss)
 
     def _encaps(self, pkrs, skss, seeds):
-        es = _prep(seeds, self._n, ErrSeedSize("kem: invalid seed size"))
+        es = _prep(seeds, self._nsk, ErrSeedSize("kem: invalid seed size"))
         n = es.shape[0]
         pk, pks = self._keys(pkrs, PublicKey, n, es, ErrPubKeySize("kem: invalid public key size"))
-        enc, ss, status = _new(es, (n, self._n)), _new(es, (n, self._nss)), _zeros(es, (n,))
+        enc, ss, status = _new(es, (n, self._npk)), _new(es, (n, self._nss)), _zeros(es, (n,))
         if skss is None:
-            _run(lambda: lib().cb200_hpke_encaps(self._id, _ptr(pk), pks, _ptr(es), _ptr(enc), _ptr(ss), _ptr(status), n),
-                 status)
+            self._run(lambda: self._c("encaps", _ptr(pk), pks, _ptr(es), _ptr(enc), _ptr(ss), _ptr(status), n), status)
         else:
             sk, sks = self._keys(skss, PrivateKey, n, es, ErrPrivKeySize("kem: invalid private key size"))
-            _run(lambda: lib().cb200_hpke_auth_encaps(self._id, _ptr(pk), pks, _ptr(sk), sks, _ptr(es), _ptr(enc),
-                                                      _ptr(ss), _ptr(status), n), status)
+            self._run(lambda: self._c("auth_encaps", _ptr(pk), pks, _ptr(sk), sks, _ptr(es), _ptr(enc), _ptr(ss),
+                                      _ptr(status), n), status)
         return enc, ss
 
     def _decaps(self, skrs, encs, pkss):
-        c = _prep(encs, self._n, ErrPubKeySize("kem: invalid public key size"))
+        c = _prep(encs, self._npk, ErrPubKeySize("kem: invalid public key size"))
         n = c.shape[0]
         sk, sks = self._keys(skrs, PrivateKey, n, c, ErrPrivKeySize("kem: invalid private key size"))
         ss, status = _new(c, (n, self._nss)), _zeros(c, (n,))
         if pkss is None:
-            _run(lambda: lib().cb200_hpke_decaps(self._id, _ptr(sk), sks, _ptr(c), _ptr(ss), _ptr(status), n), status)
+            self._run(lambda: self._c("decaps", _ptr(sk), sks, _ptr(c), _ptr(ss), _ptr(status), n), status)
         else:
             pk, pks = self._keys(pkss, PublicKey, n, c, ErrPubKeySize("kem: invalid public key size"))
-            _run(lambda: lib().cb200_hpke_auth_decaps(self._id, _ptr(sk), sks, _ptr(c), _ptr(pk), pks, _ptr(ss),
-                                                      _ptr(status), n), status)
+            self._run(lambda: self._c("auth_decaps", _ptr(sk), sks, _ptr(c), _ptr(pk), pks, _ptr(ss), _ptr(status), n),
+                      status)
         return ss
 
     # ---------------------------------------------------------------- helpers
@@ -185,7 +196,7 @@ class DHKEM:
             raise ErrTypeMismatch("kem: type mismatch")
 
     def _seed(self, seed):
-        if len(seed) != self._n:
+        if len(seed) != self._nsk:
             raise ErrSeedSize("kem: invalid seed size")
 
     @staticmethod
@@ -202,10 +213,11 @@ class DHKEM:
                 import torch
                 arr = torch.from_numpy(arr.copy()).to(like.device)
             return arr, 0
-        arr = _prep(keys, self._n, err)
+        width = self._npk if cls is PublicKey else self._nsk
+        arr = _prep(keys, width, err)
         if arr.shape[0] != n:
             raise err
-        return arr, self._n
+        return arr, width
 
 
 _SCHEMES = {"hpke_kem_x25519_hkdf_sha256": DHKEM("HPKE_KEM_X25519_HKDF_SHA256", 0x20, 32, 32),

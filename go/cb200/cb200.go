@@ -690,6 +690,80 @@ func HPKEDecaps(id int, skR, enc, pkS, ss []byte, ok []bool) error {
 	return err
 }
 
+// DHKEM(P-256, HKDF-SHA256), kem_id 0x10 (hpke/shortkem.go; include/circl_b200.h cb200_hpke_p256_*): sk and seeds 32
+// bytes, pk and enc 65 (0x04 || X || Y), ss 32.  The generic HPKE* functions above do not take this id.
+const (
+	HPKEP256HKDFSHA256     = 0x10
+	HPKEP256PrivateKeySize = 32
+	HPKEP256PublicKeySize  = 65
+	HPKEP256SharedKeySize  = 32
+)
+
+// HPKEP256Keygen: batched DeriveKeyPair (shortkem.go:63-90) on n seeds of 32 bytes; pk: n*65, sk: n*32.
+func HPKEP256Keygen(seeds, pk, sk []byte) error {
+	n := len(seeds) / HPKEP256PrivateKeySize
+	if len(seeds) != n*HPKEP256PrivateKeySize || len(pk) != n*HPKEP256PublicKeySize || len(sk) != n*HPKEP256PrivateKeySize {
+		panic("cb200: HPKEP256Keygen buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return call(func() C.int { return C.cb200_hpke_p256_keygen(u8(seeds), u8(pk), u8(sk), C.size_t(n)) })
+}
+
+// HPKEP256Encaps: batched Encap, or AuthEncap when skS is not nil.  pkR (65 bytes) and skS (32): one key or n keys
+// each; seeds: n*32; enc: n*65; ss: n*32.  After the whole batch ran, ErrPrivKey (hpke.ErrInvalidKEMPrivateKey for the
+// caller) is returned if any skS is not in [1, n - 1], else ErrPubKey (hpke.ErrInvalidKEMPublicKey) if any pkR is not
+// a P-256 point; ok[i] (may be nil) tells which operations failed.
+func HPKEP256Encaps(pkR, skS, seeds, enc, ss []byte, ok []bool) error {
+	n := len(seeds) / HPKEP256PrivateKeySize
+	if len(seeds) != n*HPKEP256PrivateKeySize || len(enc) != n*HPKEP256PublicKeySize || len(ss) != n*HPKEP256SharedKeySize ||
+		(ok != nil && len(ok) != n) {
+		panic("cb200: HPKEP256Encaps buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	pr, prs := hpkeKey(pkR, n, HPKEP256PublicKeySize, "HPKEP256Encaps")
+	status := make([]byte, n)
+	err := call(func() C.int {
+		if skS == nil {
+			return C.cb200_hpke_p256_encaps(pr, prs, u8(seeds), u8(enc), u8(ss), u8(status), C.size_t(n))
+		}
+		sp, sps := hpkeKey(skS, n, HPKEP256PrivateKeySize, "HPKEP256Encaps")
+		return C.cb200_hpke_p256_auth_encaps(pr, prs, sp, sps, u8(seeds), u8(enc), u8(ss), u8(status), C.size_t(n))
+	})
+	for i := range ok {
+		ok[i] = status[i] == 0
+	}
+	return err
+}
+
+// HPKEP256Decaps: batched Decap, or AuthDecap when pkS is not nil.  skR (32 bytes) and pkS (65): one key or n keys
+// each; enc: n*65; ss: n*32.  Errors as HPKEP256Encaps (an invalid skR is ErrPrivKey, an invalid enc or pkS ErrPubKey).
+func HPKEP256Decaps(skR, enc, pkS, ss []byte, ok []bool) error {
+	n := len(enc) / HPKEP256PublicKeySize
+	if len(enc) != n*HPKEP256PublicKeySize || len(ss) != n*HPKEP256SharedKeySize || (ok != nil && len(ok) != n) {
+		panic("cb200: HPKEP256Decaps buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	sr, srs := hpkeKey(skR, n, HPKEP256PrivateKeySize, "HPKEP256Decaps")
+	status := make([]byte, n)
+	err := call(func() C.int {
+		if pkS == nil {
+			return C.cb200_hpke_p256_decaps(sr, srs, u8(enc), u8(ss), u8(status), C.size_t(n))
+		}
+		pp, pps := hpkeKey(pkS, n, HPKEP256PublicKeySize, "HPKEP256Decaps")
+		return C.cb200_hpke_p256_auth_decaps(sr, srs, u8(enc), pp, pps, u8(ss), u8(status), C.size_t(n))
+	})
+	for i := range ok {
+		ok[i] = status[i] == 0
+	}
+	return err
+}
+
 // FrodoKEM-640-SHAKE sizes (kem/frodo/frodo640shake/frodo.go:32-51).
 const (
 	Frodo640SHAKEPublicKeySize         = 9616

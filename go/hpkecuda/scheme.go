@@ -1,7 +1,7 @@
 //go:build cuda && cgo
 
-// Package hpkecuda backs the kem/schemes entries "HPKE_KEM_X25519_HKDF_SHA256" and "HPKE_KEM_X448_HKDF_SHA512"
-// (hpke/algs.go:248-277) with the cb200 engine.  Both are kem.AuthScheme (kem/kem.go:84-90): DeriveKeyPair, the
+// Package hpkecuda backs the kem/schemes entries "HPKE_KEM_X25519_HKDF_SHA256", "HPKE_KEM_X448_HKDF_SHA512" and
+// "HPKE_KEM_P256_HKDF_SHA256" (hpke/algs.go:248-277) with the cb200 engine.  Both are kem.AuthScheme (kem/kem.go:84-90): DeriveKeyPair, the
 // (authenticated) encapsulations and decapsulations run on the GPU as batches of one, everything else (key parsing,
 // GenerateKeyPair, marshalling) delegates to CIRCL's own scheme.  EncapsulateBatch and DecapsulateBatch are the entry
 // points that make a GPU worthwhile.
@@ -20,18 +20,40 @@ import (
 )
 
 type scheme struct {
-	kem.AuthScheme // CIRCL's DHKEM (hpke/xkem.go)
+	kem.AuthScheme // CIRCL's DHKEM (hpke/xkem.go, hpke/shortkem.go)
 	id             int
 }
 
 var (
 	x25519 = &scheme{hpke.KEM_X25519_HKDF_SHA256.Scheme().(kem.AuthScheme), cb200.HPKEX25519HKDFSHA256}
 	x448   = &scheme{hpke.KEM_X448_HKDF_SHA512.Scheme().(kem.AuthScheme), cb200.HPKEX448HKDFSHA512}
+	p256   = &scheme{hpke.KEM_P256_HKDF_SHA256.Scheme().(kem.AuthScheme), cb200.HPKEP256HKDFSHA256}
 )
 
-// X25519 and X448 return the GPU-backed schemes; Name() is unchanged so kem/schemes.ByName keeps working.
+// X25519, X448 and P256 return the GPU-backed schemes; Name() is unchanged so kem/schemes.ByName keeps working.
 func X25519() kem.AuthScheme { return x25519 }
 func X448() kem.AuthScheme   { return x448 }
+func P256() kem.AuthScheme   { return p256 }
+
+// The engine calls of a scheme: P-256 has entry points of its own.
+func (s *scheme) keygen(seeds, pk, sk []byte) error {
+	if s.id == cb200.HPKEP256HKDFSHA256 {
+		return cb200.HPKEP256Keygen(seeds, pk, sk)
+	}
+	return cb200.HPKEKeygen(s.id, seeds, pk, sk)
+}
+func (s *scheme) encaps(pkR, skS, seeds, enc, ss []byte, ok []bool) error {
+	if s.id == cb200.HPKEP256HKDFSHA256 {
+		return s.mapErr(cb200.HPKEP256Encaps(pkR, skS, seeds, enc, ss, ok))
+	}
+	return s.mapErr(cb200.HPKEEncaps(s.id, pkR, skS, seeds, enc, ss, ok))
+}
+func (s *scheme) decaps(skR, enc, pkS, ss []byte, ok []bool) error {
+	if s.id == cb200.HPKEP256HKDFSHA256 {
+		return s.mapErr(cb200.HPKEP256Decaps(skR, enc, pkS, ss, ok))
+	}
+	return s.mapErr(cb200.HPKEDecaps(s.id, skR, enc, pkS, ss, ok))
+}
 
 func mustMarshal(k interface{ MarshalBinary() ([]byte, error) }) []byte {
 	b, err := k.MarshalBinary()
@@ -41,9 +63,16 @@ func mustMarshal(k interface{ MarshalBinary() ([]byte, error) }) []byte {
 	return b
 }
 
-// mapErr maps the engine's per-batch failure to hpke.ErrInvalidKEMSharedSecret (hpke/hpke.go:280)
-func mapErr(err error) error {
-	if err == cb200.ErrPubKey {
+// mapErr maps the engine's per-batch failures to the reference's errors: for X25519 / X448 a low-order point is
+// hpke.ErrInvalidKEMSharedSecret (hpke/hpke.go:280); for P-256 an invalid point or scalar is
+// hpke.ErrInvalidKEMPublicKey / ErrInvalidKEMPrivateKey (hpke/hpke.go:278-279)
+func (s *scheme) mapErr(err error) error {
+	switch {
+	case err == cb200.ErrPubKey && s.id == cb200.HPKEP256HKDFSHA256:
+		return hpke.ErrInvalidKEMPublicKey
+	case err == cb200.ErrPrivKey && s.id == cb200.HPKEP256HKDFSHA256:
+		return hpke.ErrInvalidKEMPrivateKey
+	case err == cb200.ErrPubKey:
 		return hpke.ErrInvalidKEMSharedSecret
 	}
 	return err
@@ -68,7 +97,7 @@ func (s *scheme) DeriveKeyPair(seed []byte) (kem.PublicKey, kem.PrivateKey) {
 		panic(kem.ErrSeedSize) // xkem.go:60-62
 	}
 	pk, sk := make([]byte, s.PublicKeySize()), make([]byte, s.PrivateKeySize())
-	if err := cb200.HPKEKeygen(s.id, seed, pk, sk); err != nil {
+	if err := s.keygen(seed, pk, sk); err != nil {
 		panic(err)
 	}
 	pub, err := s.UnmarshalBinaryPublicKey(pk)
@@ -91,7 +120,7 @@ func (s *scheme) encap(pkr kem.PublicKey, sks kem.PrivateKey, seed []byte) (ct, 
 		skS = s.checkPriv(sks)
 	}
 	ct, ss = make([]byte, s.CiphertextSize()), make([]byte, s.SharedKeySize())
-	if err = mapErr(cb200.HPKEEncaps(s.id, s.checkPub(pkr), skS, seed, ct, ss, nil)); err != nil {
+	if err = s.encaps(s.checkPub(pkr), skS, seed, ct, ss, nil); err != nil {
 		return nil, nil, err
 	}
 	return ct, ss, nil
@@ -101,12 +130,17 @@ func (s *scheme) decap(skr kem.PrivateKey, ct []byte, pks kem.PublicKey) ([]byte
 	if len(ct) != s.PublicKeySize() {
 		return nil, kem.ErrPubKeySize // ct is parsed as a public key (kembase.go:222, xkem.go:95-101)
 	}
+	if s.id == cb200.HPKEP256HKDFSHA256 { // shortkem.go:115-130 also checks the point
+		if _, err := s.AuthScheme.UnmarshalBinaryPublicKey(ct); err != nil {
+			return nil, err
+		}
+	}
 	var pkS []byte
 	if pks != nil {
 		pkS = s.checkPub(pks)
 	}
 	ss := make([]byte, s.SharedKeySize())
-	if err := mapErr(cb200.HPKEDecaps(s.id, s.checkPriv(skr), ct, pkS, ss, nil)); err != nil {
+	if err := s.decaps(s.checkPriv(skr), ct, pkS, ss, nil); err != nil {
 		return nil, err
 	}
 	return ss, nil
@@ -150,7 +184,7 @@ func EncapsulateBatch(s kem.AuthScheme, pkR, skS, seeds []byte, ok []bool) (enc,
 	g := s.(*scheme)
 	n := len(seeds) / g.SeedSize()
 	enc, ss = make([]byte, n*g.CiphertextSize()), make([]byte, n*g.SharedKeySize())
-	return enc, ss, mapErr(cb200.HPKEEncaps(g.id, pkR, skS, seeds, enc, ss, ok))
+	return enc, ss, g.encaps(pkR, skS, seeds, enc, ss, ok)
 }
 
 // DecapsulateBatch decapsulates len(enc)/N encapsulations with one packed skR (its public key is computed once: the
@@ -158,5 +192,5 @@ func EncapsulateBatch(s kem.AuthScheme, pkR, skS, seeds []byte, ok []bool) (enc,
 func DecapsulateBatch(s kem.AuthScheme, skR, enc, pkS []byte, ok []bool) ([]byte, error) {
 	g := s.(*scheme)
 	ss := make([]byte, len(enc)/g.CiphertextSize()*g.SharedKeySize())
-	return ss, mapErr(cb200.HPKEDecaps(g.id, skR, enc, pkS, ss, ok))
+	return ss, g.decaps(skR, enc, pkS, ss, ok)
 }

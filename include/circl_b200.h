@@ -292,6 +292,45 @@ size_t cb200_hpke_shared_key_size(int id);
 size_t cb200_hpke_seed_size(int id);
 size_t cb200_hpke_encapsulation_seed_size(int id);
 
+/* ---- P-256 ECDH (Go's crypto/ecdh.P256(), as the reference's hpke/shortkem.go uses it) ----
+ * cb200_p256: KeyGen (points == NULL: out = 0x04 || X || Y of [k]G, 65-byte rows) or Shared (out = X of [k]P, 32-byte
+ * rows) on n 32-byte big-endian scalars and 65-byte uncompressed points.  A scalar must satisfy 0 < k < n
+ * (ecdh.NewPrivateKey), a point must be 0x04 || X || Y with X, Y < p on the curve (ecdh.NewPublicKey).
+ * status (optional): bit 0 = invalid point, bit 1 = invalid scalar; a failed op's output row is all zero.  A
+ * host-pointer call finishes the batch and returns CB200_ERR_PRIVKEY if any scalar failed, else CB200_ERR_PUBKEY if any
+ * point failed.  Device pointers may start at any byte. */
+int cb200_p256(const uint8_t *scalars, const uint8_t *points, uint8_t *out, uint8_t *status, size_t n);
+
+/* ---- HPKE DHKEM(P-256, HKDF-SHA256), kem_id 0x10 (hpke/shortkem.go, hpke/kembase.go; hpke/algs.go:248-253) ----
+ * The cb200_hpke_* contracts above without the id; the generic entry points keep treating 0x10 as unknown.
+ * Sizes: seed, encapsulation seed and sk 32 (a big-endian scalar), pk and enc 65 (0x04 || X || Y), ss 32.
+ * keygen = DeriveKeyPair (shortkem.go:63-90): the first candidate LabeledExpand(dkp_prk, "candidate", I2OSP(ctr, 1), 32),
+ *   ctr = 0..255, that lies in [1, n - 1].
+ * kem_context is enc || pkR (130 bytes) or enc || pkR || pkS (195); the auth dh is dh1 || dh2 (64).
+ * status bit 0 = hpke.ErrInvalidKEMPublicKey (pkR, enc or pkS is not a P-256 point), bit 1 =
+ *   hpke.ErrInvalidKEMPrivateKey (skR or skS is not in [1, n - 1]); that op's ss is all zero and its enc is still
+ *   written.  A key shared by the batch (stride 0) that fails marks every op.  A host-pointer call finishes the batch,
+ *   then returns CB200_ERR_PRIVKEY if any op has bit 1, else CB200_ERR_PUBKEY if any has bit 0; a device-pointer call
+ *   reports only through status, which it requires.
+ * Strides: 0 = one key for the whole batch.  65-byte rows cannot all be aligned, so device pointers and strides may
+ * start at any byte. */
+#define CB200_HPKE_P256_HKDF_SHA256 0x10
+int cb200_hpke_p256_keygen(const uint8_t *seeds, uint8_t *pk, uint8_t *sk, size_t n);
+int cb200_hpke_p256_encaps(const uint8_t *pkR, size_t pkR_stride, const uint8_t *seeds, uint8_t *enc, uint8_t *ss,
+                           uint8_t *status, size_t n);
+int cb200_hpke_p256_decaps(const uint8_t *skR, size_t skR_stride, const uint8_t *enc, uint8_t *ss, uint8_t *status,
+                           size_t n);
+int cb200_hpke_p256_auth_encaps(const uint8_t *pkR, size_t pkR_stride, const uint8_t *skS, size_t skS_stride,
+                                const uint8_t *seeds, uint8_t *enc, uint8_t *ss, uint8_t *status, size_t n);
+int cb200_hpke_p256_auth_decaps(const uint8_t *skR, size_t skR_stride, const uint8_t *enc, const uint8_t *pkS,
+                                size_t pkS_stride, uint8_t *ss, uint8_t *status, size_t n);
+size_t cb200_hpke_p256_public_key_size(void);             /* 65 */
+size_t cb200_hpke_p256_private_key_size(void);            /* 32 */
+size_t cb200_hpke_p256_ciphertext_size(void);             /* 65 */
+size_t cb200_hpke_p256_shared_key_size(void);             /* 32 */
+size_t cb200_hpke_p256_seed_size(void);                   /* 32 */
+size_t cb200_hpke_p256_encapsulation_seed_size(void);     /* 32 */
+
 /* ---- FrodoKEM-640-SHAKE (kem/frodo/frodo640shake), the only parameter set the reference has ----
  * Sizes: pk 9616, sk 19888, ct 9720, ss 16, seed 48 (s || seedSE || z), encapsulation seed 16 (mu).
  * keygen = DeriveKeyPair (frodo.go:84-135); encaps = EncapsulateDeterministically (:160-240); decaps = Decapsulate

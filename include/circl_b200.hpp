@@ -63,6 +63,9 @@ struct ErrPubKey : Error { ErrPubKey() : Error("kem: invalid public key") {} };
 struct ErrPrivKey : Error { ErrPrivKey() : Error("kem: invalid private key") {} };
 // hpke.ErrInvalidKEMSharedSecret (hpke/hpke.go:280): a DH step of an HPKE DHKEM met a low-order point
 struct ErrInvalidKEMSharedSecret : Error { ErrInvalidKEMSharedSecret() : Error("hpke: invalid KEM shared secret") {} };
+// hpke.ErrInvalidKEMPublicKey / ErrInvalidKEMPrivateKey (hpke/hpke.go:278-279): DHKEM(P-256) keys that crypto/ecdh rejects
+struct ErrInvalidKEMPublicKey : Error { ErrInvalidKEMPublicKey() : Error("hpke: invalid KEM public key") {} };
+struct ErrInvalidKEMPrivateKey : Error { ErrInvalidKEMPrivateKey() : Error("hpke: invalid KEM private key") {} };
 
 class Scheme;
 
@@ -107,32 +110,32 @@ class Scheme {
   Scheme(std::string name, Kind kind, int id) : name_(std::move(name)), kind_(kind), k_(id) {}
   const std::string& Name() const { return name_; }
   size_t CiphertextSize() const {
-    if (kind_ == HPKE) return cb200_hpke_ciphertext_size(k_);
+    if (kind_ == HPKE) return p256() ? cb200_hpke_p256_ciphertext_size() : cb200_hpke_ciphertext_size(k_);
     if (kind_ == FRODO) return cb200_frodo640shake_ciphertext_size();
     return kind_ == XWING ? 1120 : kind_ == HYBRID ? cb200_hybrid_ciphertext_size(k_) : cb200_mlkem_ciphertext_size(k_);
   }
   size_t SharedKeySize() const {
-    if (kind_ == HPKE) return cb200_hpke_shared_key_size(k_);
+    if (kind_ == HPKE) return p256() ? cb200_hpke_p256_shared_key_size() : cb200_hpke_shared_key_size(k_);
     if (kind_ == FRODO) return cb200_frodo640shake_shared_key_size();
     return kind_ == HYBRID ? cb200_hybrid_shared_key_size(k_) : 32;
   }
   size_t PrivateKeySize() const {
-    if (kind_ == HPKE) return cb200_hpke_private_key_size(k_);
+    if (kind_ == HPKE) return p256() ? cb200_hpke_p256_private_key_size() : cb200_hpke_private_key_size(k_);
     if (kind_ == FRODO) return cb200_frodo640shake_private_key_size();
     return kind_ == XWING ? 32 : kind_ == HYBRID ? cb200_hybrid_private_key_size(k_) : cb200_mlkem_private_key_size(k_);
   }
   size_t PublicKeySize() const {
-    if (kind_ == HPKE) return cb200_hpke_public_key_size(k_);
+    if (kind_ == HPKE) return p256() ? cb200_hpke_p256_public_key_size() : cb200_hpke_public_key_size(k_);
     if (kind_ == FRODO) return cb200_frodo640shake_public_key_size();
     return kind_ == XWING ? 1216 : kind_ == HYBRID ? cb200_hybrid_public_key_size(k_) : cb200_mlkem_public_key_size(k_);
   }
   size_t SeedSize() const {
-    if (kind_ == HPKE) return cb200_hpke_seed_size(k_);
+    if (kind_ == HPKE) return p256() ? cb200_hpke_p256_seed_size() : cb200_hpke_seed_size(k_);
     if (kind_ == FRODO) return cb200_frodo640shake_seed_size();
     return kind_ == XWING ? 32 : kind_ == HYBRID ? cb200_hybrid_seed_size(k_) : 64;
   }
   size_t EncapsulationSeedSize() const {
-    if (kind_ == HPKE) return cb200_hpke_encapsulation_seed_size(k_);
+    if (kind_ == HPKE) return p256() ? cb200_hpke_p256_encapsulation_seed_size() : cb200_hpke_encapsulation_seed_size(k_);
     if (kind_ == FRODO) return cb200_frodo640shake_encapsulation_seed_size();
     return kind_ == XWING ? 64 : kind_ == HYBRID ? cb200_hybrid_encapsulation_seed_size(k_) : 32;
   }
@@ -155,6 +158,7 @@ class Scheme {
   }
   PrivateKey UnmarshalBinaryPrivateKey(const Bytes& buf) const {  // kyber.go:398-407
     if (buf.size() != PrivateKeySize()) throw ErrPrivKeySize();
+    if (p256() && !p256_scalar_ok(buf)) throw ErrInvalidKEMPrivateKey();  // shortkem.go:103-113
     return PrivateKey(this, buf);
   }
   // (ct, ss)
@@ -199,7 +203,10 @@ class Scheme {
       case KYBER3: check(cb200_kyber_kem_encaps(k_, eks.data(), stride, seeds.data(), cts.data(), sss.data(), n)); break;
       case XWING: check(cb200_xwing_encaps(eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)); break;
       case HYBRID: check(cb200_hybrid_encaps(k_, eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)); break;
-      case HPKE: check(cb200_hpke_encaps(k_, eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)); break;
+      case HPKE:
+        check(p256() ? cb200_hpke_p256_encaps(eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)
+                     : cb200_hpke_encaps(k_, eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n));
+        break;
       case FRODO: check(cb200_frodo640shake_encaps(eks.data(), stride, seeds.data(), cts.data(), sss.data(), n)); break;
     }
   }
@@ -225,7 +232,10 @@ class Scheme {
         }
         break;
       }
-      case HPKE: check(cb200_hpke_decaps(k_, dks.data(), stride, cts.data(), sss.data(), nullptr, n)); break;
+      case HPKE:
+        check(p256() ? cb200_hpke_p256_decaps(dks.data(), stride, cts.data(), sss.data(), nullptr, n)
+                     : cb200_hpke_decaps(k_, dks.data(), stride, cts.data(), sss.data(), nullptr, n));
+        break;
       case FRODO: check(cb200_frodo640shake_decaps(dks.data(), stride, cts.data(), sss.data(), n)); break;
     }
   }
@@ -242,7 +252,10 @@ class Scheme {
         dks = seeds;
         break;
       case HYBRID: check(cb200_hybrid_keygen(k_, seeds.data(), eks.data(), dks.data(), n)); break;
-      case HPKE: check(cb200_hpke_keygen(k_, seeds.data(), eks.data(), dks.data(), n)); break;
+      case HPKE:
+        check(p256() ? cb200_hpke_p256_keygen(seeds.data(), eks.data(), dks.data(), n)
+                     : cb200_hpke_keygen(k_, seeds.data(), eks.data(), dks.data(), n));
+        break;
       case FRODO: check(cb200_frodo640shake_keygen(seeds.data(), eks.data(), dks.data(), n)); break;
     }
   }
@@ -276,19 +289,28 @@ class Scheme {
     const size_t ps = key_stride(pkrs, n, PublicKeySize(), ErrPubKeySize()), ss = key_stride(skss, n, PrivateKeySize(), ErrPrivKeySize());
     cts.resize(n * CiphertextSize());
     sss.resize(n * SharedKeySize());
-    check(cb200_hpke_auth_encaps(k_, pkrs.data(), ps, skss.data(), ss, seeds.data(), cts.data(), sss.data(), nullptr, n));
+    check(p256() ? cb200_hpke_p256_auth_encaps(pkrs.data(), ps, skss.data(), ss, seeds.data(), cts.data(), sss.data(), nullptr, n)
+                 : cb200_hpke_auth_encaps(k_, pkrs.data(), ps, skss.data(), ss, seeds.data(), cts.data(), sss.data(), nullptr, n));
   }
   void AuthDecapsulateBatch(const Bytes& skrs, const Bytes& cts, const Bytes& pkss, Bytes& sss) const {
     auth_only();
     const size_t n = rows(cts, CiphertextSize(), ErrPubKeySize());
     const size_t ss = key_stride(skrs, n, PrivateKeySize(), ErrPrivKeySize()), ps = key_stride(pkss, n, PublicKeySize(), ErrPubKeySize());
     sss.resize(n * SharedKeySize());
-    check(cb200_hpke_auth_decaps(k_, skrs.data(), ss, cts.data(), pkss.data(), ps, sss.data(), nullptr, n));
+    check(p256() ? cb200_hpke_p256_auth_decaps(skrs.data(), ss, cts.data(), pkss.data(), ps, sss.data(), nullptr, n)
+                 : cb200_hpke_auth_decaps(k_, skrs.data(), ss, cts.data(), pkss.data(), ps, sss.data(), nullptr, n));
   }
   int k() const { return k_; }
   Kind kind() const { return kind_; }
+  // DHKEM(P-256, HKDF-SHA256): an HPKE scheme on the cb200_hpke_p256_* entry points (kem::p256::All())
+  bool p256() const { return kind_ == HPKE && k_ == CB200_HPKE_P256_HKDF_SHA256; }
 
  private:
+  static bool p256_scalar_ok(const Bytes& k) {  // 0 < k < n, big-endian (crypto/ecdh NewPrivateKey)
+    static const uint8_t n[32] = {0xff, 0xff, 0xff, 0xff, 0x00, 0x00, 0x00, 0x00, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
+                                  0xbc, 0xe6, 0xfa, 0xad, 0xa7, 0x17, 0x9e, 0x84, 0xf3, 0xb9, 0xca, 0xc2, 0xfc, 0x63, 0x25, 0x51};
+    return std::any_of(k.begin(), k.end(), [](uint8_t b) { return b != 0; }) && std::lexicographical_compare(k.begin(), k.end(), n, n + 32);
+  }
   void auth_only() const {
     if (kind_ != HPKE) throw std::logic_error("kem: " + name_ + " is not a kem.AuthScheme");
   }
@@ -305,6 +327,8 @@ class Scheme {
   }
   void check(int rc) const {
     if (rc == 0) return;
+    if (rc == CB200_ERR_PUBKEY && p256()) throw ErrInvalidKEMPublicKey();
+    if (rc == CB200_ERR_PRIVKEY && p256()) throw ErrInvalidKEMPrivateKey();
     if (rc == CB200_ERR_PUBKEY && kind_ == HPKE) throw ErrInvalidKEMSharedSecret();
     if (rc == CB200_ERR_PUBKEY) throw ErrPubKey();
     if (rc == CB200_ERR_PRIVKEY) throw ErrPrivKey();
@@ -318,9 +342,9 @@ class Scheme {
 
 inline PublicKey PrivateKey::Public() const {
   const Scheme* s = scheme_;
-  if (s->kind() == Scheme::HPKE) {  // KeyGen of the stored (unclamped) key (xkem.go:146-163)
+  if (s->kind() == Scheme::HPKE) {  // KeyGen of the stored (unclamped) key (xkem.go:146-163, shortkem.go:151-157)
     Bytes pk(s->PublicKeySize());
-    if ((pk.size() == 56 ? cb200_x448 : cb200_x25519)(packed_.data(), nullptr, pk.data(), nullptr, 1))
+    if ((s->p256() ? cb200_p256 : pk.size() == 56 ? cb200_x448 : cb200_x25519)(packed_.data(), nullptr, pk.data(), nullptr, 1))
       throw Error(cb200_last_error());
     return PublicKey(s, std::move(pk));
   }
@@ -348,7 +372,7 @@ inline PublicKey PrivateKey::Public() const {
 }
 
 inline std::pair<PublicKey, PrivateKey> Scheme::GenerateKeyPair() const {
-  if (kind_ != HPKE) return GenerateFromSeed();
+  if (kind_ != HPKE || p256()) return GenerateFromSeed();  // P-256: a uniform key in [1, n - 1] from DeriveKeyPair
   Bytes sk(PrivateKeySize());
   fill_random(sk.data(), sk.size());
   PrivateKey priv(this, std::move(sk));
@@ -391,6 +415,22 @@ inline const Scheme* ByName(const std::string& name) {  // case-insensitive; nul
   return nullptr;
 }
 }  // namespace hpke
+
+// DHKEM(P-256, HKDF-SHA256) (kem/schemes/schemes.go, HPKE_KEM_P256_HKDF_SHA256), registered on its own so that
+// hpke::All() keeps its two Montgomery-curve schemes.  UnmarshalBinaryPrivateKey checks the scalar range; a public key
+// or encapsulation that is not a P-256 point is reported by the call that uses it (ErrInvalidKEMPublicKey).
+namespace p256 {
+inline const std::vector<const Scheme*>& All() {
+  static const Scheme s("HPKE_KEM_P256_HKDF_SHA256", Scheme::HPKE, CB200_HPKE_P256_HKDF_SHA256);
+  static const std::vector<const Scheme*> all = {&s};
+  return all;
+}
+inline const Scheme* ByName(const std::string& name) {  // case-insensitive; nullptr = no such scheme
+  for (const Scheme* s : All())
+    if (lower(s->Name()) == lower(name)) return s;
+  return nullptr;
+}
+}  // namespace p256
 
 // FrodoKEM-640-SHAKE (kem/schemes/schemes.go entry 6), registered on its own like the HPKE DHKEMs.
 namespace frodo {
