@@ -111,6 +111,36 @@ SYMBOLS = {
     "cb200_hpke_p256_shared_key_size": (C.c_size_t, []),
     "cb200_hpke_p256_seed_size": (C.c_size_t, []),
     "cb200_hpke_p256_encapsulation_seed_size": (C.c_size_t, []),
+    "cb200_p384": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p384_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p384_encaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_size_t]),
+    "cb200_hpke_p384_decaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p384_auth_encaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p384_auth_decaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                              C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p384_public_key_size": (C.c_size_t, []),
+    "cb200_hpke_p384_private_key_size": (C.c_size_t, []),
+    "cb200_hpke_p384_ciphertext_size": (C.c_size_t, []),
+    "cb200_hpke_p384_shared_key_size": (C.c_size_t, []),
+    "cb200_hpke_p384_seed_size": (C.c_size_t, []),
+    "cb200_hpke_p384_encapsulation_seed_size": (C.c_size_t, []),
+    "cb200_p521": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p521_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p521_encaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_size_t]),
+    "cb200_hpke_p521_decaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p521_auth_encaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p521_auth_decaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                              C.c_void_p, C.c_size_t]),
+    "cb200_hpke_p521_public_key_size": (C.c_size_t, []),
+    "cb200_hpke_p521_private_key_size": (C.c_size_t, []),
+    "cb200_hpke_p521_ciphertext_size": (C.c_size_t, []),
+    "cb200_hpke_p521_shared_key_size": (C.c_size_t, []),
+    "cb200_hpke_p521_seed_size": (C.c_size_t, []),
+    "cb200_hpke_p521_encapsulation_seed_size": (C.c_size_t, []),
     "cb200_frodo640shake_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_frodo640shake_encaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_frodo640shake_decaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]),

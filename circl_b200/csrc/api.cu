@@ -60,7 +60,7 @@ static const char* kKernelNames[KID_COUNT] = {
     "dil_ntt", "dil_invntt", "dil_dot", "dil_elementwise",
     "mldsa_expand_key", "mldsa_mu_rhoprime", "mldsa_mask", "mldsa_w", "mldsa_challenge", "mldsa_response",
     "mldsa_compact", "x25519", "hybrid_glue", "keccak_f1600", "sampler", "mlkem_sample_fix", "x448", "ed25519", "ed448",
-    "hpke", "frodo", "frodo_gemm", "p256"};
+    "hpke", "frodo", "frodo_gemm", "p256", "p384", "p521"};
 const char* kernel_name(int id) { return (id >= 0 && id < KID_COUNT) ? kKernelNames[id] : "?"; }
 
 KernelScope::KernelScope(int id_, cudaStream_t st_) : st(st_), id(id_) {
@@ -319,6 +319,8 @@ static void dev_destroy(Dev& d) {
   if (d.x25519_table) cudaFree(d.x25519_table);
   if (d.ed448_table) cudaFree(d.ed448_table);
   if (d.p256_table) cudaFree(d.p256_table);
+  if (d.p384_table) cudaFree(d.p384_table);
+  if (d.p521_table) cudaFree(d.p521_table);
 }
 static Dev* dev_by_ordinal(int device) {
   for (auto& d : rt().devs)

@@ -61,6 +61,8 @@ struct Dev {
   void* x25519_table = nullptr; // 32 KiB: multiples 1..8 of 256^i B for the fixed-base X25519 KeyGen (x25519.cuh)
   void* ed448_table = nullptr;  // 84 KiB: multiples 1..8 of 256^i G for Ed448's fixed base (ed448.cuh)
   void* p256_table = nullptr;   // 32 KiB: affine multiples 1..8 of 16^i G for P-256's fixed base (p256.cuh)
+  void* p384_table = nullptr;   // 72 KiB: the same for P-384 (p384.cuh)
+  void* p521_table = nullptr;   // 139 KiB: the same for P-521 (p521.cuh)
   // host staging pipeline (owned by the worker thread).  A chunk lives in one of kSlots slots (device images of its
   // buffers + a work set); all input copies go down one stream, all output copies down another, the kernels of a
   // slot down that slot's stream, tied by events: the input copy of chunk c + kSlots waits only for the KERNELS of
@@ -107,7 +109,7 @@ enum KernelId {
   KID_DIL_NTT, KID_DIL_INVNTT, KID_DIL_DOT, KID_DIL_EW,
   KID_MLDSA_EXPAND, KID_MLDSA_MU, KID_MLDSA_MASK, KID_MLDSA_W, KID_MLDSA_CHALLENGE, KID_MLDSA_RESPONSE,
   KID_MLDSA_COMPACT, KID_X25519, KID_HYBRID_GLUE, KID_KECCAK, KID_SAMPLER, KID_MLKEM_SAMPLE_FIX, KID_X448, KID_ED25519, KID_ED448,
-  KID_HPKE, KID_FRODO, KID_FRODO_GEMM, KID_P256, KID_COUNT
+  KID_HPKE, KID_FRODO, KID_FRODO_GEMM, KID_P256, KID_P384, KID_P521, KID_COUNT
 };
 const char* kernel_name(int id);
 

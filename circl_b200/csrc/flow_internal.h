@@ -287,5 +287,11 @@ void x448_rows(const uint8_t* k, size_t k_stride, const uint8_t* p, size_t p_str
 // where p[i] is not a valid public key and |= 2 where k[i] is not a valid private key; that op's output is all zero.
 void p256_rows(const uint8_t* k, size_t k_stride, const uint8_t* p, size_t p_stride, uint8_t* out, size_t out_stride,
                uint8_t* status, size_t n, cudaStream_t st);
+// The same for P-384 (p384_base_kernel / p384_kernel, KID_P384: scalars and Shared outputs of 48 bytes, points and
+// KeyGen outputs of 97) and P-521 (p521_*, KID_P521: 66 and 133 bytes).
+void p384_rows(const uint8_t* k, size_t k_stride, const uint8_t* p, size_t p_stride, uint8_t* out, size_t out_stride,
+               uint8_t* status, size_t n, cudaStream_t st);
+void p521_rows(const uint8_t* k, size_t k_stride, const uint8_t* p, size_t p_stride, uint8_t* out, size_t out_stride,
+               uint8_t* status, size_t n, cudaStream_t st);
 }  // namespace hybrid
 }  // namespace cb200

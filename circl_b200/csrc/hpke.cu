@@ -1,20 +1,24 @@
 // HPKE's DHKEMs (RFC 9180 section 4.1) as the reference's kem/schemes registers them, batched on the device:
 //   hpke/xkem.go:55-71              DeriveKeyPair                  -> hpke_derive_kernel + the X25519 / X448 KeyGen
-//   hpke/shortkem.go:63-90          DeriveKeyPair (candidate loop) -> hpke_derive_kernel<0x10> + the P-256 KeyGen
+//   hpke/shortkem.go:63-90          DeriveKeyPair (candidate loop) -> hpke_derive_kernel<0x10 / 0x11 / 0x12> + the
+//                                                                     P-256 / P-384 / P-521 KeyGen
 //   hpke/kembase.go:120-241         Encap / Decap / AuthEncap / AuthDecap
 //                                   dh = Shared(...)               -> x25519_kernel / x448_kernel (hybrid.cu),
-//                                                                     p256_kernel (p256.cu)
+//                                                                     p256_kernel / p384_kernel / p521_kernel (p256.cu)
 //                                   ss = ExtractAndExpand(dh, ctx) -> hpke_ss_kernel
-//   ids 0x20 DHKEM(X25519, HKDF-SHA256) and 0x21 DHKEM(X448, HKDF-SHA512) (hpke/algs.go:248-277), and 0x10
-//   DHKEM(P-256, HKDF-SHA256) (:248-253), which has entry points of its own (cb200_hpke_p256_*)
-// The curve kernels are reached through hybrid::x25519_rows / x448_rows / p256_rows; this file adds the KDF kernels
-// (sha2.cuh, thread per op, profiling class KID_HPKE) and the flows around them.
+//   ids 0x20 DHKEM(X25519, HKDF-SHA256) and 0x21 DHKEM(X448, HKDF-SHA512) (hpke/algs.go:248-277), and the NIST ones
+//   0x10 DHKEM(P-256, HKDF-SHA256), 0x11 DHKEM(P-384, HKDF-SHA384) and 0x12 DHKEM(P-521, HKDF-SHA512) (:248-262),
+//   which have entry points of their own (cb200_hpke_p256_* / p384_* / p521_*)
+// The curve kernels are reached through hybrid::x25519_rows / x448_rows / p256_rows / p384_rows / p521_rows; this file
+// adds the KDF kernels (sha2.cuh, thread per op, profiling class KID_HPKE) and the flows around them.
 #include <cstring>
 
 #include "../../include/circl_b200.h"
 #include "common.cuh"
 #include "context.h"
 #include "flow_internal.h"
+#include "p384.cuh"
+#include "p521.cuh"
 #include "sha2.cuh"
 
 namespace cb200 {
@@ -22,7 +26,8 @@ namespace hpke {
 
 // kSk = Nsk = seed = encapsulation seed, kPk = Npk = Nenc, kDh = Ndh (xkem.go:20-24, shortkem.go:31-45); the shared
 // secret is one digest (Nh).  kFail: the status bits that zero an op's ss.  kAligned: rows are 4-byte aligned (the
-// 65-byte rows of P-256 are not, so its rows are written byte by byte).
+// 65-, 97- and 133-byte rows of the NIST curves are not, so theirs are written byte by byte).  Curve and kMask0: the
+// curve type of P-384 and P-521 and DeriveKeyPair's bitmask on a candidate's first byte.
 template <int ID>
 struct Kem;
 template <>
@@ -42,6 +47,22 @@ struct Kem<CB200_HPKE_P256_HKDF_SHA256> {
   using S = sha2::Sha256;
   static constexpr int kSk = 32, kPk = 65, kDh = 32, kFail = 3;
   static constexpr bool kAligned = false;
+};
+template <>
+struct Kem<CB200_HPKE_P384_HKDF_SHA384> {
+  using S = sha2::Sha384;
+  using Curve = nistp::P384;
+  static constexpr int kSk = 48, kPk = 97, kDh = 48, kFail = 3;
+  static constexpr bool kAligned = false;
+  static constexpr uint8_t kMask0 = 0xff;
+};
+template <>
+struct Kem<CB200_HPKE_P521_HKDF_SHA512> {
+  using S = sha2::Sha512;
+  using Curve = nistp::P521;
+  static constexpr int kSk = 66, kPk = 133, kDh = 66, kFail = 3;
+  static constexpr bool kAligned = false;
+  static constexpr uint8_t kMask0 = 0x01;
 };
 
 // the first `bytes` bytes of a digest to a row (4-byte aligned unless !ALIGNED)
@@ -120,6 +141,53 @@ __global__ void __launch_bounds__(128) hpke_derive_kernel<CB200_HPKE_P256_HKDF_S
   store_digest<S, false>(sk + i * sk_stride, t, 32, 0u - ok);
 }
 
+// P-384 and P-521 (shortkem.go:63-90): P-256's loop above on candidates of Nsk bytes whose first byte is ANDed with
+// kMask0, range-tested by nistp::candidate.  P-521's 66-byte candidate is T(1) || the first two bytes of T(2), where
+// T(2) = HMAC(prk, T(1) || info || 0x02) with T(1) read from registers.
+template <int ID>
+__device__ __forceinline__ void nist_derive(const uint8_t* __restrict__ seed, uint8_t* __restrict__ sk) {
+  using K = Kem<ID>;
+  using S = typename K::S;
+  using C = typename K::Curve;
+  typename S::W prk[8], ki[8], ko[8], t1[8], t2[8];
+  sha2::labeled_extract<S>(prk, sha2::Labeled{0, 0, ID, "dkp_prk", 7, seed, nullptr, nullptr, K::kSk, 0, 0});
+  sha2::hmac_key<S>(ki, ko, prk);
+  uint32_t k[C::kW];
+  uint32_t ok = 0;
+#pragma unroll 1
+  for (int ctr = 0; ctr < 256; ctr++) {
+    const CandidateMsg m{sha2::Labeled{1, K::kSk, ID, "candidate", 9, nullptr, nullptr, nullptr, 1, 0, 0}, (uint8_t)ctr};
+    sha2::hmac<S>(t1, ki, ko, m.len(), m);
+    if constexpr (K::kSk > S::kDigest) {
+      const sha2::ExpandNext<S, CandidateMsg> m2{t1, m};
+      sha2::hmac<S>(t2, ki, ko, m2.len(), m2);
+    }
+    ok = nistp::candidate<C>(k, [&](int j) {
+      return j < S::kDigest ? sha2::digest_byte<S>(t1, j) : sha2::digest_byte<S>(t2, j - S::kDigest);
+    }, K::kMask0);
+    if (ok) break;
+  }
+  nistp::words_to_be<C>(sk, k, ok);
+}
+template <>
+__global__ void __launch_bounds__(128) hpke_derive_kernel<CB200_HPKE_P384_HKDF_SHA384>(const uint8_t* __restrict__ seeds,
+                                                                                        size_t s_stride,
+                                                                                        uint8_t* __restrict__ sk,
+                                                                                        size_t sk_stride, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  nist_derive<CB200_HPKE_P384_HKDF_SHA384>(seeds + i * s_stride, sk + i * sk_stride);
+}
+template <>
+__global__ void __launch_bounds__(128) hpke_derive_kernel<CB200_HPKE_P521_HKDF_SHA512>(const uint8_t* __restrict__ seeds,
+                                                                                        size_t s_stride,
+                                                                                        uint8_t* __restrict__ sk,
+                                                                                        size_t sk_stride, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  nist_derive<CB200_HPKE_P521_HKDF_SHA512>(seeds + i * s_stride, sk + i * sk_stride);
+}
+
 // ss[i] = LabeledExpand(LabeledExtract("", "eae_prk", dh[i]), "shared_secret", kem_context[i], Nh) (kembase.go:94-118)
 // with dh = ND rows of Npk bytes (d0 [|| d1]) and kem_context = NC rows of Npk bytes (c0 || c1 [|| c2]), each read at
 // its own stride.  An op whose status bit 0 is set (a DH with a low-order point) gets an all-zero ss.
@@ -160,7 +228,8 @@ struct Id {
   size_t dh;  // bytes of one DH result (Ndh)
   size_t ss;  // shared secret bytes (Nh)
 };
-// the ids of cb200_hpke_*; P-256 is reached only through cb200_hpke_p256_*, which use kP256
+// the ids of cb200_hpke_*; the NIST curves are reached only through cb200_hpke_p256_* / p384_* / p521_*, which use
+// kP256 / kP384 / kP521
 static bool id_of(int id, Id* k) {
   switch (id) {
     case CB200_HPKE_X25519_HKDF_SHA256: *k = {id, 32, 32, 32, 32}; return true;
@@ -169,6 +238,17 @@ static bool id_of(int id, Id* k) {
   return false;
 }
 static const Id kP256 = {CB200_HPKE_P256_HKDF_SHA256, 32, 65, 32, 32};
+static const Id kP384 = {CB200_HPKE_P384_HKDF_SHA384, 48, 97, 48, 48};
+static const Id kP521 = {CB200_HPKE_P521_HKDF_SHA512, 66, 133, 66, 64};
+// the NIST curve of a NIST id, else null
+static const char* nist_curve(int id) {
+  switch (id) {
+    case CB200_HPKE_P256_HKDF_SHA256: return "P-256";
+    case CB200_HPKE_P384_HKDF_SHA384: return "P-384";
+    case CB200_HPKE_P521_HKDF_SHA512: return "P-521";
+  }
+  return nullptr;
+}
 // per-op intermediates: skE (Nsk) | dh (2 Ndh) | the recomputed public key (Npk); a shared key's public key sits in
 // row 0
 static size_t work_unit(const Id& k) { return k.sk + 2 * k.dh + k.pk; }
@@ -180,6 +260,10 @@ static int derive(const Id& k, const uint8_t* seeds, size_t ss_, uint8_t* sk, si
       hpke_derive_kernel<CB200_HPKE_X25519_HKDF_SHA256><<<blocks(n, 128), 128, 0, st>>>(seeds, ss_, sk, sks, n);
     else if (k.id == CB200_HPKE_X448_HKDF_SHA512)
       hpke_derive_kernel<CB200_HPKE_X448_HKDF_SHA512><<<blocks(n, 128), 128, 0, st>>>(seeds, ss_, sk, sks, n);
+    else if (k.id == CB200_HPKE_P384_HKDF_SHA384)
+      hpke_derive_kernel<CB200_HPKE_P384_HKDF_SHA384><<<blocks(n, 128), 128, 0, st>>>(seeds, ss_, sk, sks, n);
+    else if (k.id == CB200_HPKE_P521_HKDF_SHA512)
+      hpke_derive_kernel<CB200_HPKE_P521_HKDF_SHA512><<<blocks(n, 128), 128, 0, st>>>(seeds, ss_, sk, sks, n);
     else
       hpke_derive_kernel<CB200_HPKE_P256_HKDF_SHA256><<<blocks(n, 128), 128, 0, st>>>(seeds, ss_, sk, sks, n);
   }
@@ -193,6 +277,10 @@ static void dh(const Id& k, const uint8_t* sk, size_t sks, const uint8_t* p, siz
     hybrid::x25519_rows(sk, sks, p, ps, out, os, status, n, st);
   else if (k.id == CB200_HPKE_X448_HKDF_SHA512)
     hybrid::x448_rows(sk, sks, p, ps, out, os, status, n, st);
+  else if (k.id == CB200_HPKE_P384_HKDF_SHA384)
+    hybrid::p384_rows(sk, sks, p, ps, out, os, status, n, st);
+  else if (k.id == CB200_HPKE_P521_HKDF_SHA512)
+    hybrid::p521_rows(sk, sks, p, ps, out, os, status, n, st);
   else
     hybrid::p256_rows(sk, sks, p, ps, out, os, status, n, st);
 }
@@ -205,6 +293,12 @@ static void ss_launch(int id, const uint8_t* d0, size_t d0s, const uint8_t* d1, 
         <<<blocks(n, 128), 128, 0, st>>>(d0, d0s, d1, d1s, c0, c0s, c1, c1s, c2, c2s, status, ss, n);
   else if (id == CB200_HPKE_X448_HKDF_SHA512)
     hpke_ss_kernel<CB200_HPKE_X448_HKDF_SHA512, ND, NC>
+        <<<blocks(n, 128), 128, 0, st>>>(d0, d0s, d1, d1s, c0, c0s, c1, c1s, c2, c2s, status, ss, n);
+  else if (id == CB200_HPKE_P384_HKDF_SHA384)
+    hpke_ss_kernel<CB200_HPKE_P384_HKDF_SHA384, ND, NC>
+        <<<blocks(n, 128), 128, 0, st>>>(d0, d0s, d1, d1s, c0, c0s, c1, c1s, c2, c2s, status, ss, n);
+  else if (id == CB200_HPKE_P521_HKDF_SHA512)
+    hpke_ss_kernel<CB200_HPKE_P521_HKDF_SHA512, ND, NC>
         <<<blocks(n, 128), 128, 0, st>>>(d0, d0s, d1, d1s, c0, c0s, c1, c1s, c2, c2s, status, ss, n);
   else
     hpke_ss_kernel<CB200_HPKE_P256_HKDF_SHA256, ND, NC>
@@ -270,18 +364,18 @@ static int decaps_dev(const Id& k, const uint8_t* skR, size_t skRs, const uint8_
 }
 
 // Host-pointer calls: failed operations are reported after the whole batch ran.  X25519 / X448: a low-order point
-// (hpke.ErrInvalidKEMSharedSecret).  P-256: bit 1 = an invalid skR / skS (hpke.ErrInvalidKEMPrivateKey) before
+// (hpke.ErrInvalidKEMSharedSecret).  NIST curves: bit 1 = an invalid skR / skS (hpke.ErrInvalidKEMPrivateKey) before
 // bit 0 = an invalid pkR, enc or pkS (hpke.ErrInvalidKEMPublicKey).
 static int status_result(const Id& k, const Counts& c, size_t n, const char* fn) {
-  if (k.id == CB200_HPKE_P256_HKDF_SHA256) {
+  if (const char* curve = nist_curve(k.id)) {
     if (c.bit1) {
       set_error("%s: %zu of %zu operations have a private key outside [1, n - 1] (hpke: invalid KEM private key)", fn,
                 c.bit1, n);
       return CB200_ERR_PRIVKEY;
     }
     if (c.bit0) {
-      set_error("%s: %zu of %zu operations have a public key or encapsulation that is not a P-256 point "
-                "(hpke: invalid KEM public key)", fn, c.bit0, n);
+      set_error("%s: %zu of %zu operations have a public key or encapsulation that is not a %s point "
+                "(hpke: invalid KEM public key)", fn, c.bit0, n, curve);
       return CB200_ERR_PUBKEY;
     }
     return 0;
@@ -292,7 +386,7 @@ static int status_result(const Id& k, const Counts& c, size_t n, const char* fn)
   return CB200_ERR_PUBKEY;
 }
 // Device-pointer calls read and write their rows in 32-bit units; the X25519 entry points ask for 16-byte alignment
-// like cb200_x25519, the X448 ones for 8 like cb200_x448.  P-256 rows are read and written byte by byte.
+// like cb200_x25519, the X448 ones for 8 like cb200_x448.  NIST curve rows are read and written byte by byte.
 static size_t align_of(const Id& k) { return k.pk == 32 ? 16 : k.pk == 56 ? 8 : 1; }
 static const char* align_text(const Id& k) {
   return k.pk == 32 ? "%s: device buffers and strides must be 16-byte aligned"
@@ -443,37 +537,39 @@ int cb200_hpke_auth_decaps(int id, const uint8_t* skR, size_t skR_stride, const 
                       true);
 }
 
-// DHKEM(P-256, HKDF-SHA256)
-size_t cb200_hpke_p256_public_key_size(void) { return kP256.pk; }
-size_t cb200_hpke_p256_private_key_size(void) { return kP256.sk; }
-size_t cb200_hpke_p256_ciphertext_size(void) { return kP256.pk; }
-size_t cb200_hpke_p256_shared_key_size(void) { return kP256.ss; }
-size_t cb200_hpke_p256_seed_size(void) { return kP256.sk; }
-size_t cb200_hpke_p256_encapsulation_seed_size(void) { return kP256.sk; }
-
-int cb200_hpke_p256_keygen(const uint8_t* seeds, uint8_t* pk, uint8_t* sk, size_t n) {
-  return keygen_entry("cb200_hpke_p256_keygen", &kP256, seeds, pk, sk, n);
-}
-
-int cb200_hpke_p256_encaps(const uint8_t* pkR, size_t pkR_stride, const uint8_t* seeds, uint8_t* enc, uint8_t* ss,
-                           uint8_t* status, size_t n) {
-  return encaps_entry("cb200_hpke_p256_encaps", &kP256, pkR, pkR_stride, nullptr, 0, seeds, enc, ss, status, n, false);
-}
-
-int cb200_hpke_p256_decaps(const uint8_t* skR, size_t skR_stride, const uint8_t* enc, uint8_t* ss, uint8_t* status,
-                           size_t n) {
-  return decaps_entry("cb200_hpke_p256_decaps", &kP256, skR, skR_stride, enc, nullptr, 0, ss, status, n, false);
-}
-
-int cb200_hpke_p256_auth_encaps(const uint8_t* pkR, size_t pkR_stride, const uint8_t* skS, size_t skS_stride,
-                                const uint8_t* seeds, uint8_t* enc, uint8_t* ss, uint8_t* status, size_t n) {
-  return encaps_entry("cb200_hpke_p256_auth_encaps", &kP256, pkR, pkR_stride, skS, skS_stride, seeds, enc, ss, status, n,
-                      true);
-}
-
-int cb200_hpke_p256_auth_decaps(const uint8_t* skR, size_t skR_stride, const uint8_t* enc, const uint8_t* pkS,
-                                size_t pkS_stride, uint8_t* ss, uint8_t* status, size_t n) {
-  return decaps_entry("cb200_hpke_p256_auth_decaps", &kP256, skR, skR_stride, enc, pkS, pkS_stride, ss, status, n, true);
-}
+// DHKEM(P-256, HKDF-SHA256), DHKEM(P-384, HKDF-SHA384) and DHKEM(P-521, HKDF-SHA512)
+#define CB200_HPKE_NIST_ENTRIES(c, K)                                                                                  \
+  size_t cb200_hpke_##c##_public_key_size(void) { return K.pk; }                                                       \
+  size_t cb200_hpke_##c##_private_key_size(void) { return K.sk; }                                                      \
+  size_t cb200_hpke_##c##_ciphertext_size(void) { return K.pk; }                                                       \
+  size_t cb200_hpke_##c##_shared_key_size(void) { return K.ss; }                                                       \
+  size_t cb200_hpke_##c##_seed_size(void) { return K.sk; }                                                             \
+  size_t cb200_hpke_##c##_encapsulation_seed_size(void) { return K.sk; }                                               \
+  int cb200_hpke_##c##_keygen(const uint8_t* seeds, uint8_t* pk, uint8_t* sk, size_t n) {                              \
+    return keygen_entry("cb200_hpke_" #c "_keygen", &K, seeds, pk, sk, n);                                             \
+  }                                                                                                                    \
+  int cb200_hpke_##c##_encaps(const uint8_t* pkR, size_t pkR_stride, const uint8_t* seeds, uint8_t* enc, uint8_t* ss,  \
+                              uint8_t* status, size_t n) {                                                             \
+    return encaps_entry("cb200_hpke_" #c "_encaps", &K, pkR, pkR_stride, nullptr, 0, seeds, enc, ss, status, n,        \
+                        false);                                                                                        \
+  }                                                                                                                    \
+  int cb200_hpke_##c##_decaps(const uint8_t* skR, size_t skR_stride, const uint8_t* enc, uint8_t* ss, uint8_t* status, \
+                              size_t n) {                                                                              \
+    return decaps_entry("cb200_hpke_" #c "_decaps", &K, skR, skR_stride, enc, nullptr, 0, ss, status, n, false);       \
+  }                                                                                                                    \
+  int cb200_hpke_##c##_auth_encaps(const uint8_t* pkR, size_t pkR_stride, const uint8_t* skS, size_t skS_stride,       \
+                                   const uint8_t* seeds, uint8_t* enc, uint8_t* ss, uint8_t* status, size_t n) {       \
+    return encaps_entry("cb200_hpke_" #c "_auth_encaps", &K, pkR, pkR_stride, skS, skS_stride, seeds, enc, ss, status, \
+                        n, true);                                                                                      \
+  }                                                                                                                    \
+  int cb200_hpke_##c##_auth_decaps(const uint8_t* skR, size_t skR_stride, const uint8_t* enc, const uint8_t* pkS,      \
+                                   size_t pkS_stride, uint8_t* ss, uint8_t* status, size_t n) {                        \
+    return decaps_entry("cb200_hpke_" #c "_auth_decaps", &K, skR, skR_stride, enc, pkS, pkS_stride, ss, status, n,     \
+                        true);                                                                                         \
+  }
+CB200_HPKE_NIST_ENTRIES(p256, kP256)
+CB200_HPKE_NIST_ENTRIES(p384, kP384)
+CB200_HPKE_NIST_ENTRIES(p521, kP521)
+#undef CB200_HPKE_NIST_ENTRIES
 
 }  // extern "C"

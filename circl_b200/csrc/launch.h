@@ -30,5 +30,5 @@ void dil_fill_twiddles(uint32_t* out);
 struct Dev;
 int init_extra_tables(Dev& d);
 int init_ed448_table(Dev& d);  // ed448.cu
-int init_p256_table(Dev& d);   // p256.cu
+int init_nistp_tables(Dev& d);  // p256.cu: P-256, P-384 and P-521
 }  // namespace cb200

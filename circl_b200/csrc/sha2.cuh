@@ -1,5 +1,6 @@
-// SHA-256 (FIPS 180-4), and HMAC (RFC 2104) and HPKE's labeled HKDF (RFC 9180 section 4) over SHA-256 and SHA-512,
-// one message per thread.  SHA-512's compression function is ed25519.cuh's.
+// SHA-256 (FIPS 180-4), and HMAC (RFC 2104) and HPKE's labeled HKDF (RFC 9180 section 4) over SHA-256, SHA-384 and
+// SHA-512, one message per thread.  SHA-512's compression function is ed25519.cuh's; SHA-384 is the same compression
+// from its own initial value, with the digest cut to six words.
 //
 // The HPKE KEMs hash short messages of fixed, public lengths whose bytes come from a few places: constant labels,
 // rows in memory and values held in registers.  A message is therefore a functor msg(j) returning byte j; the block
@@ -82,9 +83,9 @@ CB200_XHD void sha256_block(uint32_t (&H)[8], uint32_t (&W)[16]) {
   H[7] += h;
 }
 
-// The two hashes behind one interface.  W: state and message word; a digest is 8 words, big-endian within each word.
-// ipad0 / opad0: the state after the first block of HMAC with the all-zero key (any zero key up to a block long),
-// i.e. the compression of 0x36... / 0x5c... from the initial value.
+// The three hashes behind one interface.  W: state and message word; the state is 8 words and a digest its first
+// kDigest bytes, big-endian within each word.  ipad0 / opad0: the state after the first block of HMAC with the
+// all-zero key (any zero key up to a block long), i.e. the compression of 0x36... / 0x5c... from the initial value.
 struct Sha256 {
   using W = uint32_t;
   static constexpr int kBlock = 64, kWordBytes = 4, kDigest = 32;
@@ -119,6 +120,23 @@ struct Sha512 {
   }
   CB200_XHD static void compress(W (&H)[8], W (&M)[16]) { ed25519::sha512_block(H, M); }
 };
+struct Sha384 {
+  using W = uint64_t;
+  static constexpr int kBlock = 128, kWordBytes = 8, kDigest = 48;
+  CB200_XHD static void iv(W (&H)[8]) {
+    H[0] = 0xcbbb9d5dc1059ed8ull, H[1] = 0x629a292a367cd507ull, H[2] = 0x9159015a3070dd17ull, H[3] = 0x152fecd8f70e5939ull;
+    H[4] = 0x67332667ffc00b31ull, H[5] = 0x8eb44a8768581511ull, H[6] = 0xdb0c2e0d64f98fa7ull, H[7] = 0x47b5481dbefa4fa4ull;
+  }
+  CB200_XHD static void ipad0(W (&H)[8]) {
+    H[0] = 0x53f869327560c3a2ull, H[1] = 0xc237b05164a5bbe8ull, H[2] = 0xe581f7394cfa66b8ull, H[3] = 0x846fa61922faad62ull;
+    H[4] = 0xdd0b37ce462cff5eull, H[5] = 0x7ee8a4bdc87567f3ull, H[6] = 0x39bda99c75a047f7ull, H[7] = 0xc7bd628bd3f9a734ull;
+  }
+  CB200_XHD static void opad0(W (&H)[8]) {
+    H[0] = 0xff6ce3f9ca86c81cull, H[1] = 0x585559c2ae0fc15cull, H[2] = 0xcf0d5686fb65a54eull, H[3] = 0xf1d54ee19e8cfd02ull;
+    H[4] = 0xa5c720ab778ff100ull, H[5] = 0xdeb3e5f667573e8cull, H[6] = 0xc1bfc7ec16b591f3ull, H[7] = 0x34d487c1c79d59ebull;
+  }
+  CB200_XHD static void compress(W (&H)[8], W (&M)[16]) { ed25519::sha512_block(H, M); }
+};
 
 // Hashes msg(0 .. len) with FIPS 180-4 padding into H, which already holds `done` bytes (a whole number of blocks).
 // Message lengths stay below 2^32 bits, so the length field is its last word alone.
@@ -150,18 +168,18 @@ CB200_XHD void absorb(typename S::W (&H)[8], uint32_t done, int len, const M& ms
 template <class S, class M>
 CB200_XHD void hmac(typename S::W (&out)[8], const typename S::W (&ki)[8], const typename S::W (&ko)[8], int len, const M& msg) {
   using W = typename S::W;
-  constexpr int WB = S::kWordBytes;
+  constexpr int WB = S::kWordBytes, DW = S::kDigest / WB;
   W h[8];
 #pragma unroll
   for (int i = 0; i < 8; i++) h[i] = ki[i];
   absorb<S>(h, S::kBlock, len, msg);
-  // outer hash: one block holding the inner digest (8 words), the padding and the length of block + digest
+  // outer hash: one block holding the inner digest (DW words), the padding and the length of block + digest
   W m[16];
 #pragma unroll
-  for (int i = 0; i < 8; i++) m[i] = h[i];
-  m[8] = (W)0x80 << (8 * (WB - 1));
+  for (int i = 0; i < DW; i++) m[i] = h[i];
+  m[DW] = (W)0x80 << (8 * (WB - 1));
 #pragma unroll
-  for (int i = 9; i < 15; i++) m[i] = 0;
+  for (int i = DW + 1; i < 15; i++) m[i] = 0;
   m[15] = (W)((uint64_t)(S::kBlock + S::kDigest) << 3);
 #pragma unroll
   for (int i = 0; i < 8; i++) out[i] = ko[i];
@@ -172,14 +190,15 @@ CB200_XHD void hmac(typename S::W (&out)[8], const typename S::W (&ki)[8], const
 template <class S>
 CB200_XHD void hmac_key(typename S::W (&ki)[8], typename S::W (&ko)[8], const typename S::W (&key)[8]) {
   using W = typename S::W;
+  constexpr int DW = S::kDigest / S::kWordBytes;
   const W i36 = (W)0x3636363636363636ull, i5c = (W)0x5c5c5c5c5c5c5c5cull;
   W m[16];
 #pragma unroll
-  for (int i = 0; i < 16; i++) m[i] = (i < 8 ? key[i] : 0) ^ i36;
+  for (int i = 0; i < 16; i++) m[i] = (i < DW ? key[i] : 0) ^ i36;
   S::iv(ki);
   S::compress(ki, m);
 #pragma unroll
-  for (int i = 0; i < 16; i++) m[i] = (i < 8 ? key[i] : 0) ^ i5c;
+  for (int i = 0; i < 16; i++) m[i] = (i < DW ? key[i] : 0) ^ i5c;
   S::iv(ko);
   S::compress(ko, m);
 }
@@ -193,8 +212,8 @@ CB200_XHD uint8_t digest_byte(const typename S::W (&h)[8], int j) {
 
 // ---------------------------------------------------------------- HPKE's labeled messages (RFC 9180 section 4)
 // LabeledExtract:  "HPKE-v1" || suite_id || label || ikm
-// LabeledExpand:   I2OSP(L, 2) || "HPKE-v1" || suite_id || label || info || 0x01 (the first and only HKDF-Expand
-//                  block: every L here is at most one digest)
+// LabeledExpand:   I2OSP(L, 2) || "HPKE-v1" || suite_id || label || info || 0x01 (the first HKDF-Expand block; the
+//                  only one where L is at most one digest, else ExpandNext gives the second)
 // suite_id = "KEM" || I2OSP(kem_id, 2).  ikm / info are up to three rows of r0n, r1n, r2n bytes.
 struct Labeled {
   int expand;         // 1: LabeledExpand's message, 0: LabeledExtract's
@@ -224,6 +243,20 @@ struct Labeled {
     j -= r1n;
     if (j < r2n) return r2[j];
     return 1;  // the HKDF-Expand counter
+  }
+};
+
+// HKDF-Expand's second block message T(1) || m' || 0x02, where m = m' || 0x01 is the first block's message: T(1) (one
+// digest, in registers) and m (a functor like Labeled) as given.
+template <class S, class M>
+struct ExpandNext {
+  const typename S::W (&t1)[8];
+  const M& m;
+  CB200_XHD int len() const { return S::kDigest + m.len(); }
+  CB200_XHD uint8_t operator()(int j) const {
+    if (j < S::kDigest) return digest_byte<S>(t1, j);
+    j -= S::kDigest;
+    return j == m.len() - 1 ? 2 : m(j);
   }
 };
 

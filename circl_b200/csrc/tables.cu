@@ -20,9 +20,9 @@ int init_extra_tables(Dev& c) {  // device c.device is current
   if (c.x25519_table) cudaFree(c.x25519_table);
   CB200_CUDA(cudaMalloc(&c.x25519_table, xt.size() * sizeof(int32_t)));
   CB200_CUDA(cudaMemcpy(c.x25519_table, xt.data(), xt.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-  // fixed-base tables of Ed448 (ed448.cu) and P-256 (p256.cu)
+  // fixed-base tables of Ed448 (ed448.cu) and P-256 / P-384 / P-521 (p256.cu)
   int rc = init_ed448_table(c);
   if (rc) return rc;
-  return init_p256_table(c);
+  return init_nistp_tables(c);
 }
 }  // namespace cb200

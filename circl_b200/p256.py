@@ -1,4 +1,7 @@
 """P-256 over the C ABI: the raw ECDH step and the kem.AuthScheme mirror of HPKE's DHKEM(P-256, HKDF-SHA256).
+The ECDH step (ecdh) and the scheme class (NistDHKEM) take the curve (Curve) as a parameter; circl_b200.p384 and
+circl_b200.p521 use them for P-384 and P-521.  These three names are the package's shared machinery, not part of this
+module's public surface.
 
   p256_keygen / p256_shared        crypto/ecdh.P256() PublicKey / ECDH, batched (like x448.x448_keygen / x448_shared)
   HPKE_KEM_P256_HKDF_SHA256        DHKEM(P-256, HKDF-SHA256), kem_id 0x10    hpke/shortkem.go, hpke/kembase.go
@@ -25,9 +28,29 @@ from .mlkem import ErrPrivKeySize, ErrPubKeySize, KemError, PublicKey
 __all__ = ["P256DHKEM", "ByName", "All", "ErrInvalidKEMPublicKey", "ErrInvalidKEMPrivateKey", "p256_keygen",
            "p256_shared", "PrivateKey", "PublicKey"]
 
+
+class Curve:
+    """A NIST curve y^2 = x^3 - 3x + b mod p of order n, with `size`-byte scalars and coordinates, on the C entry points
+    cb200_<prefix> and cb200_hpke_<prefix>_*."""
+
+    def __init__(self, prefix: str, size: int, p: int, n: int, b: int):
+        self.prefix, self.size, self.p, self.n, self.b = prefix, size, p, n, b
+        self.npk = 1 + 2 * size
+
+    def scalar_ok(self, b: bytes) -> bool:
+        return 0 < int.from_bytes(b, "big") < self.n
+
+    def point_ok(self, b: bytes) -> bool:
+        if len(b) != self.npk or b[0] != 4:
+            return False
+        x, y = int.from_bytes(b[1:1 + self.size], "big"), int.from_bytes(b[1 + self.size:], "big")
+        return x < self.p and y < self.p and (y * y - (x * x * x - 3 * x + self.b)) % self.p == 0
+
+
 P = 2**256 - 2**224 + 2**192 + 2**96 - 1
 N = 0xffffffff00000000ffffffffffffffffbce6faada7179e84f3b9cac2fc632551
 B = 0x5ac635d8aa3a93e7b3ebbd55769886bc651d06b0cc53b0f63bce3c3e27d2604b
+CURVE = Curve("p256", 32, P, N, B)
 
 
 class ErrInvalidKEMPublicKey(KemError):  # hpke.ErrInvalidKEMPublicKey, hpke/hpke.go:278
@@ -56,29 +79,21 @@ def _raise_for(code, status):
         raise _err(ErrInvalidKEMPublicKey, "hpke: invalid KEM public key", status)
 
 
-def _scalar_ok(b: bytes) -> bool:
-    return 0 < int.from_bytes(b, "big") < N
-
-
-def _point_ok(b: bytes) -> bool:
-    if len(b) != 65 or b[0] != 4:
-        return False
-    x, y = int.from_bytes(b[1:33], "big"), int.from_bytes(b[33:], "big")
-    return x < P and y < P and (y * y - (x * x * x - 3 * x + B)) % P == 0
-
-
 # ---------------------------------------------------------------- the raw ECDH step
-def _ecdh(scalars, points):
-    k = _prep(scalars, 32, ValueError("scalars: (n, 32) uint8"))
+def ecdh(curve: Curve, scalars, points):
+    """KeyGen (points None) or Shared on `curve`; see p256_keygen / p256_shared."""
+    B, W = curve.size, curve.npk
+    k = _prep(scalars, B, ValueError(f"scalars: (n, {B}) uint8"))
     n = k.shape[0]
     pt = None
     if points is not None:
-        pt = _prep(points, 65, ValueError("points: (n, 65) uint8"))
+        pt = _prep(points, W, ValueError(f"points: (n, {W}) uint8"))
         if pt.shape[0] != n or _is_torch(pt) != _is_torch(k):
-            raise ValueError("points: (n, 65) uint8 on the scalars' side")
-    out, status = _new(k, (n, 65 if pt is None else 32)), _zeros(k, (n,))
+            raise ValueError(f"points: (n, {W}) uint8 on the scalars' side")
+    out, status = _new(k, (n, W if pt is None else B)), _zeros(k, (n,))
     try:
-        check(lib().cb200_p256(_ptr(k), None if pt is None else _ptr(pt), _ptr(out), _ptr(status), n))
+        check(getattr(lib(), "cb200_" + curve.prefix)(_ptr(k), None if pt is None else _ptr(pt), _ptr(out),
+                                                       _ptr(status), n))
     except Cb200Error as e:
         if e.code not in (-3, -5):
             raise
@@ -91,37 +106,39 @@ def _ecdh(scalars, points):
 def p256_keygen(scalars):
     """(n, 32) big-endian scalars in [1, n - 1] -> (n, 65) public keys 0x04 || X || Y.  An invalid scalar raises
     ErrInvalidKEMPrivateKey (with .status) after the batch ran; its row is all zero."""
-    return _ecdh(scalars, None)
+    return ecdh(CURVE, scalars, None)
 
 
 def p256_shared(scalars, points):
     """(n, 32) scalars, (n, 65) public keys -> (n, 32) X coordinates of [k]P.  Invalid inputs raise as p256_keygen
     (ErrInvalidKEMPrivateKey before ErrInvalidKEMPublicKey)."""
-    return _ecdh(scalars, points)
+    return ecdh(CURVE, scalars, points)
 
 
 # ---------------------------------------------------------------- DHKEM(P-256, HKDF-SHA256)
 class PrivateKey(_DHPrivateKey):
-    """kem.PrivateKey of DHKEM(P-256): the 32-byte big-endian scalar."""
+    """kem.PrivateKey of a NIST DHKEM: the big-endian scalar (32 bytes for P-256)."""
 
     def Public(self) -> PublicKey:
         """KeyGen of this key on the GPU (shortkem.go:151-157)."""
         sk = np.frombuffer(self._packed, dtype=np.uint8).reshape(1, -1)
-        return PublicKey(self._scheme, p256_keygen(sk)[0].tobytes())
+        return PublicKey(self._scheme, ecdh(self._scheme._curve, sk, None)[0].tobytes())
 
 
-class P256DHKEM(DHKEM):
-    """DHKEM(P-256, HKDF-SHA256) on the cb200_hpke_p256_* entry points."""
+class NistDHKEM(DHKEM):
+    """A NIST DHKEM (kem_id `ident`, shared secrets of `nss` bytes) on the cb200_hpke_<curve.prefix>_* entry points;
+    P256DHKEM below, and circl_b200.p384 / p521's schemes."""
 
     _Priv = PrivateKey
 
-    def __init__(self):
-        super().__init__("HPKE_KEM_P256_HKDF_SHA256", 0x10, 32, 32)
-        self._npk = 65
+    def __init__(self, name, ident, nss, curve):
+        super().__init__(name, ident, curve.size, nss)
+        self._curve = curve
+        self._npk = curve.npk
 
     def _c(self, name, *args):
-        """cb200_hpke_p256_<name>(args...)"""
-        return getattr(lib(), "cb200_hpke_p256_" + name)(*args)
+        """cb200_hpke_<prefix>_<name>(args...)"""
+        return getattr(lib(), f"cb200_hpke_{self._curve.prefix}_" + name)(*args)
 
     @staticmethod
     def _run(call, status):
@@ -137,24 +154,33 @@ class P256DHKEM(DHKEM):
     def UnmarshalBinaryPublicKey(self, buf: bytes) -> PublicKey:
         """shortkem.go:115-130: the size, then crypto/ecdh NewPublicKey (0x04 || X || Y, X, Y < p, on the curve)."""
         pk = super().UnmarshalBinaryPublicKey(buf)
-        if not _point_ok(bytes(buf)):
+        if not self._curve.point_ok(bytes(buf)):
             raise _err(ErrInvalidKEMPublicKey, "hpke: invalid KEM public key", None)
         return pk
 
     def UnmarshalBinaryPrivateKey(self, buf: bytes) -> PrivateKey:
         """shortkem.go:103-113: the size, then crypto/ecdh NewPrivateKey (0 < k < n)."""
         sk = super().UnmarshalBinaryPrivateKey(buf)
-        if not _scalar_ok(bytes(buf)):
+        if not self._curve.scalar_ok(bytes(buf)):
             raise _err(ErrInvalidKEMPrivateKey, "hpke: invalid KEM private key", None)
         return sk
 
     def GenerateKeyPair(self):
         """A random scalar in [1, n - 1] (crypto/ecdh GenerateKey, shortkem.go:92-100)."""
         while True:
-            b = os.urandom(32)
-            if _scalar_ok(b):
+            b = bytearray(os.urandom(self._nsk))
+            b[0] &= (1 << (self._curve.n.bit_length() - 8 * (self._nsk - 1))) - 1  # P-521: the top byte's one bit
+            b = bytes(b)
+            if self._curve.scalar_ok(b):
                 sk = PrivateKey(self, b)
                 return sk.Public(), sk
+
+
+class P256DHKEM(NistDHKEM):
+    """DHKEM(P-256, HKDF-SHA256) on the cb200_hpke_p256_* entry points."""
+
+    def __init__(self):
+        super().__init__("HPKE_KEM_P256_HKDF_SHA256", 0x10, 32, CURVE)
 
 
 _SCHEME = P256DHKEM()

@@ -690,47 +690,86 @@ func HPKEDecaps(id int, skR, enc, pkS, ss []byte, ok []bool) error {
 	return err
 }
 
-// DHKEM(P-256, HKDF-SHA256), kem_id 0x10 (hpke/shortkem.go; include/circl_b200.h cb200_hpke_p256_*): sk and seeds 32
-// bytes, pk and enc 65 (0x04 || X || Y), ss 32.  The generic HPKE* functions above do not take this id.
+// The NIST DHKEMs (hpke/shortkem.go; include/circl_b200.h cb200_hpke_p256_* / p384_* / p521_*), each on entry points
+// of its own; the generic HPKE* functions above do not take these ids.
+//   DHKEM(P-256, HKDF-SHA256), kem_id 0x10: sk and seeds 32 bytes, pk and enc 65 (0x04 || X || Y), ss 32
+//   DHKEM(P-384, HKDF-SHA384), kem_id 0x11: sk and seeds 48 bytes, pk and enc 97, ss 48
+//   DHKEM(P-521, HKDF-SHA512), kem_id 0x12: sk and seeds 66 bytes, pk and enc 133, ss 64
 const (
 	HPKEP256HKDFSHA256     = 0x10
 	HPKEP256PrivateKeySize = 32
 	HPKEP256PublicKeySize  = 65
 	HPKEP256SharedKeySize  = 32
+
+	HPKEP384HKDFSHA384     = 0x11
+	HPKEP384PrivateKeySize = 48
+	HPKEP384PublicKeySize  = 97
+	HPKEP384SharedKeySize  = 48
+
+	HPKEP521HKDFSHA512     = 0x12
+	HPKEP521PrivateKeySize = 66
+	HPKEP521PublicKeySize  = 133
+	HPKEP521SharedKeySize  = 64
 )
 
-// HPKEP256Keygen: batched DeriveKeyPair (shortkem.go:63-90) on n seeds of 32 bytes; pk: n*65, sk: n*32.
-func HPKEP256Keygen(seeds, pk, sk []byte) error {
-	n := len(seeds) / HPKEP256PrivateKeySize
-	if len(seeds) != n*HPKEP256PrivateKeySize || len(pk) != n*HPKEP256PublicKeySize || len(sk) != n*HPKEP256PrivateKeySize {
-		panic("cb200: HPKEP256Keygen buffers have the wrong length")
-	}
-	if n == 0 {
-		return nil
-	}
-	return call(func() C.int { return C.cb200_hpke_p256_keygen(u8(seeds), u8(pk), u8(sk), C.size_t(n)) })
+// nist: one NIST DHKEM's id, sizes and the prefix of its Go names (for panics)
+type nist struct {
+	id, sk, pk, ss int
+	name           string
 }
 
-// HPKEP256Encaps: batched Encap, or AuthEncap when skS is not nil.  pkR (65 bytes) and skS (32): one key or n keys
-// each; seeds: n*32; enc: n*65; ss: n*32.  After the whole batch ran, ErrPrivKey (hpke.ErrInvalidKEMPrivateKey for the
-// caller) is returned if any skS is not in [1, n - 1], else ErrPubKey (hpke.ErrInvalidKEMPublicKey) if any pkR is not
-// a P-256 point; ok[i] (may be nil) tells which operations failed.
-func HPKEP256Encaps(pkR, skS, seeds, enc, ss []byte, ok []bool) error {
-	n := len(seeds) / HPKEP256PrivateKeySize
-	if len(seeds) != n*HPKEP256PrivateKeySize || len(enc) != n*HPKEP256PublicKeySize || len(ss) != n*HPKEP256SharedKeySize ||
-		(ok != nil && len(ok) != n) {
-		panic("cb200: HPKEP256Encaps buffers have the wrong length")
+var (
+	nistP256 = nist{HPKEP256HKDFSHA256, HPKEP256PrivateKeySize, HPKEP256PublicKeySize, HPKEP256SharedKeySize, "HPKEP256"}
+	nistP384 = nist{HPKEP384HKDFSHA384, HPKEP384PrivateKeySize, HPKEP384PublicKeySize, HPKEP384SharedKeySize, "HPKEP384"}
+	nistP521 = nist{HPKEP521HKDFSHA512, HPKEP521PrivateKeySize, HPKEP521PublicKeySize, HPKEP521SharedKeySize, "HPKEP521"}
+)
+
+func (c nist) keygen(seeds, pk, sk []byte) error {
+	n := len(seeds) / c.sk
+	if len(seeds) != n*c.sk || len(pk) != n*c.pk || len(sk) != n*c.sk {
+		panic("cb200: " + c.name + "Keygen buffers have the wrong length")
 	}
 	if n == 0 {
 		return nil
 	}
-	pr, prs := hpkeKey(pkR, n, HPKEP256PublicKeySize, "HPKEP256Encaps")
+	return call(func() C.int {
+		switch c.id {
+		case HPKEP384HKDFSHA384:
+			return C.cb200_hpke_p384_keygen(u8(seeds), u8(pk), u8(sk), C.size_t(n))
+		case HPKEP521HKDFSHA512:
+			return C.cb200_hpke_p521_keygen(u8(seeds), u8(pk), u8(sk), C.size_t(n))
+		}
+		return C.cb200_hpke_p256_keygen(u8(seeds), u8(pk), u8(sk), C.size_t(n))
+	})
+}
+
+func (c nist) encaps(pkR, skS, seeds, enc, ss []byte, ok []bool) error {
+	n := len(seeds) / c.sk
+	if len(seeds) != n*c.sk || len(enc) != n*c.pk || len(ss) != n*c.ss || (ok != nil && len(ok) != n) {
+		panic("cb200: " + c.name + "Encaps buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	pr, prs := hpkeKey(pkR, n, c.pk, c.name+"Encaps")
 	status := make([]byte, n)
 	err := call(func() C.int {
 		if skS == nil {
+			switch c.id {
+			case HPKEP384HKDFSHA384:
+				return C.cb200_hpke_p384_encaps(pr, prs, u8(seeds), u8(enc), u8(ss), u8(status), C.size_t(n))
+			case HPKEP521HKDFSHA512:
+				return C.cb200_hpke_p521_encaps(pr, prs, u8(seeds), u8(enc), u8(ss), u8(status), C.size_t(n))
+			}
 			return C.cb200_hpke_p256_encaps(pr, prs, u8(seeds), u8(enc), u8(ss), u8(status), C.size_t(n))
 		}
-		sp, sps := hpkeKey(skS, n, HPKEP256PrivateKeySize, "HPKEP256Encaps")
+		sp, sps := hpkeKey(skS, n, c.sk, c.name+"Encaps")
+		switch c.id {
+		case HPKEP384HKDFSHA384:
+			return C.cb200_hpke_p384_auth_encaps(pr, prs, sp, sps, u8(seeds), u8(enc), u8(ss), u8(status), C.size_t(n))
+		case HPKEP521HKDFSHA512:
+			return C.cb200_hpke_p521_auth_encaps(pr, prs, sp, sps, u8(seeds), u8(enc), u8(ss), u8(status), C.size_t(n))
+		}
 		return C.cb200_hpke_p256_auth_encaps(pr, prs, sp, sps, u8(seeds), u8(enc), u8(ss), u8(status), C.size_t(n))
 	})
 	for i := range ok {
@@ -739,23 +778,33 @@ func HPKEP256Encaps(pkR, skS, seeds, enc, ss []byte, ok []bool) error {
 	return err
 }
 
-// HPKEP256Decaps: batched Decap, or AuthDecap when pkS is not nil.  skR (32 bytes) and pkS (65): one key or n keys
-// each; enc: n*65; ss: n*32.  Errors as HPKEP256Encaps (an invalid skR is ErrPrivKey, an invalid enc or pkS ErrPubKey).
-func HPKEP256Decaps(skR, enc, pkS, ss []byte, ok []bool) error {
-	n := len(enc) / HPKEP256PublicKeySize
-	if len(enc) != n*HPKEP256PublicKeySize || len(ss) != n*HPKEP256SharedKeySize || (ok != nil && len(ok) != n) {
-		panic("cb200: HPKEP256Decaps buffers have the wrong length")
+func (c nist) decaps(skR, enc, pkS, ss []byte, ok []bool) error {
+	n := len(enc) / c.pk
+	if len(enc) != n*c.pk || len(ss) != n*c.ss || (ok != nil && len(ok) != n) {
+		panic("cb200: " + c.name + "Decaps buffers have the wrong length")
 	}
 	if n == 0 {
 		return nil
 	}
-	sr, srs := hpkeKey(skR, n, HPKEP256PrivateKeySize, "HPKEP256Decaps")
+	sr, srs := hpkeKey(skR, n, c.sk, c.name+"Decaps")
 	status := make([]byte, n)
 	err := call(func() C.int {
 		if pkS == nil {
+			switch c.id {
+			case HPKEP384HKDFSHA384:
+				return C.cb200_hpke_p384_decaps(sr, srs, u8(enc), u8(ss), u8(status), C.size_t(n))
+			case HPKEP521HKDFSHA512:
+				return C.cb200_hpke_p521_decaps(sr, srs, u8(enc), u8(ss), u8(status), C.size_t(n))
+			}
 			return C.cb200_hpke_p256_decaps(sr, srs, u8(enc), u8(ss), u8(status), C.size_t(n))
 		}
-		pp, pps := hpkeKey(pkS, n, HPKEP256PublicKeySize, "HPKEP256Decaps")
+		pp, pps := hpkeKey(pkS, n, c.pk, c.name+"Decaps")
+		switch c.id {
+		case HPKEP384HKDFSHA384:
+			return C.cb200_hpke_p384_auth_decaps(sr, srs, u8(enc), pp, pps, u8(ss), u8(status), C.size_t(n))
+		case HPKEP521HKDFSHA512:
+			return C.cb200_hpke_p521_auth_decaps(sr, srs, u8(enc), pp, pps, u8(ss), u8(status), C.size_t(n))
+		}
 		return C.cb200_hpke_p256_auth_decaps(sr, srs, u8(enc), pp, pps, u8(ss), u8(status), C.size_t(n))
 	})
 	for i := range ok {
@@ -763,6 +812,37 @@ func HPKEP256Decaps(skR, enc, pkS, ss []byte, ok []bool) error {
 	}
 	return err
 }
+
+// HPKEP256Keygen: batched DeriveKeyPair (shortkem.go:63-90) on n seeds of 32 bytes; pk: n*65, sk: n*32.
+func HPKEP256Keygen(seeds, pk, sk []byte) error { return nistP256.keygen(seeds, pk, sk) }
+
+// HPKEP256Encaps: batched Encap, or AuthEncap when skS is not nil.  pkR (65 bytes) and skS (32): one key or n keys
+// each; seeds: n*32; enc: n*65; ss: n*32.  After the whole batch ran, ErrPrivKey (hpke.ErrInvalidKEMPrivateKey for the
+// caller) is returned if any skS is not in [1, n - 1], else ErrPubKey (hpke.ErrInvalidKEMPublicKey) if any pkR is not
+// a P-256 point; ok[i] (may be nil) tells which operations failed.
+func HPKEP256Encaps(pkR, skS, seeds, enc, ss []byte, ok []bool) error {
+	return nistP256.encaps(pkR, skS, seeds, enc, ss, ok)
+}
+
+// HPKEP256Decaps: batched Decap, or AuthDecap when pkS is not nil.  skR (32 bytes) and pkS (65): one key or n keys
+// each; enc: n*65; ss: n*32.  Errors as HPKEP256Encaps (an invalid skR is ErrPrivKey, an invalid enc or pkS ErrPubKey).
+func HPKEP256Decaps(skR, enc, pkS, ss []byte, ok []bool) error { return nistP256.decaps(skR, enc, pkS, ss, ok) }
+
+// HPKEP384Keygen, HPKEP384Encaps, HPKEP384Decaps: the P-256 functions above for DHKEM(P-384, HKDF-SHA384), with
+// sk and seeds of 48 bytes, pk and enc of 97 and ss of 48.
+func HPKEP384Keygen(seeds, pk, sk []byte) error { return nistP384.keygen(seeds, pk, sk) }
+func HPKEP384Encaps(pkR, skS, seeds, enc, ss []byte, ok []bool) error {
+	return nistP384.encaps(pkR, skS, seeds, enc, ss, ok)
+}
+func HPKEP384Decaps(skR, enc, pkS, ss []byte, ok []bool) error { return nistP384.decaps(skR, enc, pkS, ss, ok) }
+
+// HPKEP521Keygen, HPKEP521Encaps, HPKEP521Decaps: the same for DHKEM(P-521, HKDF-SHA512), with sk and seeds of 66
+// bytes, pk and enc of 133 and ss of 64.
+func HPKEP521Keygen(seeds, pk, sk []byte) error { return nistP521.keygen(seeds, pk, sk) }
+func HPKEP521Encaps(pkR, skS, seeds, enc, ss []byte, ok []bool) error {
+	return nistP521.encaps(pkR, skS, seeds, enc, ss, ok)
+}
+func HPKEP521Decaps(skR, enc, pkS, ss []byte, ok []bool) error { return nistP521.decaps(skR, enc, pkS, ss, ok) }
 
 // FrodoKEM-640-SHAKE sizes (kem/frodo/frodo640shake/frodo.go:32-51).
 const (

@@ -2,7 +2,8 @@
 
 // Drop-in file for github.com/cloudflare/circl/kem/schemes (next to schemes.go): with the `cuda` build tag the registry
 // entries "ML-KEM-768", "ML-KEM-1024", "X-Wing", "HPKE_KEM_X25519_HKDF_SHA256", "HPKE_KEM_X448_HKDF_SHA512",
-// "HPKE_KEM_P256_HKDF_SHA256" and "FrodoKEM-640-SHAKE" (kem/schemes/schemes.go:30-55) are served by the cb200 engine; every
+// "HPKE_KEM_P256_HKDF_SHA256", "HPKE_KEM_P384_HKDF_SHA384", "HPKE_KEM_P521_HKDF_SHA512" and "FrodoKEM-640-SHAKE"
+// (kem/schemes/schemes.go:30-55) are served by the cb200 engine; every
 // other scheme, and every build without the tag, is untouched.  ByName keeps matching on the lower-cased Name()
 // (schemes.go:57-72), which the GPU schemes do not change.
 //
@@ -29,7 +30,7 @@ func init() {
 		return
 	}
 	for _, s := range []kem.Scheme{mlkem768cuda.Scheme(), mlkem1024cuda.Scheme(), xwingcuda.Scheme(), hpkecuda.X25519(),
-		hpkecuda.X448(), hpkecuda.P256(), frodo640shakecuda.Scheme()} {
+		hpkecuda.X448(), hpkecuda.P256(), hpkecuda.P384(), hpkecuda.P521(), frodo640shakecuda.Scheme()} {
 		name := strings.ToLower(s.Name())
 		allSchemeNames[name] = s
 		for i := range allSchemes {

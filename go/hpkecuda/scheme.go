@@ -1,7 +1,8 @@
 //go:build cuda && cgo
 
-// Package hpkecuda backs the kem/schemes entries "HPKE_KEM_X25519_HKDF_SHA256", "HPKE_KEM_X448_HKDF_SHA512" and
-// "HPKE_KEM_P256_HKDF_SHA256" (hpke/algs.go:248-277) with the cb200 engine.  Both are kem.AuthScheme (kem/kem.go:84-90): DeriveKeyPair, the
+// Package hpkecuda backs the kem/schemes entries "HPKE_KEM_X25519_HKDF_SHA256", "HPKE_KEM_X448_HKDF_SHA512",
+// "HPKE_KEM_P256_HKDF_SHA256", "HPKE_KEM_P384_HKDF_SHA384" and "HPKE_KEM_P521_HKDF_SHA512" (hpke/algs.go:248-277) with
+// the cb200 engine.  All are kem.AuthScheme (kem/kem.go:84-90): DeriveKeyPair, the
 // (authenticated) encapsulations and decapsulations run on the GPU as batches of one, everything else (key parsing,
 // GenerateKeyPair, marshalling) delegates to CIRCL's own scheme.  EncapsulateBatch and DecapsulateBatch are the entry
 // points that make a GPU worthwhile.
@@ -28,29 +29,54 @@ var (
 	x25519 = &scheme{hpke.KEM_X25519_HKDF_SHA256.Scheme().(kem.AuthScheme), cb200.HPKEX25519HKDFSHA256}
 	x448   = &scheme{hpke.KEM_X448_HKDF_SHA512.Scheme().(kem.AuthScheme), cb200.HPKEX448HKDFSHA512}
 	p256   = &scheme{hpke.KEM_P256_HKDF_SHA256.Scheme().(kem.AuthScheme), cb200.HPKEP256HKDFSHA256}
+	p384   = &scheme{hpke.KEM_P384_HKDF_SHA384.Scheme().(kem.AuthScheme), cb200.HPKEP384HKDFSHA384}
+	p521   = &scheme{hpke.KEM_P521_HKDF_SHA512.Scheme().(kem.AuthScheme), cb200.HPKEP521HKDFSHA512}
 )
 
-// X25519, X448 and P256 return the GPU-backed schemes; Name() is unchanged so kem/schemes.ByName keeps working.
+// X25519, X448, P256, P384 and P521 return the GPU-backed schemes; Name() is unchanged so kem/schemes.ByName keeps
+// working.
 func X25519() kem.AuthScheme { return x25519 }
 func X448() kem.AuthScheme   { return x448 }
 func P256() kem.AuthScheme   { return p256 }
+func P384() kem.AuthScheme   { return p384 }
+func P521() kem.AuthScheme   { return p521 }
 
-// The engine calls of a scheme: P-256 has entry points of its own.
+// isNIST: the NIST curves have entry points of their own and validate points and scalars
+func (s *scheme) isNIST() bool {
+	return s.id == cb200.HPKEP256HKDFSHA256 || s.id == cb200.HPKEP384HKDFSHA384 || s.id == cb200.HPKEP521HKDFSHA512
+}
+
+// The engine calls of a scheme.
 func (s *scheme) keygen(seeds, pk, sk []byte) error {
-	if s.id == cb200.HPKEP256HKDFSHA256 {
+	switch s.id {
+	case cb200.HPKEP256HKDFSHA256:
 		return cb200.HPKEP256Keygen(seeds, pk, sk)
+	case cb200.HPKEP384HKDFSHA384:
+		return cb200.HPKEP384Keygen(seeds, pk, sk)
+	case cb200.HPKEP521HKDFSHA512:
+		return cb200.HPKEP521Keygen(seeds, pk, sk)
 	}
 	return cb200.HPKEKeygen(s.id, seeds, pk, sk)
 }
 func (s *scheme) encaps(pkR, skS, seeds, enc, ss []byte, ok []bool) error {
-	if s.id == cb200.HPKEP256HKDFSHA256 {
+	switch s.id {
+	case cb200.HPKEP256HKDFSHA256:
 		return s.mapErr(cb200.HPKEP256Encaps(pkR, skS, seeds, enc, ss, ok))
+	case cb200.HPKEP384HKDFSHA384:
+		return s.mapErr(cb200.HPKEP384Encaps(pkR, skS, seeds, enc, ss, ok))
+	case cb200.HPKEP521HKDFSHA512:
+		return s.mapErr(cb200.HPKEP521Encaps(pkR, skS, seeds, enc, ss, ok))
 	}
 	return s.mapErr(cb200.HPKEEncaps(s.id, pkR, skS, seeds, enc, ss, ok))
 }
 func (s *scheme) decaps(skR, enc, pkS, ss []byte, ok []bool) error {
-	if s.id == cb200.HPKEP256HKDFSHA256 {
+	switch s.id {
+	case cb200.HPKEP256HKDFSHA256:
 		return s.mapErr(cb200.HPKEP256Decaps(skR, enc, pkS, ss, ok))
+	case cb200.HPKEP384HKDFSHA384:
+		return s.mapErr(cb200.HPKEP384Decaps(skR, enc, pkS, ss, ok))
+	case cb200.HPKEP521HKDFSHA512:
+		return s.mapErr(cb200.HPKEP521Decaps(skR, enc, pkS, ss, ok))
 	}
 	return s.mapErr(cb200.HPKEDecaps(s.id, skR, enc, pkS, ss, ok))
 }
@@ -64,13 +90,13 @@ func mustMarshal(k interface{ MarshalBinary() ([]byte, error) }) []byte {
 }
 
 // mapErr maps the engine's per-batch failures to the reference's errors: for X25519 / X448 a low-order point is
-// hpke.ErrInvalidKEMSharedSecret (hpke/hpke.go:280); for P-256 an invalid point or scalar is
+// hpke.ErrInvalidKEMSharedSecret (hpke/hpke.go:280); for the NIST curves an invalid point or scalar is
 // hpke.ErrInvalidKEMPublicKey / ErrInvalidKEMPrivateKey (hpke/hpke.go:278-279)
 func (s *scheme) mapErr(err error) error {
 	switch {
-	case err == cb200.ErrPubKey && s.id == cb200.HPKEP256HKDFSHA256:
+	case err == cb200.ErrPubKey && s.isNIST():
 		return hpke.ErrInvalidKEMPublicKey
-	case err == cb200.ErrPrivKey && s.id == cb200.HPKEP256HKDFSHA256:
+	case err == cb200.ErrPrivKey && s.isNIST():
 		return hpke.ErrInvalidKEMPrivateKey
 	case err == cb200.ErrPubKey:
 		return hpke.ErrInvalidKEMSharedSecret
@@ -130,7 +156,7 @@ func (s *scheme) decap(skr kem.PrivateKey, ct []byte, pks kem.PublicKey) ([]byte
 	if len(ct) != s.PublicKeySize() {
 		return nil, kem.ErrPubKeySize // ct is parsed as a public key (kembase.go:222, xkem.go:95-101)
 	}
-	if s.id == cb200.HPKEP256HKDFSHA256 { // shortkem.go:115-130 also checks the point
+	if s.isNIST() { // shortkem.go:115-130 also checks the point
 		if _, err := s.AuthScheme.UnmarshalBinaryPublicKey(ct); err != nil {
 			return nil, err
 		}

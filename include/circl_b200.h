@@ -331,6 +331,52 @@ size_t cb200_hpke_p256_shared_key_size(void);             /* 32 */
 size_t cb200_hpke_p256_seed_size(void);                   /* 32 */
 size_t cb200_hpke_p256_encapsulation_seed_size(void);     /* 32 */
 
+/* ---- P-384 and P-521 ECDH (crypto/ecdh.P384() / P521()) ----
+ * cb200_p384 / cb200_p521: the contract of cb200_p256 with 48-byte scalars and Shared outputs and 97-byte points and
+ * KeyGen outputs (P-384), or 66 and 133 bytes (P-521).  A 66-byte P-521 scalar whose leading byte is above 0x01 is
+ * >= n, so invalid. */
+int cb200_p384(const uint8_t *scalars, const uint8_t *points, uint8_t *out, uint8_t *status, size_t n);
+int cb200_p521(const uint8_t *scalars, const uint8_t *points, uint8_t *out, uint8_t *status, size_t n);
+
+/* ---- HPKE DHKEM(P-384, HKDF-SHA384), kem_id 0x11, and DHKEM(P-521, HKDF-SHA512), kem_id 0x12 (hpke/algs.go) ----
+ * The cb200_hpke_p256_* contracts, on their own entry points; the generic entry points keep treating 0x11 and 0x12 as
+ * unknown.  Sizes (P-384 / P-521): seed, encapsulation seed and sk 48 / 66, pk and enc 97 / 133, ss 48 / 64.
+ * keygen = DeriveKeyPair (shortkem.go:63-90): the first candidate LabeledExpand(dkp_prk, "candidate", I2OSP(ctr, 1),
+ *   Nsk), with its first byte ANDed with 0xff / 0x01, that lies in [1, n - 1].  P-521's 66-byte candidate is two
+ *   HKDF-Expand blocks. */
+#define CB200_HPKE_P384_HKDF_SHA384 0x11
+#define CB200_HPKE_P521_HKDF_SHA512 0x12
+int cb200_hpke_p384_keygen(const uint8_t *seeds, uint8_t *pk, uint8_t *sk, size_t n);
+int cb200_hpke_p384_encaps(const uint8_t *pkR, size_t pkR_stride, const uint8_t *seeds, uint8_t *enc, uint8_t *ss,
+                           uint8_t *status, size_t n);
+int cb200_hpke_p384_decaps(const uint8_t *skR, size_t skR_stride, const uint8_t *enc, uint8_t *ss, uint8_t *status,
+                           size_t n);
+int cb200_hpke_p384_auth_encaps(const uint8_t *pkR, size_t pkR_stride, const uint8_t *skS, size_t skS_stride,
+                                const uint8_t *seeds, uint8_t *enc, uint8_t *ss, uint8_t *status, size_t n);
+int cb200_hpke_p384_auth_decaps(const uint8_t *skR, size_t skR_stride, const uint8_t *enc, const uint8_t *pkS,
+                                size_t pkS_stride, uint8_t *ss, uint8_t *status, size_t n);
+size_t cb200_hpke_p384_public_key_size(void);             /* 97 */
+size_t cb200_hpke_p384_private_key_size(void);            /* 48 */
+size_t cb200_hpke_p384_ciphertext_size(void);             /* 97 */
+size_t cb200_hpke_p384_shared_key_size(void);             /* 48 */
+size_t cb200_hpke_p384_seed_size(void);                   /* 48 */
+size_t cb200_hpke_p384_encapsulation_seed_size(void);     /* 48 */
+int cb200_hpke_p521_keygen(const uint8_t *seeds, uint8_t *pk, uint8_t *sk, size_t n);
+int cb200_hpke_p521_encaps(const uint8_t *pkR, size_t pkR_stride, const uint8_t *seeds, uint8_t *enc, uint8_t *ss,
+                           uint8_t *status, size_t n);
+int cb200_hpke_p521_decaps(const uint8_t *skR, size_t skR_stride, const uint8_t *enc, uint8_t *ss, uint8_t *status,
+                           size_t n);
+int cb200_hpke_p521_auth_encaps(const uint8_t *pkR, size_t pkR_stride, const uint8_t *skS, size_t skS_stride,
+                                const uint8_t *seeds, uint8_t *enc, uint8_t *ss, uint8_t *status, size_t n);
+int cb200_hpke_p521_auth_decaps(const uint8_t *skR, size_t skR_stride, const uint8_t *enc, const uint8_t *pkS,
+                                size_t pkS_stride, uint8_t *ss, uint8_t *status, size_t n);
+size_t cb200_hpke_p521_public_key_size(void);             /* 133 */
+size_t cb200_hpke_p521_private_key_size(void);            /* 66 */
+size_t cb200_hpke_p521_ciphertext_size(void);             /* 133 */
+size_t cb200_hpke_p521_shared_key_size(void);             /* 64 */
+size_t cb200_hpke_p521_seed_size(void);                   /* 66 */
+size_t cb200_hpke_p521_encapsulation_seed_size(void);     /* 66 */
+
 /* ---- FrodoKEM-640-SHAKE (kem/frodo/frodo640shake), the only parameter set the reference has ----
  * Sizes: pk 9616, sk 19888, ct 9720, ss 16, seed 48 (s || seedSE || z), encapsulation seed 16 (mu).
  * keygen = DeriveKeyPair (frodo.go:84-135); encaps = EncapsulateDeterministically (:160-240); decaps = Decapsulate

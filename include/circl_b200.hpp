@@ -94,13 +94,54 @@ class PrivateKey {  // kem.PrivateKey (kem/kem.go:22-30)
   Bytes packed_;
 };
 
+// The entry points of one NIST DHKEM (cb200_hpke_p256_* / p384_* / p521_*), its raw ECDH (cb200_p256 / p384 / p521)
+// and its group order n (big-endian, Nsk bytes); nullptr for any other id.
+struct NistOps {
+  size_t (*pk_size)(void), (*sk_size)(void), (*ss_size)(void);
+  int (*keygen)(const uint8_t*, uint8_t*, uint8_t*, size_t);
+  int (*encaps)(const uint8_t*, size_t, const uint8_t*, uint8_t*, uint8_t*, uint8_t*, size_t);
+  int (*decaps)(const uint8_t*, size_t, const uint8_t*, uint8_t*, uint8_t*, size_t);
+  int (*auth_encaps)(const uint8_t*, size_t, const uint8_t*, size_t, const uint8_t*, uint8_t*, uint8_t*, uint8_t*, size_t);
+  int (*auth_decaps)(const uint8_t*, size_t, const uint8_t*, const uint8_t*, size_t, uint8_t*, uint8_t*, size_t);
+  int (*ecdh)(const uint8_t*, const uint8_t*, uint8_t*, uint8_t*, size_t);
+  const uint8_t* n;
+};
+inline const NistOps* nist_ops(int id) {
+  static const uint8_t n256[32] = {0xff, 0xff, 0xff, 0xff, 0x00, 0x00, 0x00, 0x00, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
+                                   0xff, 0xff, 0xbc, 0xe6, 0xfa, 0xad, 0xa7, 0x17, 0x9e, 0x84, 0xf3, 0xb9, 0xca, 0xc2,
+                                   0xfc, 0x63, 0x25, 0x51};
+  static const uint8_t n384[48] = {0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
+                                   0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xc7, 0x63, 0x4d, 0x81,
+                                   0xf4, 0x37, 0x2d, 0xdf, 0x58, 0x1a, 0x0d, 0xb2, 0x48, 0xb0, 0xa7, 0x7a, 0xec, 0xec,
+                                   0x19, 0x6a, 0xcc, 0xc5, 0x29, 0x73};
+  static const uint8_t n521[66] = {0x01, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
+                                   0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
+                                   0xff, 0xff, 0xff, 0xff, 0xff, 0xfa, 0x51, 0x86, 0x87, 0x83, 0xbf, 0x2f, 0x96, 0x6b,
+                                   0x7f, 0xcc, 0x01, 0x48, 0xf7, 0x09, 0xa5, 0xd0, 0x3b, 0xb5, 0xc9, 0xb8, 0x89, 0x9c,
+                                   0x47, 0xae, 0xbb, 0x6f, 0xb7, 0x1e, 0x91, 0x38, 0x64, 0x09};
+#define CIRCL_NIST_OPS(c, n)                                                                                         \
+  {cb200_hpke_##c##_public_key_size, cb200_hpke_##c##_private_key_size, cb200_hpke_##c##_shared_key_size,            \
+   cb200_hpke_##c##_keygen, cb200_hpke_##c##_encaps, cb200_hpke_##c##_decaps, cb200_hpke_##c##_auth_encaps,          \
+   cb200_hpke_##c##_auth_decaps, cb200_##c, n}
+  static const NistOps p256 = CIRCL_NIST_OPS(p256, n256), p384 = CIRCL_NIST_OPS(p384, n384),
+                       p521 = CIRCL_NIST_OPS(p521, n521);
+#undef CIRCL_NIST_OPS
+  switch (id) {
+    case CB200_HPKE_P256_HKDF_SHA256: return &p256;
+    case CB200_HPKE_P384_HKDF_SHA384: return &p384;
+    case CB200_HPKE_P521_HKDF_SHA512: return &p521;
+  }
+  return nullptr;
+}
+
 // kem.Scheme (kem/kem.go:33-82).  One class serves the four families behind the C ABI:
 //   MLKEM   ML-KEM-512/768/1024            kem/mlkem/mlkem768/kyber.go:267-407
 //   KYBER3  round-3 Kyber512/768/1024      kem/kyber/kyber768/kyber.go:267-407
 //   XWING   X-Wing                         kem/xwing/scheme.go:1-140
 //   HYBRID  X25519MLKEM768, Kyber768-X25519, Kyber512-X25519,
 //           Kyber768-X448, Kyber1024-X448                      kem/hybrid/hybrid.go:76-315
-//   HPKE    HPKE_KEM_X25519_HKDF_SHA256, HPKE_KEM_X448_HKDF_SHA512   hpke/kembase.go, hpke/xkem.go; these are also
+//   HPKE    HPKE_KEM_X25519_HKDF_SHA256, HPKE_KEM_X448_HKDF_SHA512   hpke/kembase.go, hpke/xkem.go, and the NIST
+//           DHKEMs HPKE_KEM_P256/P384/P521_* (hpke/shortkem.go, their own entry points: nist()); these are also
 //           kem.AuthScheme (kem/kem.go:84-90): the Auth* methods below serve them only
 //   FRODO   FrodoKEM-640-SHAKE             kem/frodo/frodo640shake/frodo.go:405-547
 class Scheme {
@@ -110,32 +151,32 @@ class Scheme {
   Scheme(std::string name, Kind kind, int id) : name_(std::move(name)), kind_(kind), k_(id) {}
   const std::string& Name() const { return name_; }
   size_t CiphertextSize() const {
-    if (kind_ == HPKE) return p256() ? cb200_hpke_p256_ciphertext_size() : cb200_hpke_ciphertext_size(k_);
+    if (kind_ == HPKE) return nist() ? nist()->pk_size() : cb200_hpke_ciphertext_size(k_);
     if (kind_ == FRODO) return cb200_frodo640shake_ciphertext_size();
     return kind_ == XWING ? 1120 : kind_ == HYBRID ? cb200_hybrid_ciphertext_size(k_) : cb200_mlkem_ciphertext_size(k_);
   }
   size_t SharedKeySize() const {
-    if (kind_ == HPKE) return p256() ? cb200_hpke_p256_shared_key_size() : cb200_hpke_shared_key_size(k_);
+    if (kind_ == HPKE) return nist() ? nist()->ss_size() : cb200_hpke_shared_key_size(k_);
     if (kind_ == FRODO) return cb200_frodo640shake_shared_key_size();
     return kind_ == HYBRID ? cb200_hybrid_shared_key_size(k_) : 32;
   }
   size_t PrivateKeySize() const {
-    if (kind_ == HPKE) return p256() ? cb200_hpke_p256_private_key_size() : cb200_hpke_private_key_size(k_);
+    if (kind_ == HPKE) return nist() ? nist()->sk_size() : cb200_hpke_private_key_size(k_);
     if (kind_ == FRODO) return cb200_frodo640shake_private_key_size();
     return kind_ == XWING ? 32 : kind_ == HYBRID ? cb200_hybrid_private_key_size(k_) : cb200_mlkem_private_key_size(k_);
   }
   size_t PublicKeySize() const {
-    if (kind_ == HPKE) return p256() ? cb200_hpke_p256_public_key_size() : cb200_hpke_public_key_size(k_);
+    if (kind_ == HPKE) return nist() ? nist()->pk_size() : cb200_hpke_public_key_size(k_);
     if (kind_ == FRODO) return cb200_frodo640shake_public_key_size();
     return kind_ == XWING ? 1216 : kind_ == HYBRID ? cb200_hybrid_public_key_size(k_) : cb200_mlkem_public_key_size(k_);
   }
   size_t SeedSize() const {
-    if (kind_ == HPKE) return p256() ? cb200_hpke_p256_seed_size() : cb200_hpke_seed_size(k_);
+    if (kind_ == HPKE) return nist() ? nist()->sk_size() : cb200_hpke_seed_size(k_);
     if (kind_ == FRODO) return cb200_frodo640shake_seed_size();
     return kind_ == XWING ? 32 : kind_ == HYBRID ? cb200_hybrid_seed_size(k_) : 64;
   }
   size_t EncapsulationSeedSize() const {
-    if (kind_ == HPKE) return p256() ? cb200_hpke_p256_encapsulation_seed_size() : cb200_hpke_encapsulation_seed_size(k_);
+    if (kind_ == HPKE) return nist() ? nist()->sk_size() : cb200_hpke_encapsulation_seed_size(k_);
     if (kind_ == FRODO) return cb200_frodo640shake_encapsulation_seed_size();
     return kind_ == XWING ? 64 : kind_ == HYBRID ? cb200_hybrid_encapsulation_seed_size(k_) : 32;
   }
@@ -158,7 +199,7 @@ class Scheme {
   }
   PrivateKey UnmarshalBinaryPrivateKey(const Bytes& buf) const {  // kyber.go:398-407
     if (buf.size() != PrivateKeySize()) throw ErrPrivKeySize();
-    if (p256() && !p256_scalar_ok(buf)) throw ErrInvalidKEMPrivateKey();  // shortkem.go:103-113
+    if (nist() && !nist_scalar_ok(buf)) throw ErrInvalidKEMPrivateKey();  // shortkem.go:103-113
     return PrivateKey(this, buf);
   }
   // (ct, ss)
@@ -204,7 +245,7 @@ class Scheme {
       case XWING: check(cb200_xwing_encaps(eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)); break;
       case HYBRID: check(cb200_hybrid_encaps(k_, eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)); break;
       case HPKE:
-        check(p256() ? cb200_hpke_p256_encaps(eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)
+        check(nist() ? nist()->encaps(eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n)
                      : cb200_hpke_encaps(k_, eks.data(), stride, seeds.data(), cts.data(), sss.data(), nullptr, n));
         break;
       case FRODO: check(cb200_frodo640shake_encaps(eks.data(), stride, seeds.data(), cts.data(), sss.data(), n)); break;
@@ -233,7 +274,7 @@ class Scheme {
         break;
       }
       case HPKE:
-        check(p256() ? cb200_hpke_p256_decaps(dks.data(), stride, cts.data(), sss.data(), nullptr, n)
+        check(nist() ? nist()->decaps(dks.data(), stride, cts.data(), sss.data(), nullptr, n)
                      : cb200_hpke_decaps(k_, dks.data(), stride, cts.data(), sss.data(), nullptr, n));
         break;
       case FRODO: check(cb200_frodo640shake_decaps(dks.data(), stride, cts.data(), sss.data(), n)); break;
@@ -253,7 +294,7 @@ class Scheme {
         break;
       case HYBRID: check(cb200_hybrid_keygen(k_, seeds.data(), eks.data(), dks.data(), n)); break;
       case HPKE:
-        check(p256() ? cb200_hpke_p256_keygen(seeds.data(), eks.data(), dks.data(), n)
+        check(nist() ? nist()->keygen(seeds.data(), eks.data(), dks.data(), n)
                      : cb200_hpke_keygen(k_, seeds.data(), eks.data(), dks.data(), n));
         break;
       case FRODO: check(cb200_frodo640shake_keygen(seeds.data(), eks.data(), dks.data(), n)); break;
@@ -289,7 +330,7 @@ class Scheme {
     const size_t ps = key_stride(pkrs, n, PublicKeySize(), ErrPubKeySize()), ss = key_stride(skss, n, PrivateKeySize(), ErrPrivKeySize());
     cts.resize(n * CiphertextSize());
     sss.resize(n * SharedKeySize());
-    check(p256() ? cb200_hpke_p256_auth_encaps(pkrs.data(), ps, skss.data(), ss, seeds.data(), cts.data(), sss.data(), nullptr, n)
+    check(nist() ? nist()->auth_encaps(pkrs.data(), ps, skss.data(), ss, seeds.data(), cts.data(), sss.data(), nullptr, n)
                  : cb200_hpke_auth_encaps(k_, pkrs.data(), ps, skss.data(), ss, seeds.data(), cts.data(), sss.data(), nullptr, n));
   }
   void AuthDecapsulateBatch(const Bytes& skrs, const Bytes& cts, const Bytes& pkss, Bytes& sss) const {
@@ -297,19 +338,21 @@ class Scheme {
     const size_t n = rows(cts, CiphertextSize(), ErrPubKeySize());
     const size_t ss = key_stride(skrs, n, PrivateKeySize(), ErrPrivKeySize()), ps = key_stride(pkss, n, PublicKeySize(), ErrPubKeySize());
     sss.resize(n * SharedKeySize());
-    check(p256() ? cb200_hpke_p256_auth_decaps(skrs.data(), ss, cts.data(), pkss.data(), ps, sss.data(), nullptr, n)
+    check(nist() ? nist()->auth_decaps(skrs.data(), ss, cts.data(), pkss.data(), ps, sss.data(), nullptr, n)
                  : cb200_hpke_auth_decaps(k_, skrs.data(), ss, cts.data(), pkss.data(), ps, sss.data(), nullptr, n));
   }
   int k() const { return k_; }
   Kind kind() const { return kind_; }
   // DHKEM(P-256, HKDF-SHA256): an HPKE scheme on the cb200_hpke_p256_* entry points (kem::p256::All())
   bool p256() const { return kind_ == HPKE && k_ == CB200_HPKE_P256_HKDF_SHA256; }
+  // a NIST DHKEM (P-256, P-384 or P-521; kem::p256 / p384 / p521::All()): its entry points, else nullptr
+  const NistOps* nist() const { return kind_ == HPKE ? nist_ops(k_) : nullptr; }
 
  private:
-  static bool p256_scalar_ok(const Bytes& k) {  // 0 < k < n, big-endian (crypto/ecdh NewPrivateKey)
-    static const uint8_t n[32] = {0xff, 0xff, 0xff, 0xff, 0x00, 0x00, 0x00, 0x00, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
-                                  0xbc, 0xe6, 0xfa, 0xad, 0xa7, 0x17, 0x9e, 0x84, 0xf3, 0xb9, 0xca, 0xc2, 0xfc, 0x63, 0x25, 0x51};
-    return std::any_of(k.begin(), k.end(), [](uint8_t b) { return b != 0; }) && std::lexicographical_compare(k.begin(), k.end(), n, n + 32);
+  bool nist_scalar_ok(const Bytes& k) const {  // 0 < k < n, big-endian (crypto/ecdh NewPrivateKey)
+    const uint8_t* n = nist()->n;
+    return std::any_of(k.begin(), k.end(), [](uint8_t b) { return b != 0; }) &&
+           std::lexicographical_compare(k.begin(), k.end(), n, n + k.size());
   }
   void auth_only() const {
     if (kind_ != HPKE) throw std::logic_error("kem: " + name_ + " is not a kem.AuthScheme");
@@ -327,8 +370,8 @@ class Scheme {
   }
   void check(int rc) const {
     if (rc == 0) return;
-    if (rc == CB200_ERR_PUBKEY && p256()) throw ErrInvalidKEMPublicKey();
-    if (rc == CB200_ERR_PRIVKEY && p256()) throw ErrInvalidKEMPrivateKey();
+    if (rc == CB200_ERR_PUBKEY && nist()) throw ErrInvalidKEMPublicKey();
+    if (rc == CB200_ERR_PRIVKEY && nist()) throw ErrInvalidKEMPrivateKey();
     if (rc == CB200_ERR_PUBKEY && kind_ == HPKE) throw ErrInvalidKEMSharedSecret();
     if (rc == CB200_ERR_PUBKEY) throw ErrPubKey();
     if (rc == CB200_ERR_PRIVKEY) throw ErrPrivKey();
@@ -344,7 +387,7 @@ inline PublicKey PrivateKey::Public() const {
   const Scheme* s = scheme_;
   if (s->kind() == Scheme::HPKE) {  // KeyGen of the stored (unclamped) key (xkem.go:146-163, shortkem.go:151-157)
     Bytes pk(s->PublicKeySize());
-    if ((s->p256() ? cb200_p256 : pk.size() == 56 ? cb200_x448 : cb200_x25519)(packed_.data(), nullptr, pk.data(), nullptr, 1))
+    if ((s->nist() ? s->nist()->ecdh : pk.size() == 56 ? cb200_x448 : cb200_x25519)(packed_.data(), nullptr, pk.data(), nullptr, 1))
       throw Error(cb200_last_error());
     return PublicKey(s, std::move(pk));
   }
@@ -372,7 +415,7 @@ inline PublicKey PrivateKey::Public() const {
 }
 
 inline std::pair<PublicKey, PrivateKey> Scheme::GenerateKeyPair() const {
-  if (kind_ != HPKE || p256()) return GenerateFromSeed();  // P-256: a uniform key in [1, n - 1] from DeriveKeyPair
+  if (kind_ != HPKE || nist()) return GenerateFromSeed();  // NIST curves: a uniform key in [1, n - 1] from DeriveKeyPair
   Bytes sk(PrivateKeySize());
   fill_random(sk.data(), sk.size());
   PrivateKey priv(this, std::move(sk));
@@ -431,6 +474,33 @@ inline const Scheme* ByName(const std::string& name) {  // case-insensitive; nul
   return nullptr;
 }
 }  // namespace p256
+
+// DHKEM(P-384, HKDF-SHA384) and DHKEM(P-521, HKDF-SHA512) (kem/schemes/schemes.go), registered like P-256's and with
+// its checks.
+namespace p384 {
+inline const std::vector<const Scheme*>& All() {
+  static const Scheme s("HPKE_KEM_P384_HKDF_SHA384", Scheme::HPKE, CB200_HPKE_P384_HKDF_SHA384);
+  static const std::vector<const Scheme*> all = {&s};
+  return all;
+}
+inline const Scheme* ByName(const std::string& name) {  // case-insensitive; nullptr = no such scheme
+  for (const Scheme* s : All())
+    if (lower(s->Name()) == lower(name)) return s;
+  return nullptr;
+}
+}  // namespace p384
+namespace p521 {
+inline const std::vector<const Scheme*>& All() {
+  static const Scheme s("HPKE_KEM_P521_HKDF_SHA512", Scheme::HPKE, CB200_HPKE_P521_HKDF_SHA512);
+  static const std::vector<const Scheme*> all = {&s};
+  return all;
+}
+inline const Scheme* ByName(const std::string& name) {  // case-insensitive; nullptr = no such scheme
+  for (const Scheme* s : All())
+    if (lower(s->Name()) == lower(name)) return s;
+  return nullptr;
+}
+}  // namespace p521
 
 // FrodoKEM-640-SHAKE (kem/schemes/schemes.go entry 6), registered on its own like the HPKE DHKEMs.
 namespace frodo {

@@ -285,14 +285,9 @@ def frodo_lines(res):
     torch.cuda.empty_cache()
 
 
-def p256_lines(res):
-    """P-256 raw KeyGen / Shared and DHKEM(P-256, HKDF-SHA256) through the C ABI, device-resident, 2^16 operations, per-op
-    and shared keys, with X25519 KeyGen / Shared of the same run beside them; the card and its power limit; and the
-    time of the curve kernels (profiling class p256) and of the KDF kernels (class hpke) for every DHKEM line, read in
-    a separate profiled call."""
-    import ctypes as C
+def _nist_setup(res):
+    """The library on torch's stream, and the card and its power limit into res."""
     import subprocess
-    from circl_b200 import hybrid
     from circl_b200._ffi import check, lib
     L = lib()
     check(L.cb200_set_stream(torch.cuda.current_stream().cuda_stream))
@@ -302,75 +297,107 @@ def p256_lines(res):
         res["card"] = q[0] if q else "unknown"
     except (OSError, subprocess.SubprocessError):
         res["card"] = "unknown"
-    n = 1 << 16
-    g = torch.Generator(device="cuda").manual_seed(17)
+    return L
+
+
+def _split_ms(L, fn, c):
+    """(ms of kernel class c, ms of class hpke) of one call of fn, with per-kernel event timing on."""
+    import ctypes as C
+    from circl_b200._ffi import check
     names = L.cb200_profile_kernel_count()
     kn = [L.cb200_profile_kernel_name(i).decode() for i in range(names)]
-    pk_id, hk_id = kn.index("p256"), kn.index("hpke")
+    check(L.cb200_profile_enable(1))
+    fn()
+    torch.cuda.synchronize()
+    ms = (C.c_double * names)()
+    cnt = (C.c_uint64 * names)()
+    check(L.cb200_profile_read(ms, cnt, names))
+    check(L.cb200_profile_enable(0))
+    return ms[kn.index(c)], ms[kn.index("hpke")]
 
-    def split_ms(fn):
-        """(p256 kernel ms, hpke kernel ms) of one call, with per-kernel event timing on."""
-        check(L.cb200_profile_enable(1))
-        fn()
-        torch.cuda.synchronize()
-        ms = (C.c_double * names)()
-        cnt = (C.c_uint64 * names)()
-        check(L.cb200_profile_read(ms, cnt, names))
-        check(L.cb200_profile_enable(0))
-        return ms[pk_id], ms[hk_id]
 
+def p256_lines(res):
+    """P-256 raw KeyGen / Shared and DHKEM(P-256, HKDF-SHA256) through the C ABI, device-resident, 2^16 operations, per-op
+    and shared keys, with X25519 KeyGen / Shared of the same run beside them; the card and its power limit; and the
+    time of the curve kernels (profiling class p256) and of the KDF kernels (class hpke) for every DHKEM line, read in
+    a separate profiled call."""
+    from circl_b200 import hybrid
+    L = _nist_setup(res)
+    n = 1 << 16
+    g = torch.Generator(device="cuda").manual_seed(17)
     k = torch.randint(0, 256, (n, 32), generator=g, device="cuda", dtype=torch.uint8)
     t = timed(lambda: hybrid.x25519_keygen(k), steps=3)
     res["X25519 KeyGen"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
     pub = hybrid.x25519_keygen(k)
     t = timed(lambda: hybrid.x25519_shared(k, pub), steps=3)
     res["X25519 Shared"] = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
-    del pub
+    del pub, k
+    torch.cuda.empty_cache()
+    nist_lines(res, L, "p256", 32, 32, "P-256", "DHKEM(P-256, HKDF-SHA256)", n, g)
+
+
+def nist_lines(res, L, c, B, nss, curve, name, n, g):
+    """Raw KeyGen / Shared and every DHKEM line of one NIST curve (entry points cb200_<c> and cb200_hpke_<c>_*, B-byte
+    scalars, nss-byte shared secrets), each with the time of its curve kernels (<c>_ms) and KDF kernels (hpke_ms)."""
+    from circl_b200._ffi import check
+    W = 1 + 2 * B
     P = lambda x: x.data_ptr()  # noqa: E731
-    seeds = torch.randint(0, 256, (n, 32), generator=g, device="cuda", dtype=torch.uint8)
-    es = torch.randint(0, 256, (n, 32), generator=g, device="cuda", dtype=torch.uint8)
-    pk = torch.empty((n, 65), dtype=torch.uint8, device="cuda")
-    sk = torch.empty((n, 32), dtype=torch.uint8, device="cuda")
-    enc = torch.empty((n, 65), dtype=torch.uint8, device="cuda")
-    ss = torch.empty((n, 32), dtype=torch.uint8, device="cuda")
-    ss2 = torch.empty((n, 32), dtype=torch.uint8, device="cuda")
+    H = lambda op: getattr(L, f"cb200_hpke_{c}_{op}")  # noqa: E731
+    seeds = torch.randint(0, 256, (n, B), generator=g, device="cuda", dtype=torch.uint8)
+    es = torch.randint(0, 256, (n, B), generator=g, device="cuda", dtype=torch.uint8)
+    pk = torch.empty((n, W), dtype=torch.uint8, device="cuda")
+    sk = torch.empty((n, B), dtype=torch.uint8, device="cuda")
+    enc = torch.empty((n, W), dtype=torch.uint8, device="cuda")
+    ss = torch.empty((n, nss), dtype=torch.uint8, device="cuda")
+    ss2 = torch.empty((n, nss), dtype=torch.uint8, device="cuda")
     st = torch.zeros((n,), dtype=torch.uint8, device="cuda")
-    check(L.cb200_hpke_p256_keygen(P(seeds), P(pk), P(sk), n))  # valid scalars and points for the raw lines
-    raw = torch.empty((n, 65), dtype=torch.uint8, device="cuda")
+    check(H("keygen")(P(seeds), P(pk), P(sk), n))  # valid scalars and points for the raw lines
+    raw = torch.empty((n, W), dtype=torch.uint8, device="cuda")
+    ecdh = getattr(L, f"cb200_{c}")
     ops = {
-        "P-256 KeyGen": lambda: check(L.cb200_p256(P(sk), None, P(raw), P(st), n)),
-        "P-256 Shared": lambda: check(L.cb200_p256(P(sk), P(pk), P(raw), P(st), n)),
+        f"{curve} KeyGen": lambda: check(ecdh(P(sk), None, P(raw), P(st), n)),
+        f"{curve} Shared": lambda: check(ecdh(P(sk), P(pk), P(raw), P(st), n)),
+        f"{name} KeyGen": lambda: check(H("keygen")(P(seeds), P(pk), P(sk), n)),
+        f"{name} Encaps": lambda: check(H("encaps")(P(pk), W, P(es), P(enc), P(ss), P(st), n)),
+        f"{name} Decaps": lambda: check(H("decaps")(P(sk), B, P(enc), P(ss2), P(st), n)),
+        f"{name} Encaps (shared pkR)": lambda: check(H("encaps")(P(pk), 0, P(es), P(enc), P(ss), P(st), n)),
+        f"{name} Decaps (shared skR)": lambda: check(H("decaps")(P(sk), 0, P(enc), P(ss2), P(st), n)),
+        f"{name} AuthEncaps": lambda: check(H("auth_encaps")(P(pk), W, P(sk), B, P(es), P(enc), P(ss), P(st), n)),
+        f"{name} AuthDecaps": lambda: check(H("auth_decaps")(P(sk), B, P(enc), P(pk), W, P(ss2), P(st), n)),
+        f"{name} AuthEncaps (shared pkR, skS)": lambda: check(H("auth_encaps")(P(pk), 0, P(sk), 0, P(es), P(enc), P(ss),
+                                                                                 P(st), n)),
+        f"{name} AuthDecaps (shared skR, pkS)": lambda: check(H("auth_decaps")(P(sk), 0, P(enc), P(pk), 0, P(ss2), P(st),
+                                                                                 n)),
     }
-    name = "DHKEM(P-256, HKDF-SHA256)"
-    ops.update({
-        f"{name} KeyGen": lambda: check(L.cb200_hpke_p256_keygen(P(seeds), P(pk), P(sk), n)),
-        f"{name} Encaps": lambda: check(L.cb200_hpke_p256_encaps(P(pk), 65, P(es), P(enc), P(ss), P(st), n)),
-        f"{name} Decaps": lambda: check(L.cb200_hpke_p256_decaps(P(sk), 32, P(enc), P(ss2), P(st), n)),
-        f"{name} Encaps (shared pkR)": lambda: check(L.cb200_hpke_p256_encaps(P(pk), 0, P(es), P(enc), P(ss), P(st), n)),
-        f"{name} Decaps (shared skR)": lambda: check(L.cb200_hpke_p256_decaps(P(sk), 0, P(enc), P(ss2), P(st), n)),
-        f"{name} AuthEncaps": lambda: check(L.cb200_hpke_p256_auth_encaps(P(pk), 65, P(sk), 32, P(es), P(enc), P(ss),
-                                                                          P(st), n)),
-        f"{name} AuthDecaps": lambda: check(L.cb200_hpke_p256_auth_decaps(P(sk), 32, P(enc), P(pk), 65, P(ss2), P(st),
-                                                                          n)),
-        f"{name} AuthEncaps (shared pkR, skS)": lambda: check(L.cb200_hpke_p256_auth_encaps(P(pk), 0, P(sk), 0, P(es),
-                                                                                            P(enc), P(ss), P(st), n)),
-        f"{name} AuthDecaps (shared skR, pkS)": lambda: check(L.cb200_hpke_p256_auth_decaps(P(sk), 0, P(enc), P(pk), 0,
-                                                                                            P(ss2), P(st), n)),
-    })
     for op, fn in ops.items():
         t = timed(fn, steps=3)
         line = {"n": n, "ms": t, "per_s": n / (t * 1e-3)}
-        line["p256_ms"], line["hpke_ms"] = split_ms(fn)
+        line[f"{c}_ms"], line["hpke_ms"] = _split_ms(L, fn, c)
         if "Decaps" in op:
             torch.cuda.synchronize()
             line["roundtrip_ok"] = bool(torch.equal(ss, ss2)) and st.sum().item() == 0
         res[op] = line
-    del k, seeds, es, pk, sk, enc, ss, ss2, st, raw
+    del seeds, es, pk, sk, enc, ss, ss2, st, raw
     torch.cuda.empty_cache()
+
+
+def nist_extra_lines(res):
+    """The lines of nist_lines for P-384 and P-521 (2^14 operations each), with the card and its power limit."""
+    L = _nist_setup(res)
+    g = torch.Generator(device="cuda").manual_seed(19)
+    n = 1 << 14
+    nist_lines(res, L, "p384", 48, 48, "P-384", "DHKEM(P-384, HKDF-SHA384)", n, g)
+    nist_lines(res, L, "p521", 66, 64, "P-521", "DHKEM(P-521, HKDF-SHA512)", n, g)
 
 
 if "--p256" in sys.argv:  # only the P-256 lines above and the X25519 lines they are compared with
     p256_lines(res)
+    print(json.dumps(res, indent=1))
+    sys.exit(0)
+
+
+if "--nistp" in sys.argv:  # only the P-384 and P-521 lines
+    nist_extra_lines(res)
     print(json.dumps(res, indent=1))
     sys.exit(0)
 
