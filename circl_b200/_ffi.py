@@ -112,6 +112,16 @@ SYMBOLS = {
     "cb200_hpke_p256_seed_size": (C.c_size_t, []),
     "cb200_hpke_p256_encapsulation_seed_size": (C.c_size_t, []),
     "cb200_p384": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_oprf_element_size": (C.c_size_t, [C.c_int]),
+    "cb200_oprf_scalar_size": (C.c_size_t, [C.c_int]),
+    "cb200_oprf_output_size": (C.c_size_t, [C.c_int]),
+    "cb200_oprf_proof_size": (C.c_size_t, [C.c_int]),
+    "cb200_oprf_derive_key": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                        C.c_size_t]),
+    "cb200_oprf_evaluate": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                      C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_oprf_full_evaluate": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_hpke_p384_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_hpke_p384_encaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_size_t]),

@@ -41,6 +41,21 @@ struct P256 {
                             0x7c0f9e16u, 0x8ee7eb4au, 0xfe1a7f9bu, 0x4fe342e2u};
     return w[i];
   }
+  // for oprf.cuh: R^2 mod n, and the SSWU map's Z = -10 and c2 = sqrt(-Z) (RFC 9380 F.2) times R mod p
+  CB200_XHD static uint32_t rn2(int i) {
+    const uint32_t w[kW] = {0xbe79eea2u, 0x83244c95u, 0x49bd6fa6u, 0x4699799cu,
+                            0x2b6bec59u, 0x2845b239u, 0xf3d95620u, 0x66e12d94u};
+    return w[i];
+  }
+  CB200_XHD static uint32_t sswu_z(int i) {
+    const uint32_t w[kW] = {0xfffffff5u, 0xffffffffu, 0xffffffffu, 0x0000000au, 0u, 0u, 0x0000000bu, 0xfffffff5u};
+    return w[i];
+  }
+  CB200_XHD static uint32_t sswu_c2(int i) {
+    const uint32_t w[kW] = {0x98a195fdu, 0xa1fd38eeu, 0x423dcf70u, 0x78400ad7u,
+                            0x9ea8dfeeu, 0x6913c88fu, 0x12a8f304u, 0x9051d26eu};
+    return w[i];
+  }
   // h = f^(p - 2).  p - 2 = 2^256 - 2^224 + 2^192 + 2^96 - 3: the words of p - 2 from the top are
   // ffffffff 00000001 00000000 00000000 00000000 ffffffff ffffffff fffffffd; x_k below is f^(2^k - 1).
   CB200_NISTP_NOINLINE void invert(Fe<P256>& h, const Fe<P256>& f) {

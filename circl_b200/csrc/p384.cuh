@@ -43,6 +43,22 @@ struct P384 {
                             0x289a147cu, 0xf8f41dbdu, 0x9292dc29u, 0x5d9e98bfu, 0x96262c6fu, 0x3617de4au};
     return w[i];
   }
+  // for oprf.cuh: R^2 mod n, and the SSWU map's Z = -12 and c2 = sqrt(-Z) (RFC 9380 F.2) times R mod p
+  CB200_XHD static uint32_t rn2(int i) {
+    const uint32_t w[kW] = {0x19b409a9u, 0x2d319b24u, 0xdf1aa419u, 0xff3d81e5u, 0xfcb82947u, 0xbc3e483au,
+                            0x4aab1cc5u, 0xd40d4917u, 0x28266895u, 0x3fb05b7au, 0x2b39bf21u, 0x0c84ee01u};
+    return w[i];
+  }
+  CB200_XHD static uint32_t sswu_z(int i) {
+    const uint32_t w[kW] = {0xfffffff3u, 0x0000000cu, 0u, 0xfffffff3u, 0xfffffff2u, 0xffffffffu,
+                            0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu};
+    return w[i];
+  }
+  CB200_XHD static uint32_t sswu_c2(int i) {
+    const uint32_t w[kW] = {0xc0a3f1f8u, 0x1cdf6f1cu, 0x4c08f647u, 0xfdf2313bu, 0xd4183d32u, 0x89cb6776u,
+                            0x476b11b6u, 0xacb3a761u, 0xc093fceau, 0xe428a383u, 0x3ae40b98u, 0xd78fa36bu};
+    return w[i];
+  }
   // h = f^(p - 2).  The bits of p - 2 from the top: 255 ones, a zero, 32 ones, 64 zeros, 30 ones, 0, 1 (words
   // ffffffff x 7, fffffffe, ffffffff, 00000000, 00000000, fffffffd); x_k below is f^(2^k - 1).
   CB200_NISTP_NOINLINE void invert(Fe<P384>& h, const Fe<P384>& f) {

@@ -38,6 +38,15 @@ struct P521 {
                             0x2c7d1bd9u, 0x5c8a5fb4u, 0x9a3bc004u, 0x39296a78u, 0x118u};
     return w[i];
   }
+  // for oprf.cuh: R^2 mod n, and the SSWU map's Z = -4 and c2 = sqrt(-Z) = 2 (RFC 9380 F.2) times R mod p
+  CB200_XHD static uint32_t rn2(int i) {
+    const uint32_t w[kW] = {0x61c64ca7u, 0x1163115au, 0x4374a642u, 0x18354a56u, 0x0791d9dcu, 0x5d4dd6d3u,
+                            0xd3402705u, 0x4fb35b72u, 0xb7756e3au, 0xcff3d142u, 0xa8e567bcu, 0x5bcc6d61u,
+                            0x492d0d45u, 0x2d8e03d1u, 0x8c44383du, 0x5b5a3afeu, 0x19au};
+    return w[i];
+  }
+  CB200_XHD static uint32_t sswu_z(int i) { return i == 0 ? 0xfdffffffu : i < 16 ? 0xffffffffu : 0x1ffu; }
+  CB200_XHD static uint32_t sswu_c2(int i) { return i == 0 ? 0x01000000u : 0u; }
   // h = f^(p - 2).  p - 2 = 2^521 - 3: 519 ones, then 0, 1; x_k below is f^(2^k - 1).
   CB200_NISTP_NOINLINE void invert(Fe<P521>& h, const Fe<P521>& f) {
     Fe<P521> x2, x3, x4, x7, t;

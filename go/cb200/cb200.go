@@ -945,3 +945,112 @@ func KyberDeriveUniform(polys [][256]int16, seeds []byte, xy []byte) error {
 			stride, (*C.uint8_t)(unsafe.Pointer(&xy[0])), C.size_t(n))
 	})
 }
+
+// ---- OPRF servers (RFC 9497, the reference's oprf package) over P-256, P-384 and P-521
+
+// Suite ids of cb200_oprf_* (include/circl_b200.h).
+const (
+	OPRFP256SHA256 = int(C.CB200_OPRF_P256_SHA256)
+	OPRFP384SHA384 = int(C.CB200_OPRF_P384_SHA384)
+	OPRFP521SHA512 = int(C.CB200_OPRF_P521_SHA512)
+)
+
+// OPRFSizes returns (Ne, Ns, Nh, proof size) of a suite.
+func OPRFSizes(suite int) (ne, ns, nh, proof int) {
+	s := C.int(suite)
+	return int(C.cb200_oprf_element_size(s)), int(C.cb200_oprf_scalar_size(s)), int(C.cb200_oprf_output_size(s)),
+		int(C.cb200_oprf_proof_size(s))
+}
+
+// oprfSizes is OPRFSizes for a suite the library serves (an unknown suite panics, as a wrong length does)
+func oprfSizes(suite int) (ne, ns, nh, proof int) {
+	ne, ns, nh, proof = OPRFSizes(suite)
+	if ne == 0 {
+		panic("cb200: unknown OPRF suite")
+	}
+	return
+}
+
+// oprfKeyLen is the length of the sk argument: one key (shared) or one per op
+func oprfKeyLen(ns, n int, shared bool) int {
+	if shared {
+		return ns
+	}
+	return n * ns
+}
+
+func optPtr(b []byte) *C.uint8_t {
+	if len(b) == 0 {
+		return nil
+	}
+	return u8(b)
+}
+
+// OPRFDeriveKey: oprf.DeriveKey (oprf/keys.go:103-132) on n 32-byte seeds with one info; sk receives n*Ns bytes, pk
+// n*Ne (compressed).  A buffer of the wrong length or an unknown suite panics.
+func OPRFDeriveKey(suite, mode int, seeds, info, sk, pk []byte) error {
+	ne, ns, _, _ := oprfSizes(suite)
+	n := len(seeds) / 32
+	if len(seeds) != n*32 || len(sk) != n*ns || len(pk) != n*ne {
+		panic("cb200: OPRFDeriveKey seeds/sk/pk have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return call(func() C.int {
+		return C.cb200_oprf_derive_key(C.int(suite), C.int(mode), u8(seeds), optPtr(info), C.size_t(len(info)), u8(sk),
+			u8(pk), C.size_t(n))
+	})
+}
+
+// OPRFEvaluate: Server / VerifiableServer / PartialObliviousServer.Evaluate (oprf/server.go:23-85) on n requests of
+// m blinded elements each (n*m*Ne bytes).  sk holds one key (shared) or n; rnd n*Ns bytes of proof randomness (modes 1
+// and 2).  evaluated receives n*m*Ne bytes, proof n*2*Ns (modes 1 and 2), status one byte per request (0 = ok; the
+// failed requests' rows are zero).  A buffer of the wrong length, 1 <= m <= 65535 unmet or an unknown suite panics.
+func OPRFEvaluate(suite, mode int, sk []byte, shared bool, blinded []byte, m int, rnd, info, evaluated, proof,
+	status []byte) error {
+	ne, ns, _, np := oprfSizes(suite)
+	n := len(status)
+	if m < 1 || m > 65535 || len(sk) != oprfKeyLen(ns, n, shared) || len(blinded) != n*m*ne ||
+		len(evaluated) != n*m*ne || (mode != 0 && (len(rnd) != n*ns || len(proof) != n*np)) {
+		panic("cb200: OPRFEvaluate buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	stride := C.size_t(ns)
+	if shared {
+		stride = 0
+	}
+	var rp, pp *C.uint8_t // mode 0 reads no randomness and writes no proof
+	if mode != 0 {
+		rp, pp = u8(rnd), u8(proof)
+	}
+	return call(func() C.int {
+		return C.cb200_oprf_evaluate(C.int(suite), C.int(mode), u8(sk), stride, u8(blinded), C.size_t(m), rp,
+			optPtr(info), C.size_t(len(info)), u8(evaluated), pp, u8(status), C.size_t(n))
+	})
+}
+
+// OPRFFullEvaluate: the servers' FullEvaluate (oprf/server.go:97-117) on len(inputs) inputs of at most 65535 bytes;
+// sk holds Ns bytes (shared) or len(inputs)*Ns; out receives len(inputs)*Nh bytes, status one byte per op.  A buffer of
+// the wrong length or an unknown suite panics.
+func OPRFFullEvaluate(suite, mode int, sk []byte, shared bool, inputs [][]byte, info, out, status []byte) error {
+	_, ns, nh, _ := oprfSizes(suite)
+	n := len(inputs)
+	if len(sk) != oprfKeyLen(ns, n, shared) || len(out) != n*nh || len(status) != n {
+		panic("cb200: OPRFFullEvaluate buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	blob, off := packMsgs(inputs)
+	stride := C.size_t(ns)
+	if shared {
+		stride = 0
+	}
+	return call(func() C.int {
+		return C.cb200_oprf_full_evaluate(C.int(suite), C.int(mode), u8(sk), stride, u8(blob),
+			(*C.uint64_t)(unsafe.Pointer(&off[0])), optPtr(info), C.size_t(len(info)), u8(out), u8(status), C.size_t(n))
+	})
+}

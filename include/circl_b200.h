@@ -331,6 +331,41 @@ size_t cb200_hpke_p256_shared_key_size(void);             /* 32 */
 size_t cb200_hpke_p256_seed_size(void);                   /* 32 */
 size_t cb200_hpke_p256_encapsulation_seed_size(void);     /* 32 */
 
+/* ---- OPRF servers (RFC 9497) over the NIST curves: the reference's oprf package (oprf/oprf.go, server.go, keys.go,
+ * zk/dleq/dleq.go:84-243, group/short.go:100-135,246-283,404-470, expander/expander.go) ----
+ * suite: one of the ids below (the suite ids of the CFRG drafts); mode: 0 (Server), 1 (VerifiableServer) or 2
+ * (PartialObliviousServer).  Elements are compressed points (0x02 | 0x03 || X, Ne bytes), scalars Ns big-endian bytes.
+ * An unknown suite or mode, an info longer than 65535 bytes (oprf.ErrInvalidInfo) or a null required pointer is
+ * CB200_ERR_ARG.  Key rows have a stride (0 = one key for the batch).  Rows of device buffers may start at any byte.
+ * status (required, one byte per op, all-zero outputs on failure): 1 = a blinded element does not decode
+ * (group.UnmarshalBinary), 2 = sk not in [1, n - 1] (oprf.ErrInvalidPrivateKey), 4 = r not in [1, n - 1], 8 = mode 2
+ * with t = sk + HashToScalar(info) = 0 (oprf.ErrInverseZero), 16 = a FullEvaluate input over 65535 bytes on a
+ * device-pointer call.  The call itself returns 0. */
+#define CB200_OPRF_P256_SHA256 3 /* Ne 33, Ns 32, Nh 32, proof 64 */
+#define CB200_OPRF_P384_SHA384 4 /* Ne 49, Ns 48, Nh 48, proof 96 */
+#define CB200_OPRF_P521_SHA512 5 /* Ne 67, Ns 66, Nh 64, proof 132 */
+size_t cb200_oprf_element_size(int suite); /* Ne; 0 for an unknown suite */
+size_t cb200_oprf_scalar_size(int suite);  /* Ns */
+size_t cb200_oprf_output_size(int suite);  /* Nh */
+size_t cb200_oprf_proof_size(int suite);   /* 2 Ns: c || s */
+/* DeriveKey (keys.go:103-132): 32-byte seeds, one info for the batch -> sk (Ns) and pk = compress([sk]G) (Ne). */
+int cb200_oprf_derive_key(int suite, int mode, const uint8_t *seeds, const uint8_t *info, size_t info_len, uint8_t *sk,
+                          uint8_t *pk, size_t n);
+/* Evaluate (server.go:23-85): n requests of m blinded elements each (1 <= m <= 65535, n * m rows of Ne) -> evaluated
+ * (n * m rows of Ne) and, in modes 1 and 2, one proof per request (2 Ns) from the randomness rnd (one Ns row per
+ * request, the reference's rand.Reader draw; rnd and proof are ignored in mode 0).  info: mode 2 only. */
+int cb200_oprf_evaluate(int suite, int mode, const uint8_t *sk, size_t sk_stride, const uint8_t *blinded, size_t m,
+                        const uint8_t *rnd, const uint8_t *info, size_t info_len, uint8_t *evaluated, uint8_t *proof,
+                        uint8_t *status, size_t n);
+/* FullEvaluate (server.go:97-117): input i is msgs[msg_off[i] .. msg_off[i + 1]) -> out (Nh).  Inputs are limited to
+ * 65535 bytes as RFC 9497 bounds them (the reference silently truncates the length prefix instead): a host-pointer
+ * call refuses a longer one with CB200_ERR_ARG before any device work; on a device-pointer call, whose offsets the
+ * host does not read, that op gets status bit 16 and an all-zero output.  info: mode 2 only.
+ * VerifyFinalize is this call followed by a constant-time compare. */
+int cb200_oprf_full_evaluate(int suite, int mode, const uint8_t *sk, size_t sk_stride, const uint8_t *msgs,
+                             const uint64_t *msg_off, const uint8_t *info, size_t info_len, uint8_t *out,
+                             uint8_t *status, size_t n);
+
 /* ---- P-384 and P-521 ECDH (crypto/ecdh.P384() / P521()) ----
  * cb200_p384 / cb200_p521: the contract of cb200_p256 with 48-byte scalars and Shared outputs and 97-byte points and
  * KeyGen outputs (P-384), or 66 and 133 bytes (P-521).  A 66-byte P-521 scalar whose leading byte is above 0x01 is

@@ -746,4 +746,213 @@ inline const Scheme* ByName(const std::string& name) {  // case-insensitive; nul
 }  // namespace ed448
 
 }  // namespace sign
+
+// ---------------------------------------------------------------- oprf: RFC 9497 servers (oprf/{oprf,server,keys}.go)
+// The suites P256-SHA256, P384-SHA384 and P521-SHA512; Server, VerifiableServer and PartialObliviousServer with
+// Evaluate, FullEvaluate, VerifyFinalize and PublicKey, plus batch forms on host rows.  The proof randomness
+// of Evaluate comes from fill_random (the reference's rand.Reader) unless the batch form is given rows of it.
+namespace oprf {
+enum Mode : int { BaseMode = 0, VerifiableMode = 1, PartialObliviousMode = 2 };
+struct OprfError : Error {
+  std::vector<uint8_t> status;  // per-op bits of a failed batch: 1 element, 2 key, 4 r, 8 t = 0, 16 input length
+  explicit OprfError(const std::string& m, std::vector<uint8_t> st = {}) : Error(m), status(std::move(st)) {}
+};
+#define CIRCL_OPRF_ERROR(name, text) \
+  struct name : OprfError {          \
+    explicit name(std::vector<uint8_t> st = {}) : OprfError(text, std::move(st)) {} \
+  };
+CIRCL_OPRF_ERROR(ErrInvalidSuite, "oprf: invalid suite")
+CIRCL_OPRF_ERROR(ErrInvalidMode, "oprf: invalid mode")
+CIRCL_OPRF_ERROR(ErrInvalidSeed, "oprf: invalid seed size")
+CIRCL_OPRF_ERROR(ErrInvalidInfo, "oprf: invalid info")
+CIRCL_OPRF_ERROR(ErrInvalidInput, "oprf: invalid input")
+CIRCL_OPRF_ERROR(ErrInvalidPrivateKey, "oprf: invalid private key")
+CIRCL_OPRF_ERROR(ErrInverseZero, "oprf: inverting a zero value")
+CIRCL_OPRF_ERROR(ErrInvalidRandomness, "oprf: invalid proof randomness")
+#undef CIRCL_OPRF_ERROR
+
+struct Suite {
+  int id;
+  const char* identifier;
+  std::string Identifier() const { return identifier; }
+  size_t Ne() const { return cb200_oprf_element_size(id); }
+  size_t Ns() const { return cb200_oprf_scalar_size(id); }
+  size_t Nh() const { return cb200_oprf_output_size(id); }
+  size_t ProofSize() const { return cb200_oprf_proof_size(id); }
+};
+inline const Suite SuiteP256{CB200_OPRF_P256_SHA256, "P256-SHA256"};
+inline const Suite SuiteP384{CB200_OPRF_P384_SHA384, "P384-SHA384"};
+inline const Suite SuiteP521{CB200_OPRF_P521_SHA512, "P521-SHA512"};
+inline Suite GetSuite(const std::string& identifier) {
+  for (const Suite* s : {&SuiteP256, &SuiteP384, &SuiteP521})
+    if (identifier == s->identifier) return *s;
+  throw ErrInvalidSuite();
+}
+
+namespace detail {
+inline void check_call(int rc) {
+  if (rc == CB200_ERR_ARG) throw std::logic_error(cb200_last_error());
+  if (rc != 0) throw Error(cb200_last_error());
+}
+// the error of the first failure class, as circl_b200.oprf raises it
+inline void check_status(const uint8_t* st, size_t n) {
+  uint8_t any = 0;
+  for (size_t i = 0; i < n; i++) any |= st[i];
+  if (!any) return;
+  std::vector<uint8_t> v(st, st + n);
+  if (any & 2) throw ErrInvalidPrivateKey(v);
+  if (any & 8) throw ErrInverseZero(v);
+  if (any & (1 | 16)) throw ErrInvalidInput(v);
+  throw ErrInvalidRandomness(v);
+}
+inline void check_mode_info(int mode, const Bytes& info) {
+  if (mode < 0 || mode > 2) throw ErrInvalidMode();
+  if (info.size() > 65535) throw ErrInvalidInfo();
+}
+}  // namespace detail
+
+struct PrivateKey {
+  Suite suite;
+  Bytes k, pk;
+  Bytes MarshalBinary() const { return k; }
+  Bytes Public() const { return pk; }
+};
+// DeriveKey (keys.go:103-132)
+inline PrivateKey DeriveKey(const Suite& s, int mode, const Bytes& seed, const Bytes& info = {}) {
+  detail::check_mode_info(mode, info);
+  if (seed.size() != 32) throw ErrInvalidSeed();
+  PrivateKey key{s, Bytes(s.Ns()), Bytes(s.Ne())};
+  detail::check_call(cb200_oprf_derive_key(s.id, mode, seed.data(), info.data(), info.size(), key.k.data(),
+                                           key.pk.data(), 1));
+  return key;
+}
+
+struct Evaluation {
+  std::vector<Bytes> Elements;
+  Bytes Proof;  // c || s; empty in mode 0
+};
+
+class ServerBase {
+ public:
+  ServerBase(Suite s, PrivateKey key, int mode) : s_(s), key_(std::move(key)), mode_(mode) {}
+  Bytes PublicKey() const { return key_.Public(); }
+  // n requests of m elements (n * m rows of Ne at `blinded`), rnd: n rows of Ns (modes 1, 2) -> evaluated (n * m rows
+  // of Ne) and proof (n rows of 2 Ns).  Host buffers (the key and the status bytes are host memory); a failed op raises
+  // after the batch, rows zeroed.
+  void EvaluateBatch(const uint8_t* blinded, size_t m, const uint8_t* rnd, const Bytes& info, uint8_t* evaluated,
+                     uint8_t* proof, size_t n) const {
+    detail::check_mode_info(mode_, info);
+    std::vector<uint8_t> st(n);
+    detail::check_call(cb200_oprf_evaluate(s_.id, mode_, key_.k.data(), 0, blinded, m, rnd, info.data(), info.size(),
+                                           evaluated, proof, st.data(), n));
+    detail::check_status(st.data(), n);
+  }
+  // inputs msgs[off[i] .. off[i + 1]) -> n rows of Nh
+  void FullEvaluateBatch(const uint8_t* msgs, const uint64_t* off, const Bytes& info, uint8_t* out, size_t n) const {
+    detail::check_mode_info(mode_, info);
+    std::vector<uint8_t> st(n);
+    detail::check_call(cb200_oprf_full_evaluate(s_.id, mode_, key_.k.data(), 0, msgs, off, info.data(), info.size(), out,
+                                                st.data(), n));
+    detail::check_status(st.data(), n);
+  }
+
+ protected:
+  Evaluation evaluate(const std::vector<Bytes>& elements, const Bytes& info) const {
+    const size_t Ne = s_.Ne(), Ns = s_.Ns();
+    Bytes b;
+    for (const Bytes& e : elements) {
+      if (e.size() != Ne) throw ErrInvalidInput();
+      b.insert(b.end(), e.begin(), e.end());
+    }
+    if (elements.empty()) throw ErrInvalidInput();
+    Bytes r(Ns), ev(b.size()), proof(mode_ ? 2 * Ns : 0);
+    if (mode_) random_scalar(r);
+    EvaluateBatch(b.data(), elements.size(), mode_ ? r.data() : nullptr, info, ev.data(), mode_ ? proof.data() : nullptr,
+                  1);
+    Evaluation out{{}, proof};
+    for (size_t j = 0; j < elements.size(); j++) out.Elements.emplace_back(ev.begin() + j * Ne, ev.begin() + (j + 1) * Ne);
+    return out;
+  }
+  Bytes full(const Bytes& input, const Bytes& info) const {
+    if (input.size() > 65535) throw ErrInvalidInput();
+    const uint64_t off[2] = {0, input.size()};
+    Bytes out(s_.Nh());
+    const uint8_t zero = 0;
+    FullEvaluateBatch(input.empty() ? &zero : input.data(), off, info, out.data(), 1);
+    return out;
+  }
+  bool verify(const Bytes& input, const Bytes& info, const Bytes& expected) const {
+    Bytes got;
+    try {
+      got = full(input, info);
+    } catch (const OprfError&) {
+      return false;
+    }
+    if (got.size() != expected.size()) return false;
+    uint8_t d = 0;
+    for (size_t i = 0; i < got.size(); i++) d |= got[i] ^ expected[i];
+    return d == 0;
+  }
+  // a uniform r in [1, n - 1]: the leading byte masked to the order's bit length, then rejection against the device's
+  // own range test (an r the call would flag is drawn again)
+  void random_scalar(Bytes& r) const {
+    const uint8_t top = s_.Ns() == 66 ? 0x01 : 0xff;
+    for (;;) {
+      fill_random(r.data(), r.size());
+      r[0] &= top;
+      if (lt_order(r)) return;
+    }
+  }
+  bool lt_order(const Bytes& r) const {
+    static const uint8_t n256[32] = {0xff, 0xff, 0xff, 0xff, 0x00, 0x00, 0x00, 0x00, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
+                                     0xff, 0xff, 0xbc, 0xe6, 0xfa, 0xad, 0xa7, 0x17, 0x9e, 0x84, 0xf3, 0xb9, 0xca, 0xc2,
+                                     0xfc, 0x63, 0x25, 0x51};
+    static const uint8_t n384[48] = {0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
+                                     0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xc7, 0x63, 0x4d, 0x81,
+                                     0xf4, 0x37, 0x2d, 0xdf, 0x58, 0x1a, 0x0d, 0xb2, 0x48, 0xb0, 0xa7, 0x7a, 0xec, 0xec,
+                                     0x19, 0x6a, 0xcc, 0xc5, 0x29, 0x73};
+    static const uint8_t n521[66] = {0x01, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
+                                     0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
+                                     0xff, 0xff, 0xff, 0xff, 0xff, 0xfa, 0x51, 0x86, 0x87, 0x83, 0xbf, 0x2f, 0x96, 0x6b,
+                                     0x7f, 0xcc, 0x01, 0x48, 0xf7, 0x09, 0xa5, 0xd0, 0x3b, 0xb5, 0xc9, 0xb8, 0x89, 0x9c,
+                                     0x47, 0xae, 0xbb, 0x6f, 0xb7, 0x1e, 0x91, 0x38, 0x64, 0x09};
+    const uint8_t* n = r.size() == 32 ? n256 : r.size() == 48 ? n384 : n521;
+    bool nz = false;
+    for (uint8_t v : r) nz |= v != 0;
+    return nz && std::lexicographical_compare(r.begin(), r.end(), n, n + r.size());
+  }
+  Suite s_;
+  PrivateKey key_;
+  int mode_;
+};
+
+class Server : public ServerBase {
+ public:
+  Server(Suite s, PrivateKey key) : ServerBase(s, std::move(key), BaseMode) {}
+  Evaluation Evaluate(const std::vector<Bytes>& elements) const { return evaluate(elements, {}); }
+  Bytes FullEvaluate(const Bytes& input) const { return full(input, {}); }
+  bool VerifyFinalize(const Bytes& input, const Bytes& expected) const { return verify(input, {}, expected); }
+};
+class VerifiableServer : public ServerBase {
+ public:
+  VerifiableServer(Suite s, PrivateKey key) : ServerBase(s, std::move(key), VerifiableMode) {}
+  Evaluation Evaluate(const std::vector<Bytes>& elements) const { return evaluate(elements, {}); }
+  Bytes FullEvaluate(const Bytes& input) const { return full(input, {}); }
+  bool VerifyFinalize(const Bytes& input, const Bytes& expected) const { return verify(input, {}, expected); }
+};
+class PartialObliviousServer : public ServerBase {
+ public:
+  PartialObliviousServer(Suite s, PrivateKey key) : ServerBase(s, std::move(key), PartialObliviousMode) {}
+  Evaluation Evaluate(const std::vector<Bytes>& elements, const Bytes& info) const { return evaluate(elements, info); }
+  Bytes FullEvaluate(const Bytes& input, const Bytes& info) const { return full(input, info); }
+  bool VerifyFinalize(const Bytes& input, const Bytes& info, const Bytes& expected) const {
+    return verify(input, info, expected);
+  }
+};
+inline Server NewServer(const Suite& s, const PrivateKey& k) { return Server(s, k); }
+inline VerifiableServer NewVerifiableServer(const Suite& s, const PrivateKey& k) { return VerifiableServer(s, k); }
+inline PartialObliviousServer NewPartialObliviousServer(const Suite& s, const PrivateKey& k) {
+  return PartialObliviousServer(s, k);
+}
+}  // namespace oprf
 }  // namespace circl
