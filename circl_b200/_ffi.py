@@ -122,6 +122,12 @@ SYMBOLS = {
                                       C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_oprf_full_evaluate": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_brsa_modulus_bytes": (C.c_size_t, [C.c_char_p, C.c_size_t]),
+    "cb200_brsa_blind_sign": (C.c_int, [C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t,
+                                        C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t,
+                                        C.c_char_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
+    "cb200_brsa_verify": (C.c_int, [C.c_int, C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_hpke_p384_keygen": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "cb200_hpke_p384_encaps": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_size_t]),

@@ -1,0 +1,291 @@
+// RSA blind signatures (RFC 9474, RSABSSA-SHA384), server side: BlindSign under one private key and Verify under one
+// public key per call, batched on the device with one thread per operation.  The arithmetic is rsa.cuh:
+//   BlindSign   brsa_sign_kernel<WP, WN>    c^dp mod p and c^dq mod q at WP words, Garner, s^e mod N == c at WN words
+//   Verify      brsa_verify_kernel<WN>      s^e mod N, SHA-384 of the message, EMSA-PSS decode
+// WP is 32, 48 or 64 words by the larger prime, WN 64, 96 or 128 by N.  The key's Montgomery constants are computed
+// on the host once per call and copied into the call's level-1 work area; every thread reads the same key words.
+// Like the reference, the library does not wipe key material: the host copies and the work area keep the CRT key
+// until they are reused.
+// Timed under the profiling class rsa.
+#include <vector>
+
+#include "../../include/circl_b200.h"
+#include "common.cuh"
+#include "context.h"
+#include "flow_internal.h"
+#include "rsa.cuh"
+
+namespace cb200 {
+namespace brsak {
+
+template <int WP, int WN>
+__global__ void __launch_bounds__(128) brsa_sign_kernel(const rsa::SignKey<WP, WN>* __restrict__ K,
+                                                        const uint8_t* __restrict__ in, size_t in_stride,
+                                                        uint8_t* __restrict__ out, size_t out_stride,
+                                                        uint8_t* __restrict__ status, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  status[i] = (uint8_t)rsa::blind_sign<WP, WN>(out + i * out_stride, in + i * in_stride, *K);
+}
+
+template <int WN>
+__global__ void __launch_bounds__(128) brsa_verify_kernel(const rsa::VerifyKey<WN>* __restrict__ K,
+                                                          const uint8_t* __restrict__ msgs,
+                                                          const uint64_t* __restrict__ msg_off,
+                                                          const uint8_t* __restrict__ sig, size_t sig_stride,
+                                                          uint8_t* __restrict__ status, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint64_t m0 = msg_off[i], m1 = msg_off[i + 1];
+  // a message of 2^31 bytes or more, or offsets that decrease (only a device-pointer call can pass either), fails its
+  // op rather than being hashed with a truncated length
+  status[i] = m1 < m0 || m1 - m0 > 0x7fffffff ? 2 : (uint8_t)rsa::verify<WN>(msgs + m0, m1 - m0, sig + i * sig_stride, *K);
+}
+
+static inline unsigned blocks(size_t units, size_t per) { return (unsigned)((units + per - 1) / per); }
+
+// ---------------------------------------------------------------- host side
+using Words = std::vector<uint32_t>;  // little-endian, without leading zero words
+
+static Words be_words(const uint8_t* s, size_t len) {
+  Words w((len + 3) / 4, 0);
+  for (size_t i = 0; i < len; i++) {
+    const size_t k = len - 1 - i;
+    w[k / 4] |= (uint32_t)s[i] << (8 * (k % 4));
+  }
+  while (!w.empty() && !w.back()) w.pop_back();
+  return w;
+}
+static int bitlen(const Words& w) {
+  if (w.empty()) return 0;
+  int b = 32;
+  while (!((w.back() >> (b - 1)) & 1)) b--;
+  return 32 * ((int)w.size() - 1) + b;
+}
+static Words mul(const Words& a, const Words& b) {
+  Words r(a.size() + b.size(), 0);
+  for (size_t i = 0; i < a.size(); i++) {
+    uint64_t c = 0;
+    for (size_t j = 0; j < b.size(); j++) {
+      c += (uint64_t)a[i] * b[j] + r[i + j];
+      r[i + j] = (uint32_t)c;
+      c >>= 32;
+    }
+    r[i + b.size()] = (uint32_t)c;
+  }
+  while (!r.empty() && !r.back()) r.pop_back();
+  return r;
+}
+// the word count serving a modulus of `bits` bits: 32, 48, 64 (primes) or 64, 96, 128 (N); 0 past the largest
+static int word_class(int bits, int unit) {
+  for (int w = unit; w <= 2 * unit; w += unit / 2)
+    if (bits <= 32 * w) return w;
+  return 0;
+}
+static void fill(uint32_t* dst, int W, const Words& w) {
+  for (int j = 0; j < W; j++) dst[j] = j < (int)w.size() ? w[j] : 0;
+}
+
+struct PubKey {
+  Words n;
+  uint32_t e;
+  int nbits, klen, wn;
+};
+// N of 2048 to 4096 bits and an odd e with 3 <= e < 2^32
+static int parse_public(const char* fn, const uint8_t* N, size_t N_len, const uint8_t* e, size_t e_len, PubKey* k) {
+  if (!N || !e) {
+    set_error("%s: null key field", fn);
+    return CB200_ERR_ARG;
+  }
+  k->n = be_words(N, N_len);
+  k->nbits = bitlen(k->n);
+  if (k->nbits < 2048 || k->nbits > 4096) {
+    set_error("%s: the modulus has %d bits; 2048 to 4096 are served", fn, k->nbits);
+    return CB200_ERR_ARG;
+  }
+  const Words ew = be_words(e, e_len);
+  if (ew.size() != 1 || ew[0] < 3 || !(ew[0] & 1)) {
+    set_error("%s: the public exponent must be odd, at least 3 and below 2^32", fn);
+    return CB200_ERR_ARG;
+  }
+  k->e = ew[0];
+  k->klen = (k->nbits + 7) / 8;
+  k->wn = word_class(k->nbits, 64);
+  return 0;
+}
+
+struct PrivKey {
+  PubKey pub;
+  Words p, q, dp, dq, qinv;
+  int wp;
+};
+static int parse_private(const char* fn, const uint8_t* const* f, const size_t* len, PrivKey* k) {
+  int rc = parse_public(fn, f[0], len[0], f[1], len[1], &k->pub);
+  if (rc) return rc;
+  for (int i = 2; i < 7; i++)
+    if (!f[i]) {
+      set_error("%s: null key field", fn);
+      return CB200_ERR_ARG;
+    }
+  k->p = be_words(f[2], len[2]);
+  k->q = be_words(f[3], len[3]);
+  k->dp = be_words(f[4], len[4]);
+  k->dq = be_words(f[5], len[5]);
+  k->qinv = be_words(f[6], len[6]);
+  if (k->p.empty() || k->q.empty() || !(k->p[0] & 1) || !(k->q[0] & 1) || mul(k->p, k->q) != k->pub.n ||
+      bitlen(k->p) < 2 || bitlen(k->q) < 2) {
+    set_error("%s: the key is not two odd primes p, q with p q = N", fn);
+    return CB200_ERR_ARG;
+  }
+  k->wp = word_class(std::max(bitlen(k->p), bitlen(k->q)), 32);
+  if (!k->wp) {
+    set_error("%s: the larger prime has %d bits; at most 2048 are served", fn, std::max(bitlen(k->p), bitlen(k->q)));
+    return CB200_ERR_ARG;
+  }
+  if ((int)std::max({k->dp.size(), k->dq.size(), k->qinv.size()}) > k->wp) {
+    set_error("%s: dp, dq and qinv must be reduced mod p - 1, q - 1 and p", fn);
+    return CB200_ERR_ARG;
+  }
+  return 0;
+}
+
+// the sign body at one pair of word counts: key constants once per call, then run_batch
+template <int WP, int WN>
+static int sign(const char* fn, const PrivKey& k, const uint8_t* blinded, uint8_t* sig, uint8_t* status, size_t n) {
+  using Key = rsa::SignKey<WP, WN>;
+  uint32_t w[WN > WP ? WN : WP];
+  Key K;
+  fill(w, WP, k.p);
+  rsa::mod_init<WP>(K.p, w);
+  fill(w, WP, k.q);
+  rsa::mod_init<WP>(K.q, w);
+  fill(K.dp, WP, k.dp);
+  fill(K.dq, WP, k.dq);
+  fill(K.qinv, WP, k.qinv);
+  fill(w, WN, k.pub.n);
+  rsa::mod_init<WN>(K.n, w);
+  K.e = k.pub.e;
+  K.klen = k.pub.klen;
+  const size_t kl = (size_t)k.pub.klen;
+  Batch b{fn, n, sig, 1u << 14, 1u << 10, {{blinded, kl, kl, kIn}, {sig, kl, kl, kOut}, {status, 1, 1, kStatus}}, {}};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) -> int {
+    Arena A;
+    int rc = arena(slot, sizeof(Key), &A);
+    if (rc) return rc;
+    Key* dk = (Key*)A.take(sizeof(Key));
+    CB200_CUDA(cudaMemcpyAsync(dk, &K, sizeof(Key), cudaMemcpyHostToDevice, st));
+    {
+      KernelScope ks(KID_RSA, st);
+      brsa_sign_kernel<WP, WN><<<blocks(cnt, 128), 128, 0, st>>>(dk, r[0].p, r[0].stride, r[1].p, r[1].stride, r[2].p,
+                                                                 cnt);
+    }
+    CB200_CUDA(cudaGetLastError());
+    return 0;
+  });
+}
+
+template <int WN>
+static int verify(const char* fn, const PubKey& k, int slen, const uint8_t* msgs, const uint64_t* msg_off,
+                  const uint8_t* sigs, uint8_t* status, size_t n) {
+  using Key = rsa::VerifyKey<WN>;
+  uint32_t w[WN];
+  Key K;
+  fill(w, WN, k.n);
+  rsa::mod_init<WN>(K.n, w);
+  K.e = k.e;
+  K.klen = k.klen;
+  K.slen = slen;
+  const size_t kl = (size_t)k.klen;
+  Batch b{fn, n, sigs, 1u << 14, 1u << 10, {{sigs, kl, kl, kIn}, {status, 1, 1, kStatus}},
+          {{!aligned({msg_off}, {}, 8), "%s: device msg_off must be 8-byte aligned"}}, msgs, msg_off};
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) -> int {
+    Arena A;
+    int rc = arena(slot, sizeof(Key), &A);
+    if (rc) return rc;
+    Key* dk = (Key*)A.take(sizeof(Key));
+    CB200_CUDA(cudaMemcpyAsync(dk, &K, sizeof(Key), cudaMemcpyHostToDevice, st));
+    {
+      KernelScope ks(KID_RSA, st);
+      brsa_verify_kernel<WN><<<blocks(cnt, 128), 128, 0, st>>>(dk, r.msgs, r.msg_off, r[0].p, r[0].stride, r[1].p,
+                                                               cnt);
+    }
+    CB200_CUDA(cudaGetLastError());
+    return 0;
+  });
+}
+
+}  // namespace brsak
+}  // namespace cb200
+
+using namespace cb200;
+using namespace cb200::brsak;
+
+extern "C" {
+
+size_t cb200_brsa_modulus_bytes(const uint8_t* N, size_t N_len) {
+  if (!N) return 0;
+  const int bits = bitlen(be_words(N, N_len));
+  return bits >= 2048 && bits <= 4096 ? (size_t)(bits + 7) / 8 : 0;
+}
+
+int cb200_brsa_blind_sign(const uint8_t* N, size_t N_len, const uint8_t* e, size_t e_len, const uint8_t* p,
+                          size_t p_len, const uint8_t* q, size_t q_len, const uint8_t* dp, size_t dp_len,
+                          const uint8_t* dq, size_t dq_len, const uint8_t* qinv, size_t qinv_len,
+                          const uint8_t* blinded, uint8_t* sig, uint8_t* status, size_t n) {
+  const char* fn = "cb200_brsa_blind_sign";
+  const uint8_t* f[7] = {N, e, p, q, dp, dq, qinv};
+  const size_t len[7] = {N_len, e_len, p_len, q_len, dp_len, dq_len, qinv_len};
+  PrivKey k;
+  int rc = parse_private(fn, f, len, &k);
+  if (rc) return rc;
+  if (!blinded || !sig || !status) {
+    set_error("%s: null pointer", fn);
+    return CB200_ERR_ARG;
+  }
+  rc = require_ready();
+  if (rc) return rc;
+  if (n == 0) return 0;
+  switch (k.wp * 1000 + k.pub.wn) {
+    case 32064: return sign<32, 64>(fn, k, blinded, sig, status, n);
+    case 48064: return sign<48, 64>(fn, k, blinded, sig, status, n);
+    case 48096: return sign<48, 96>(fn, k, blinded, sig, status, n);
+    case 64064: return sign<64, 64>(fn, k, blinded, sig, status, n);
+    case 64096: return sign<64, 96>(fn, k, blinded, sig, status, n);
+    default: return sign<64, 128>(fn, k, blinded, sig, status, n);
+  }
+}
+
+int cb200_brsa_verify(int variant, const uint8_t* N, size_t N_len, const uint8_t* e, size_t e_len,
+                      const uint8_t* msgs, const uint64_t* msg_off, const uint8_t* sigs, uint8_t* status, size_t n) {
+  const char* fn = "cb200_brsa_verify";
+  if (variant < CB200_BRSA_SHA384_PSS_RANDOMIZED || variant > CB200_BRSA_SHA384_PSSZERO_DETERMINISTIC) {
+    set_error("%s: unknown variant %d", fn, variant);
+    return CB200_ERR_ARG;
+  }
+  PubKey k;
+  int rc = parse_public(fn, N, N_len, e, e_len, &k);
+  if (rc) return rc;
+  if (!msgs || !msg_off || !sigs || !status) {
+    set_error("%s: null pointer", fn);
+    return CB200_ERR_ARG;
+  }
+  rc = require_ready();
+  if (rc) return rc;
+  if (n == 0) return 0;
+  if (!is_device_ptr(msg_off))
+    for (size_t i = 0; i < n; i++)
+      if (msg_off[i + 1] < msg_off[i] || msg_off[i + 1] - msg_off[i] > 0x7fffffff) {
+        set_error("%s: message %zu has a bad offset or is 2^31 bytes or longer", fn, i);
+        return CB200_ERR_ARG;
+      }
+  const int slen = (variant == CB200_BRSA_SHA384_PSS_RANDOMIZED || variant == CB200_BRSA_SHA384_PSS_DETERMINISTIC)
+                       ? rsa::kHash
+                       : 0;
+  switch (k.wn) {
+    case 64: return verify<64>(fn, k, slen, msgs, msg_off, sigs, status, n);
+    case 96: return verify<96>(fn, k, slen, msgs, msg_off, sigs, status, n);
+    default: return verify<128>(fn, k, slen, msgs, msg_off, sigs, status, n);
+  }
+}
+
+}  // extern "C"

@@ -1054,3 +1054,64 @@ func OPRFFullEvaluate(suite, mode int, sk []byte, shared bool, inputs [][]byte, 
 			(*C.uint64_t)(unsafe.Pointer(&off[0])), optPtr(info), C.size_t(len(info)), u8(out), u8(status), C.size_t(n))
 	})
 }
+
+// ---- RSA blind signatures (RFC 9474, RSABSSA-SHA384, the reference's blindsign/blindrsa package), server side
+// Keys are big-endian byte strings, one key per call; rows are kLen = BRSAModulusBytes(N) bytes.
+
+// Variant ids, in the reference's blindrsa.Variant order.
+const (
+	BRSASHA384PSSRandomized        = int(C.CB200_BRSA_SHA384_PSS_RANDOMIZED)
+	BRSASHA384PSSZeroRandomized    = int(C.CB200_BRSA_SHA384_PSSZERO_RANDOMIZED)
+	BRSASHA384PSSDeterministic     = int(C.CB200_BRSA_SHA384_PSS_DETERMINISTIC)
+	BRSASHA384PSSZeroDeterministic = int(C.CB200_BRSA_SHA384_PSSZERO_DETERMINISTIC)
+)
+
+// BRSAModulusBytes returns kLen of the modulus N, or 0 outside 2048 to 4096 bits.
+func BRSAModulusBytes(N []byte) int {
+	if len(N) == 0 {
+		return 0
+	}
+	return int(C.cb200_brsa_modulus_bytes(u8(N), C.size_t(len(N))))
+}
+
+// BRSABlindSign: Signer.BlindSign (blindsign/blindrsa/brsa.go:237-257) on n blinded rows of kLen under the CRT key
+// (N, e, p, q, dp, dq, qinv); sig receives n*kLen bytes, status n bytes (1 = c > N, 2 = the s^e mod N == c check
+// failed; that row is zero).  A buffer of the wrong length panics; a key outside the served range is an error.
+func BRSABlindSign(N, e, p, q, dp, dq, qinv, blinded, sig, status []byte) error {
+	k := BRSAModulusBytes(N)
+	n := len(status)
+	if k == 0 || len(blinded) != n*k || len(sig) != n*k {
+		panic("cb200: BRSABlindSign buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	for _, f := range [][]byte{e, p, q, dp, dq, qinv} {
+		if len(f) == 0 {
+			panic("cb200: BRSABlindSign key field is empty")
+		}
+	}
+	return call(func() C.int {
+		return C.cb200_brsa_blind_sign(u8(N), C.size_t(len(N)), u8(e), C.size_t(len(e)), u8(p), C.size_t(len(p)),
+			u8(q), C.size_t(len(q)), u8(dp), C.size_t(len(dp)), u8(dq), C.size_t(len(dq)), u8(qinv),
+			C.size_t(len(qinv)), u8(blinded), u8(sig), u8(status), C.size_t(n))
+	})
+}
+
+// BRSAVerify: Verifier.Verify (brsa.go:214) of msgs[i] and the kLen-byte sigs row i under (N, e) for a variant;
+// status receives n bytes (0 valid, 1 = s >= N, 2 = an inconsistent encoding; both rsa.ErrVerification).
+func BRSAVerify(variant int, N, e []byte, msgs [][]byte, sigs, status []byte) error {
+	k := BRSAModulusBytes(N)
+	n := len(msgs)
+	if k == 0 || len(e) == 0 || len(sigs) != n*k || len(status) != n {
+		panic("cb200: BRSAVerify buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	blob, off := packMsgs(msgs)
+	return call(func() C.int {
+		return C.cb200_brsa_verify(C.int(variant), u8(N), C.size_t(len(N)), u8(e), C.size_t(len(e)), u8(blob),
+			(*C.uint64_t)(unsafe.Pointer(&off[0])), u8(sigs), u8(status), C.size_t(n))
+	})
+}

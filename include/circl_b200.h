@@ -366,6 +366,36 @@ int cb200_oprf_full_evaluate(int suite, int mode, const uint8_t *sk, size_t sk_s
                              const uint64_t *msg_off, const uint8_t *info, size_t info_len, uint8_t *out,
                              uint8_t *status, size_t n);
 
+/* ---- RSA blind signatures (RFC 9474, RSABSSA-SHA384), server side: the reference's blindsign/blindrsa package
+ * (brsa.go:202-257, internal/common/common.go:80-93,121-137, internal/common/pss.go:132-221) ----
+ * variant: the reference's Variant order below.  Keys are big-endian byte strings (leading zero bytes allowed), one
+ * key per call, always in host memory: N of 2048 to 4096 bits and an odd e with 3 <= e < 2^32 (and, for BlindSign, two
+ * primes of at most 2048 bits each).  Anything else, a null
+ * required pointer or an unknown variant is CB200_ERR_ARG with a message, before the device is touched.  Rows are
+ * kLen = ceil(bitlen(N) / 8) bytes (cb200_brsa_modulus_bytes) and on device buffers may start at any byte.  The status
+ * bytes are required; a failed op's output row is all zero and the call itself returns 0. */
+#define CB200_BRSA_SHA384_PSS_RANDOMIZED 0         /* salt 48 bytes, 32-byte message prefix */
+#define CB200_BRSA_SHA384_PSSZERO_RANDOMIZED 1     /* salt 0 */
+#define CB200_BRSA_SHA384_PSS_DETERMINISTIC 2      /* salt 48, no prefix */
+#define CB200_BRSA_SHA384_PSSZERO_DETERMINISTIC 3  /* salt 0 */
+size_t cb200_brsa_modulus_bytes(const uint8_t *N, size_t N_len); /* kLen; 0 outside 2048 to 4096 bits */
+/* Signer.BlindSign (brsa.go:237-257): blinded (n rows of kLen) -> sig = c^d mod N (n rows of kLen), from the PKCS #1
+ * CRT fields (the two primes with p q = N, dp = d mod (p - 1), dq = d mod (q - 1), qinv = q^-1 mod p, each at most as
+ * many 32-bit words as the larger prime).  The exponentiation is constant-time in place of the reference's base
+ * blinding, so the call takes no randomness.  status: 1 = c > N (ErrInvalidMessageLength), 2 = s^e mod N != c
+ * (DecryptAndCheck's "rsa: internal error", also the result of c = N or of inconsistent CRT fields). */
+int cb200_brsa_blind_sign(const uint8_t *N, size_t N_len, const uint8_t *e, size_t e_len, const uint8_t *p,
+                          size_t p_len, const uint8_t *q, size_t q_len, const uint8_t *dp, size_t dp_len,
+                          const uint8_t *dq, size_t dq_len, const uint8_t *qinv, size_t qinv_len,
+                          const uint8_t *blinded, uint8_t *sig, uint8_t *status, size_t n);
+/* Verifier.Verify (brsa.go:214): message i = msgs[msg_off[i] .. msg_off[i + 1]) (n + 1 offsets; for the randomized
+ * variants the prepared message, prefix included) and sigs (n rows of kLen).  status: 0 = valid, 1 = s >= N,
+ * 2 = an inconsistent EMSA-PSS encoding (both rsa.ErrVerification in the reference).  Messages are limited to
+ * 2^31 - 1 bytes: a host-pointer call refuses offsets that decrease or a longer message with CB200_ERR_ARG before any
+ * device work; on a device-pointer call, whose offsets the host does not read, that op gets status 2. */
+int cb200_brsa_verify(int variant, const uint8_t *N, size_t N_len, const uint8_t *e, size_t e_len,
+                      const uint8_t *msgs, const uint64_t *msg_off, const uint8_t *sigs, uint8_t *status, size_t n);
+
 /* ---- P-384 and P-521 ECDH (crypto/ecdh.P384() / P521()) ----
  * cb200_p384 / cb200_p521: the contract of cb200_p256 with 48-byte scalars and Shared outputs and 97-byte points and
  * KeyGen outputs (P-384), or 66 and 133 bytes (P-521).  A 66-byte P-521 scalar whose leading byte is above 0x01 is

@@ -955,4 +955,135 @@ inline PartialObliviousServer NewPartialObliviousServer(const Suite& s, const Pr
   return PartialObliviousServer(s, k);
 }
 }  // namespace oprf
+
+// RSA blind signatures (RFC 9474, RSABSSA-SHA384), server side: the reference's blindsign/blindrsa package (brsa.go).
+// Keys are big-endian byte strings; a private key carries the PKCS #1 CRT fields (Go's Precomputed Dp, Dq, Qinv).
+// The constructors check the key without a device (cb200_brsa_* with n = 0) and throw ErrInvalidKey for one outside
+// the served range; a batch whose ops fail throws the error of the first failure class with the per-op status bytes.
+namespace blindrsa {
+enum Variant : int {
+  SHA384PSSRandomized = CB200_BRSA_SHA384_PSS_RANDOMIZED,
+  SHA384PSSZeroRandomized = CB200_BRSA_SHA384_PSSZERO_RANDOMIZED,
+  SHA384PSSDeterministic = CB200_BRSA_SHA384_PSS_DETERMINISTIC,
+  SHA384PSSZeroDeterministic = CB200_BRSA_SHA384_PSSZERO_DETERMINISTIC,
+};
+struct BlindRSAError : Error {
+  std::vector<uint8_t> status;  // per-op bytes of a failed batch
+  explicit BlindRSAError(const std::string& m, std::vector<uint8_t> st = {}) : Error(m), status(std::move(st)) {}
+};
+#define CIRCL_BRSA_ERROR(name, text) \
+  struct name : BlindRSAError {      \
+    explicit name(std::vector<uint8_t> st = {}) : BlindRSAError(text, std::move(st)) {} \
+  };
+CIRCL_BRSA_ERROR(ErrInvalidVariant, "blindrsa: invalid BRSA variant")
+CIRCL_BRSA_ERROR(ErrUnexpectedSize, "blindrsa: unexpected input size")
+CIRCL_BRSA_ERROR(ErrInvalidMessageLength, "blindrsa: invalid message length")
+CIRCL_BRSA_ERROR(ErrInternal, "rsa: internal error")
+CIRCL_BRSA_ERROR(ErrVerification, "crypto/rsa: verification error")
+#undef CIRCL_BRSA_ERROR
+struct ErrInvalidKey : BlindRSAError {
+  explicit ErrInvalidKey(const std::string& m) : BlindRSAError(m) {}
+};
+
+struct PublicKey {
+  Bytes N, E;
+  size_t Size() const { return N.empty() ? 0 : cb200_brsa_modulus_bytes(N.data(), N.size()); }
+};
+struct PrivateKey {
+  PublicKey pub;
+  Bytes P, Q, Dp, Dq, Qinv;
+  const PublicKey& Public() const { return pub; }
+};
+
+namespace detail {
+inline const uint8_t* p(const Bytes& b) { return b.empty() ? nullptr : b.data(); }
+inline void check_call(int rc) {
+  if (rc == CB200_ERR_ARG) throw std::logic_error(cb200_last_error());
+  if (rc != 0) throw Error(cb200_last_error());
+}
+}  // namespace detail
+
+class Signer {
+ public:
+  explicit Signer(PrivateKey sk) : sk_(std::move(sk)) {
+    uint8_t z[1] = {0};
+    if (call(z, z, z, 0) == CB200_ERR_ARG) throw ErrInvalidKey(cb200_last_error());
+  }
+  size_t KLen() const { return sk_.pub.Size(); }
+  // n blinded rows of KLen bytes back to back -> n blind signatures; throws ErrInvalidMessageLength (c > N) or
+  // ErrInternal (the s^e mod N == c check) with the status bytes; failed rows are zero
+  Bytes BlindSignBatch(const Bytes& blinded) const {
+    const size_t k = KLen();
+    if (blinded.size() % k) throw ErrUnexpectedSize();
+    const size_t n = blinded.size() / k;
+    Bytes sig(n * k);
+    std::vector<uint8_t> st(n);
+    if (n) detail::check_call(call(blinded.data(), sig.data(), st.data(), n));
+    for (uint8_t bit : {1, 2})
+      for (uint8_t s : st)
+        if (s == bit) {
+          if (bit == 1) throw ErrInvalidMessageLength(st);
+          throw ErrInternal(st);
+        }
+    return sig;
+  }
+  Bytes BlindSign(const Bytes& data) const {  // brsa.go:237-257
+    if (data.size() != KLen()) throw ErrUnexpectedSize();
+    return BlindSignBatch(data);
+  }
+
+ private:
+  int call(const uint8_t* in, uint8_t* out, uint8_t* st, size_t n) const {
+    using detail::p;
+    const PublicKey& k = sk_.pub;
+    return cb200_brsa_blind_sign(p(k.N), k.N.size(), p(k.E), k.E.size(), p(sk_.P), sk_.P.size(), p(sk_.Q), sk_.Q.size(),
+                                 p(sk_.Dp), sk_.Dp.size(), p(sk_.Dq), sk_.Dq.size(), p(sk_.Qinv), sk_.Qinv.size(), in,
+                                 out, st, n);
+  }
+  PrivateKey sk_;
+};
+
+class Verifier {
+ public:
+  Verifier(Variant v, PublicKey pk) : v_(v), pk_(std::move(pk)) {
+    if (v < SHA384PSSRandomized || v > SHA384PSSZeroDeterministic) throw ErrInvalidVariant();
+    uint8_t z[1] = {0};
+    uint64_t off[1] = {0};
+    if (call(z, off, z, z, 0) == CB200_ERR_ARG) throw ErrInvalidKey(cb200_last_error());
+  }
+  size_t KLen() const { return pk_.Size(); }
+  // status bytes of messages[i] against signature row i (KLen bytes each, back to back): 0 valid, 1 s >= N, 2 an
+  // inconsistent encoding; throws ErrVerification with them if any op fails
+  std::vector<uint8_t> VerifyBatch(const std::vector<Bytes>& messages, const Bytes& sigs) const {
+    const size_t n = messages.size(), k = KLen();
+    if (sigs.size() != n * k) throw ErrUnexpectedSize();
+    std::vector<uint64_t> off(n + 1, 0);
+    Bytes blob;
+    for (size_t i = 0; i < n; i++) {
+      blob.insert(blob.end(), messages[i].begin(), messages[i].end());
+      off[i + 1] = blob.size();
+    }
+    blob.push_back(0);  // never empty
+    std::vector<uint8_t> st(n);
+    if (n) detail::check_call(call(blob.data(), off.data(), sigs.data(), st.data(), n));
+    for (uint8_t s : st)
+      if (s) throw ErrVerification(st);
+    return st;
+  }
+  void Verify(const Bytes& message, const Bytes& signature) const {  // brsa.go:214
+    if (signature.size() != KLen()) throw ErrVerification();
+    VerifyBatch({message}, signature);
+  }
+
+ private:
+  int call(const uint8_t* msgs, const uint64_t* off, const uint8_t* sigs, uint8_t* st, size_t n) const {
+    using detail::p;
+    return cb200_brsa_verify(v_, p(pk_.N), pk_.N.size(), p(pk_.E), pk_.E.size(), msgs, off, sigs, st, n);
+  }
+  Variant v_;
+  PublicKey pk_;
+};
+inline Signer NewSigner(const PrivateKey& sk) { return Signer(sk); }
+inline Verifier NewVerifier(Variant v, const PublicKey& pk) { return Verifier(v, pk); }
+}  // namespace blindrsa
 }  // namespace circl
