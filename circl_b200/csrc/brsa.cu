@@ -14,6 +14,7 @@
 #include "context.h"
 #include "flow_internal.h"
 #include "rsa.cuh"
+#include "rsa_host.h"
 
 namespace cb200 {
 namespace brsak {
@@ -45,46 +46,7 @@ __global__ void __launch_bounds__(128) brsa_verify_kernel(const rsa::VerifyKey<W
 static inline unsigned blocks(size_t units, size_t per) { return (unsigned)((units + per - 1) / per); }
 
 // ---------------------------------------------------------------- host side
-using Words = std::vector<uint32_t>;  // little-endian, without leading zero words
-
-static Words be_words(const uint8_t* s, size_t len) {
-  Words w((len + 3) / 4, 0);
-  for (size_t i = 0; i < len; i++) {
-    const size_t k = len - 1 - i;
-    w[k / 4] |= (uint32_t)s[i] << (8 * (k % 4));
-  }
-  while (!w.empty() && !w.back()) w.pop_back();
-  return w;
-}
-static int bitlen(const Words& w) {
-  if (w.empty()) return 0;
-  int b = 32;
-  while (!((w.back() >> (b - 1)) & 1)) b--;
-  return 32 * ((int)w.size() - 1) + b;
-}
-static Words mul(const Words& a, const Words& b) {
-  Words r(a.size() + b.size(), 0);
-  for (size_t i = 0; i < a.size(); i++) {
-    uint64_t c = 0;
-    for (size_t j = 0; j < b.size(); j++) {
-      c += (uint64_t)a[i] * b[j] + r[i + j];
-      r[i + j] = (uint32_t)c;
-      c >>= 32;
-    }
-    r[i + b.size()] = (uint32_t)c;
-  }
-  while (!r.empty() && !r.back()) r.pop_back();
-  return r;
-}
-// the word count serving a modulus of `bits` bits: 32, 48, 64 (primes) or 64, 96, 128 (N); 0 past the largest
-static int word_class(int bits, int unit) {
-  for (int w = unit; w <= 2 * unit; w += unit / 2)
-    if (bits <= 32 * w) return w;
-  return 0;
-}
-static void fill(uint32_t* dst, int W, const Words& w) {
-  for (int j = 0; j < W; j++) dst[j] = j < (int)w.size() ? w[j] : 0;
-}
+using namespace rsah;
 
 struct PubKey {
   Words n;
@@ -97,20 +59,19 @@ static int parse_public(const char* fn, const uint8_t* N, size_t N_len, const ui
     set_error("%s: null key field", fn);
     return CB200_ERR_ARG;
   }
-  k->n = be_words(N, N_len);
-  k->nbits = bitlen(k->n);
-  if (k->nbits < 2048 || k->nbits > 4096) {
-    set_error("%s: the modulus has %d bits; 2048 to 4096 are served", fn, k->nbits);
-    return CB200_ERR_ARG;
-  }
+  Modulus m;
+  int rc = parse_modulus(fn, N, N_len, &m);
+  if (rc) return rc;
+  k->n = m.n;
+  k->nbits = m.nbits;
   const Words ew = be_words(e, e_len);
   if (ew.size() != 1 || ew[0] < 3 || !(ew[0] & 1)) {
     set_error("%s: the public exponent must be odd, at least 3 and below 2^32", fn);
     return CB200_ERR_ARG;
   }
   k->e = ew[0];
-  k->klen = (k->nbits + 7) / 8;
-  k->wn = word_class(k->nbits, 64);
+  k->klen = m.klen;
+  k->wn = m.wn;
   return 0;
 }
 
@@ -127,21 +88,11 @@ static int parse_private(const char* fn, const uint8_t* const* f, const size_t* 
       set_error("%s: null key field", fn);
       return CB200_ERR_ARG;
     }
-  k->p = be_words(f[2], len[2]);
-  k->q = be_words(f[3], len[3]);
+  rc = parse_primes(fn, k->pub.n, f[2], len[2], f[3], len[3], &k->p, &k->q, &k->wp);
+  if (rc) return rc;
   k->dp = be_words(f[4], len[4]);
   k->dq = be_words(f[5], len[5]);
   k->qinv = be_words(f[6], len[6]);
-  if (k->p.empty() || k->q.empty() || !(k->p[0] & 1) || !(k->q[0] & 1) || mul(k->p, k->q) != k->pub.n ||
-      bitlen(k->p) < 2 || bitlen(k->q) < 2) {
-    set_error("%s: the key is not two odd primes p, q with p q = N", fn);
-    return CB200_ERR_ARG;
-  }
-  k->wp = word_class(std::max(bitlen(k->p), bitlen(k->q)), 32);
-  if (!k->wp) {
-    set_error("%s: the larger prime has %d bits; at most 2048 are served", fn, std::max(bitlen(k->p), bitlen(k->q)));
-    return CB200_ERR_ARG;
-  }
   if ((int)std::max({k->dp.size(), k->dq.size(), k->qinv.size()}) > k->wp) {
     set_error("%s: dp, dq and qinv must be reduced mod p - 1, q - 1 and p", fn);
     return CB200_ERR_ARG;

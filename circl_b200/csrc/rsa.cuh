@@ -10,6 +10,9 @@
 //   exp_public    x^e by left-to-right square-and-multiply on the bits of the public e < 2^32
 //   blind_sign    s_p = c^dp mod p, s_q = c^dq mod q, Garner's recombination with qinv, the check s^e mod N == c
 //   verify        s^e mod N and the EMSA-PSS decode with MGF1-SHA-384
+//   pb_*          partially blind RSA (RSAPBSSA-SHA384, partiallyblindrsa/pbrsa.go): e' from the metadata by
+//                 HKDF-SHA-384, d' by Fermat inversion mod p' = (p - 1) / 2 and q', exp_public_words for the
+//                 multi-word e'; see that section
 //
 // Secret values (p, q, dp, dq, qinv, s_p, s_q) reach no branch and no address: every loop count and index comes from
 // the word counts and the public bit lengths of p and q, the window digit only forms masks, and the final subtraction
@@ -162,8 +165,9 @@ CB200_XHD void add_mod(uint32_t* r, const uint32_t* a, const uint32_t* b, const 
 
 // r = x^d R mod m from xm = x R mod m, for the secret d of W words of which the low M->bits count (d < m).  Every
 // one of the ceil(bits / 4) windows costs four squarings and one product with a table entry selected by masks.
-template <int W>
-CB200_RSA_NOINLINE void exp_secret(uint32_t* r, const uint32_t* xm, const uint32_t* d, const Mod<W>* M) {
+// digit(w) reads window w of d.
+template <int W, class Digit>
+CB200_XHD void exp_windows(uint32_t* r, const uint32_t* xm, const Digit& digit_of, const Mod<W>* M) {
   uint32_t tbl[16][W], one[W];
   for (int j = 0; j < W; j++) one[j] = j == 0;
   mont_mul<W>(tbl[0], M->r2, one, M);  // R mod m
@@ -177,7 +181,7 @@ CB200_RSA_NOINLINE void exp_secret(uint32_t* r, const uint32_t* xm, const uint32
   for (int w = nwin - 1; w >= 0; w--) {
 #pragma unroll 1
     for (int s = 0; s < 4; s++) mont_mul<W>(r, r, r, M);
-    const uint32_t digit = (ldk(&d[w >> 3]) >> (4 * (w & 7))) & 15;
+    const uint32_t digit = digit_of(w);
 #pragma unroll
     for (int j = 0; j < W; j++) sel[j] = 0;
 #pragma unroll 1
@@ -188,6 +192,16 @@ CB200_RSA_NOINLINE void exp_secret(uint32_t* r, const uint32_t* xm, const uint32
     }
     mont_mul<W>(r, r, sel, M);
   }
+}
+// d in the key (global memory on the device)
+template <int W>
+CB200_RSA_NOINLINE void exp_secret(uint32_t* r, const uint32_t* xm, const uint32_t* d, const Mod<W>* M) {
+  exp_windows<W>(r, xm, [&](int w) { return (ldk(&d[w >> 3]) >> (4 * (w & 7))) & 15; }, M);
+}
+// d in the thread's own memory (an exponent computed per operation)
+template <int W>
+CB200_RSA_NOINLINE void exp_secret_own(uint32_t* r, const uint32_t* xm, const uint32_t* d, const Mod<W>* M) {
+  exp_windows<W>(r, xm, [&](int w) { return (d[w >> 3] >> (4 * (w & 7))) & 15; }, M);
 }
 
 // r = x^e R mod m from xm = x R mod m for a public e >= 1
@@ -226,9 +240,10 @@ CB200_XHD int cmp(const uint32_t* a, const uint32_t* b) {
 }
 
 // ---------------------------------------------------------------- BlindSign
-// s = q h + s_q, with h = (s_p - s_q) qinv mod p (Garner), from spm = s_p R mod p and sq = s_q (< q); s has WN words
-template <int WP, int WN>
-CB200_XHD void garner(uint32_t* s, const uint32_t* spm, const uint32_t* sq, const SignKey<WP, WN>& K) {
+// s = q h + s_q, with h = (s_p - s_q) qinv mod p (Garner), from spm = s_p R mod p and sq = s_q (< q); s has WN words.
+// K: a key with the members p, q (Mod<WP>) and qinv.
+template <int WP, int WN, class Key>
+CB200_XHD void garner(uint32_t* s, const uint32_t* spm, const uint32_t* sq, const Key& K) {
   uint32_t sqm[WP], h[WP], qinv[WP];
   mont_mul<WP>(sqm, sq, K.p.r2, &K.p);  // s_q R mod p (s_q < q may exceed p)
   sub_mod<WP>(h, spm, sqm, &K.p);       // (s_p - s_q) R mod p
@@ -358,6 +373,190 @@ CB200_XHD uint32_t verify(const uint8_t* msg, uint64_t len, const uint8_t* sig, 
   return emsa_pss_verify<WN>(v, klen, ldk((const uint32_t*)&K.n.bits), mh, ldk((const uint32_t*)&K.slen));
 }
 
+// ---------------------------------------------------------------- partially blind RSA (RSAPBSSA-SHA384)
+// draft-amjad-cfrg-partially-blind-rsa as the reference's blindsign/blindrsa/partiallyblindrsa (pbrsa.go): every
+// metadata value selects the key (N, e') and d' = e'^-1 mod phi(N), derived per operation.  The primes are safe,
+// p = 2 p' + 1 with p' prime and p = 3 mod 4.  e' has fewer than lambda = bitlen(N) / 2 bits, so it fits in WN / 2
+// words, never more than WP.  p', q', p' - 2, q' - 2, d'_p, d'_q, s_p and s_q are secret under the rules above; e'
+// and the metadata are public.
+template <int WN>
+struct PbVerifyKey {
+  Mod<WN> n;
+  uint64_t si[8], so[8];  // HMAC-SHA-384 pad states of HKDF's salt N (kLen bytes, longer than a block: SHA-384(N))
+  int klen;
+};
+template <int WP, int WN>
+struct PbSignKey {
+  Mod<WP> p, q;
+  Mod<WP> ph, qh;             // p' = (p - 1) / 2, q' = (q - 1) / 2
+  uint32_t ph2[WP], qh2[WP];  // p' - 2, q' - 2: Fermat's exponents
+  uint32_t qinv[WP];
+  Mod<WN> n;
+  uint64_t si[8], so[8];
+  int klen;
+};
+
+// bits of e' that can be set: the first lambda / 8 bytes, bits lambda - 1 and lambda - 2 clear
+CB200_XHD int pb_exp_bits(int nbits) {
+  const int lambda = nbits / 2;
+  return lambda - 2 < 8 * (lambda / 8) ? lambda - 2 : 8 * (lambda / 8);
+}
+
+// e' (WN / 2 words) of derivePublicKey (pbrsa.go:81-117) for the metadata meta[0 .. mlen): HKDF-SHA-384 with salt N,
+// IKM "key" || meta || 0x00 and info "PBRSA", its first lambda / 8 bytes read big-endian, bit 0 set and bits lambda - 1
+// and lambda - 2 cleared.  Only the Expand blocks holding those bytes are computed: a block does not depend on the
+// output length.  si / so: the salt's pad states (PbVerifyKey).
+template <int WN>
+CB200_XHD void derive_exponent(uint32_t* e, int nbits, const uint8_t* meta, int mlen, const uint64_t (&si)[8],
+                               const uint64_t (&so)[8]) {
+  using S = sha2::Sha384;
+  uint64_t prk[8], ki[8], ko[8], t[8], prev[8];
+  sha2::hmac<S>(prk, si, so, mlen + 4, [&](int j) -> uint8_t {
+    if (j < 3) return (uint8_t)"key"[j];
+    return j - 3 < mlen ? meta[j - 3] : 0;
+  });
+  sha2::hmac_key<S>(ki, ko, prk);
+  const int lambda = nbits / 2, nb = lambda / 8;
+  for (int j = 0; j < WN / 2; j++) e[j] = 0;
+#pragma unroll 1
+  for (int blk = 0; blk * kHash < nb; blk++) {
+    const int tl = blk ? kHash : 0;  // T(0) is empty
+    for (int i = 0; i < 8; i++) prev[i] = t[i];
+    sha2::hmac<S>(t, ki, ko, tl + 6, [&](int j) -> uint8_t {
+      if (j < tl) return sha2::digest_byte<S>(prev, j);
+      return j < tl + 5 ? (uint8_t)"PBRSA"[j - tl] : (uint8_t)(blk + 1);
+    });
+    for (int k = 0; k < kHash && blk * kHash + k < nb; k++) {
+      const int i = nb - 1 - (blk * kHash + k);  // byte index from the least significant end
+      e[i >> 2] |= (uint32_t)sha2::digest_byte<S>(t, k) << (8 * (i & 3));
+    }
+  }
+  e[0] |= 1;
+  for (int b = lambda - 2; b < lambda; b++)
+    if (b < 8 * nb) e[b >> 5] &= ~(1u << (b & 31));
+}
+
+// r = x^e R mod m from xm = x R mod m for a public e below 2^bits: fixed windows of kPubWin bits from the top, each
+// kPubWin squarings and one product with the table entry of its digit (entry 0 is R mod m, so a zero digit costs the
+// same product).  The sequence of products depends on `bits` alone, so the threads of a warp, which share N, run in
+// step whatever their e.
+constexpr int kPubWin = 5;
+template <int W>
+CB200_RSA_NOINLINE void exp_public_words(uint32_t* r, const uint32_t* xm, const uint32_t* e, int bits, const Mod<W>* M) {
+  uint32_t tbl[1 << kPubWin][W], one[W];
+  for (int j = 0; j < W; j++) one[j] = j == 0;
+  mont_mul<W>(tbl[0], M->r2, one, M);
+  for (int j = 0; j < W; j++) tbl[1][j] = xm[j];
+#pragma unroll 1
+  for (int k = 2; k < (1 << kPubWin); k++) mont_mul<W>(tbl[k], tbl[k - 1], xm, M);
+  const int nw = (bits + 31) / 32, nwin = (bits + kPubWin - 1) / kPubWin;
+  auto digit = [&](int b) {  // bits b .. b + kPubWin - 1 of e
+    uint32_t v = e[b >> 5] >> (b & 31);
+    if ((b & 31) > 32 - kPubWin && (b >> 5) + 1 < nw) v |= e[(b >> 5) + 1] << (32 - (b & 31));
+    return v & ((1u << kPubWin) - 1);
+  };
+  const uint32_t* top = tbl[digit(kPubWin * (nwin - 1))];
+  for (int j = 0; j < W; j++) r[j] = top[j];
+#pragma unroll 1
+  for (int w = nwin - 2; w >= 0; w--) {
+#pragma unroll 1
+    for (int s = 0; s < kPubWin; s++) mont_mul<W>(r, r, r, M);
+    mont_mul<W>(r, r, tbl[digit(kPubWin * w)], M);
+  }
+}
+
+// s_p R mod p = c^d'_p R mod p from cm = c R mod p, with d'_p = e'^-1 mod (p - 1) = 2 p': x = e'^(p' - 2) mod p'
+// (Fermat's inverse, p' prime), lifted to its odd representative below 2 p' (e' is odd, so is d'_p) by adding p' under
+// a mask.  e: e' in WP words; H: p'; h2: p' - 2.
+template <int WP>
+CB200_XHD void pb_half(uint32_t* sm, const uint32_t* cm, const uint32_t* e, const Mod<WP>& P, const Mod<WP>& H,
+                       const uint32_t* h2) {
+  uint32_t x[WP], d[WP];
+  mont_mul<WP>(x, e, H.r2, &H);  // e' R mod p' (e' < R)
+  exp_secret<WP>(d, x, h2, &H);
+  for (int j = 0; j < WP; j++) x[j] = j == 0;
+  mont_mul<WP>(d, d, x, &H);
+  const uint32_t even = (d[0] & 1) - 1u;
+  uint64_t c = 0;
+  for (int j = 0; j < WP; j++) {
+    c += (uint64_t)d[j] + (ldk(&H.m[j]) & even);
+    d[j] = (uint32_t)c;
+    c >>= 32;
+  }
+  exp_secret_own<WP>(sm, cm, d, &P);
+}
+
+// BlindSign (pbrsa.go:350-375) of the kLen-byte blinded message c under the key of meta[0 .. mlen): status 0 and
+// s = c^d' mod N in out, or 1 for c > N (ErrInvalidMessageLength) and 2 for s^e' mod N != c (DecryptAndCheck's
+// "rsa: internal error"), with out all zero
+template <int WP, int WN>
+CB200_XHD uint32_t pb_blind_sign(uint8_t* out, const uint8_t* in, const uint8_t* meta, int mlen,
+                                 const PbSignKey<WP, WN>& K) {
+  const int klen = K.klen, nbits = ldk((const uint32_t*)&K.n.bits);
+  uint32_t c[WN], nw[WN];
+  from_be<WN>(c, in, klen);
+  for (int j = 0; j < WN; j++) nw[j] = ldk(&K.n.m[j]);
+  uint32_t st = cmp<WN>(c, nw) > 0 ? 1u : 0u;
+  uint32_t e[WP];
+  derive_exponent<WN>(e, nbits, meta, mlen, K.si, K.so);
+  for (int j = WN / 2; j < WP; j++) e[j] = 0;
+  // c R mod p and c R mod q as in blind_sign
+  uint32_t lo[WP], hi[WP], x[WP], y[WP], sp[WP], sq[WP];
+  for (int j = 0; j < WP; j++) {
+    lo[j] = c[j];
+    hi[j] = j + WP < WN ? c[j + WP] : 0;
+  }
+  auto to_mont = [&](const Mod<WP>& P) {
+    mont_mul<WP>(x, hi, P.r3, &P);
+    mont_mul<WP>(y, lo, P.r2, &P);
+    add_mod<WP>(x, x, y, &P);
+  };
+  to_mont(K.p);
+  pb_half<WP>(sp, x, e, K.p, K.ph, K.ph2);  // s_p R mod p
+  to_mont(K.q);
+  pb_half<WP>(y, x, e, K.q, K.qh, K.qh2);  // s_q R mod q
+  for (int j = 0; j < WP; j++) x[j] = j == 0;
+  mont_mul<WP>(sq, y, x, &K.q);
+  uint32_t s[WN], sm[WN], v[WN];
+  garner<WP, WN>(s, sp, sq, K);
+  mont_mul<WN>(sm, s, K.n.r2, &K.n);
+  exp_public_words<WN>(v, sm, e, pb_exp_bits(nbits), &K.n);
+  for (int j = 0; j < WN; j++) sm[j] = j == 0;
+  mont_mul<WN>(v, v, sm, &K.n);
+  uint32_t diff = 0;
+  for (int j = 0; j < WN; j++) diff |= v[j] ^ c[j];
+  if (!st && diff) st = 2;
+  const uint32_t keep = st ? 0u : ~0u;
+  for (int i = 0; i < klen; i++) out[i] = be_byte(s, klen, i) & keep;
+  return st;
+}
+
+// Verify (pbrsa.go:244-251) of msg[0 .. len) under the metadata meta[0 .. mlen) and the kLen-byte signature: the
+// message framed as "msg" || I2OSP(mlen, 4) || meta || msg, RSA-PSS-SHA-384 with a 48-byte salt under (N, e').
+// 0, 1 for s >= N, 2 for an inconsistent encoding.  7 + mlen + len < 2^31.
+template <int WN>
+CB200_XHD uint32_t pb_verify(const uint8_t* msg, int len, const uint8_t* meta, int mlen, const uint8_t* sig,
+                             const PbVerifyKey<WN>& K) {
+  const int klen = K.klen, nbits = ldk((const uint32_t*)&K.n.bits);
+  uint32_t s[WN], nw[WN], sm[WN], v[WN], e[WN / 2];
+  from_be<WN>(s, sig, klen);
+  for (int j = 0; j < WN; j++) nw[j] = ldk(&K.n.m[j]);
+  if (cmp<WN>(s, nw) >= 0) return 1;
+  derive_exponent<WN>(e, nbits, meta, mlen, K.si, K.so);
+  mont_mul<WN>(sm, s, K.n.r2, &K.n);
+  exp_public_words<WN>(v, sm, e, pb_exp_bits(nbits), &K.n);
+  for (int j = 0; j < WN; j++) sm[j] = j == 0;
+  mont_mul<WN>(v, v, sm, &K.n);
+  uint64_t mh[8];
+  sha2::Sha384::iv(mh);
+  sha2::absorb<sha2::Sha384>(mh, 0, 7 + mlen + len, [&](int j) -> uint8_t {
+    if (j < 3) return (uint8_t)"msg"[j];
+    if (j < 7) return (uint8_t)((uint32_t)mlen >> (8 * (6 - j)));
+    return j - 7 < mlen ? meta[j - 7] : msg[j - 7 - mlen];
+  });
+  return emsa_pss_verify<WN>(v, klen, nbits, mh, kHash);
+}
+
 // ---------------------------------------------------------------- host preparation
 // M from the odd modulus m > 1 of W words: n0 by Newton's iteration, R^2 mod m from R mod m (32 W modular doublings of
 // 1) by t more doublings and s Montgomery squarings with t 2^s = 32 W (each squaring doubles the exponent of 2 over R),
@@ -384,6 +583,56 @@ inline void mod_init(Mod<W>& M, const uint32_t* m) {
   for (int i = 0; i < s; i++) mont_mul<W>(x, x, x, &M);
   for (int j = 0; j < W; j++) M.r2[j] = x[j];
   mont_mul<W>(M.r3, M.r2, M.r2, &M);
+}
+
+// the HMAC-SHA-384 pad states of HKDF's salt, the klen-byte big-endian N (longer than a block, so HMAC keys with
+// SHA-384(N))
+inline void pb_salt_states(uint64_t (&si)[8], uint64_t (&so)[8], const uint8_t* n, int klen) {
+  uint64_t h[8];
+  sha2::Sha384::iv(h);
+  sha2::absorb<sha2::Sha384>(h, 0, klen, [&](int j) { return n[j]; });
+  sha2::hmac_key<sha2::Sha384>(si, so, h);
+}
+
+// Miller-Rabin on the odd n >= 3 of W words with `rounds` random bases below 2^(bitlen(n) - 1), drawn from rnd() (32
+// random bits a call): false if a round proves n composite
+template <int W, class Rnd>
+inline bool probably_prime(const uint32_t* n, int rounds, Rnd& rnd) {
+  Mod<W> M;
+  mod_init<W>(M, n);
+  if (M.bits == 2) return true;  // n = 3
+  uint32_t d[W], one[W], m1[W], a[W], x[W];
+  for (int j = 0; j < W; j++) d[j] = n[j], one[j] = j == 0;
+  d[0] -= 1;  // n - 1 = 2^s d, d odd
+  int s = 0;
+  while (!(d[0] & 1)) {
+    for (int j = 0; j < W; j++) d[j] = (d[j] >> 1) | (j + 1 < W ? d[j + 1] << 31 : 0);
+    s++;
+  }
+  mont_mul<W>(one, M.r2, one, &M);  // R mod n, 1 in Montgomery form
+  uint32_t zero[W] = {0};
+  sub_mod<W>(m1, zero, one, &M);  // -1
+  for (int r = 0; r < rounds; r++) {
+    const int top = M.bits - 1;  // a < 2^top < n
+    for (int j = 0; j < W; j++)
+      a[j] = 32 * j >= top ? 0 : 32 * j + 32 <= top ? (uint32_t)rnd() : (uint32_t)rnd() & ((1u << (top & 31)) - 1);
+    bool small = a[0] < 2;
+    for (int j = 1; j < W; j++) small = small && !a[j];
+    if (small) {  // bases 0 and 1 prove nothing: draw again
+      r--;
+      continue;
+    }
+    mont_mul<W>(x, a, M.r2, &M);
+    exp_secret<W>(x, x, d, &M);
+    if (!cmp<W>(x, one) || !cmp<W>(x, m1)) continue;
+    bool witness = true;
+    for (int i = 1; i < s && witness; i++) {
+      mont_mul<W>(x, x, x, &M);
+      if (!cmp<W>(x, m1)) witness = false;
+    }
+    if (witness) return false;
+  }
+  return true;
 }
 
 }  // namespace rsa

@@ -1115,3 +1115,62 @@ func BRSAVerify(variant int, N, e []byte, msgs [][]byte, sigs, status []byte) er
 			(*C.uint64_t)(unsafe.Pointer(&off[0])), u8(sigs), u8(status), C.size_t(n))
 	})
 }
+
+// ---- Partially blind RSA signatures (RSAPBSSA-SHA384, the reference's blindsign/blindrsa/partiallyblindrsa
+// package), server side.  Keys are big-endian byte strings, one key per call; rows are kLen = BRSAModulusBytes(N)
+// bytes; each op has its own metadata, which selects the key it is signed and verified under.
+
+// PBRSACheckKey is NewSigner's safe-prime test (pbrsa.go:324-343) on the host: an error unless (p - 1) / 2 and
+// (q - 1) / 2 pass 20 Miller-Rabin rounds and the key is in the served range.  It needs no device.
+func PBRSACheckKey(N, p, q []byte) error {
+	if len(N) == 0 || len(p) == 0 || len(q) == 0 {
+		panic("cb200: PBRSACheckKey key field is empty")
+	}
+	return call(func() C.int {
+		return C.cb200_pbrsa_check_key(u8(N), C.size_t(len(N)), u8(p), C.size_t(len(p)), u8(q), C.size_t(len(q)))
+	})
+}
+
+// PBRSABlindSign: Signer.BlindSign (pbrsa.go:350-375) on n blinded rows of kLen, op i under metadata[i], with the key
+// (N, p, q, qinv = q^-1 mod p); sig receives n*kLen bytes, status n bytes (1 = c > N, 2 = the s^e' mod N == c check
+// failed; that row is zero).  A buffer of the wrong length panics; a key outside the served range is an error.
+func PBRSABlindSign(N, p, q, qinv, blinded []byte, metadata [][]byte, sig, status []byte) error {
+	k := BRSAModulusBytes(N)
+	n := len(status)
+	if k == 0 || len(blinded) != n*k || len(sig) != n*k || len(metadata) != n {
+		panic("cb200: PBRSABlindSign buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	for _, f := range [][]byte{p, q, qinv} {
+		if len(f) == 0 {
+			panic("cb200: PBRSABlindSign key field is empty")
+		}
+	}
+	blob, off := packMsgs(metadata)
+	return call(func() C.int {
+		return C.cb200_pbrsa_blind_sign(u8(N), C.size_t(len(N)), u8(p), C.size_t(len(p)), u8(q), C.size_t(len(q)),
+			u8(qinv), C.size_t(len(qinv)), u8(blinded), u8(blob), (*C.uint64_t)(unsafe.Pointer(&off[0])), u8(sig),
+			u8(status), C.size_t(n))
+	})
+}
+
+// PBRSAVerify: Verifier.Verify (pbrsa.go:244-251) of msgs[i] under metadata[i] and the kLen-byte sigs row i under N;
+// status receives n bytes (0 valid, 1 = s >= N, 2 = an inconsistent encoding; both rsa.ErrVerification).
+func PBRSAVerify(N []byte, msgs, metadata [][]byte, sigs, status []byte) error {
+	k := BRSAModulusBytes(N)
+	n := len(msgs)
+	if k == 0 || len(metadata) != n || len(sigs) != n*k || len(status) != n {
+		panic("cb200: PBRSAVerify buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	blob, off := packMsgs(msgs)
+	mblob, moff := packMsgs(metadata)
+	return call(func() C.int {
+		return C.cb200_pbrsa_verify(u8(N), C.size_t(len(N)), u8(blob), (*C.uint64_t)(unsafe.Pointer(&off[0])),
+			u8(mblob), (*C.uint64_t)(unsafe.Pointer(&moff[0])), u8(sigs), u8(status), C.size_t(n))
+	})
+}

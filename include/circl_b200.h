@@ -396,6 +396,34 @@ int cb200_brsa_blind_sign(const uint8_t *N, size_t N_len, const uint8_t *e, size
 int cb200_brsa_verify(int variant, const uint8_t *N, size_t N_len, const uint8_t *e, size_t e_len,
                       const uint8_t *msgs, const uint64_t *msg_off, const uint8_t *sigs, uint8_t *status, size_t n);
 
+/* ---- Partially blind RSA signatures (draft-amjad-cfrg-partially-blind-rsa, RSAPBSSA-SHA384), server side: the
+ * reference's blindsign/blindrsa/partiallyblindrsa package (pbrsa.go) ----
+ * Each op's metadata selects the key: e' from HKDF-SHA-384 of the metadata (derivePublicKey, pbrsa.go:81-117) and
+ * d' = e'^-1 mod phi(N).  Keys follow the cb200_brsa_* rules (big-endian byte strings in host memory, one key per
+ * call, N of 2048 to 4096 bits, primes of at most 2048 bits with p q = N); in addition p and q must be = 3 mod 4 and
+ * qinv = q^-1 mod p below p.  Metadata i is meta[meta_off[i] .. meta_off[i + 1]) (n + 1 offsets), at most 2^31 - 8
+ * bytes, and in Verify metadata and message together are at most 2^31 - 8 bytes.  A host-pointer call refuses offsets
+ * that decrease or longer strings with CB200_ERR_ARG, like any other argument error, before the device is touched; on a
+ * device-pointer call, whose offsets the host does not read, that op gets status 2.  Rows are kLen bytes
+ * (cb200_brsa_modulus_bytes) and on device buffers may start at any byte.  The status bytes are required; a failed
+ * op's output row is all zero and the call itself returns 0. */
+/* NewSigner's safe-prime test (pbrsa.go:324-343): 20 Miller-Rabin rounds with random bases on (p - 1) / 2 and
+ * (q - 1) / 2, on the host (no device needed).  0, or CB200_ERR_ARG with a message.  BlindSign does not repeat it: a key
+ * that passes by chance fails every op with status 2. */
+int cb200_pbrsa_check_key(const uint8_t *N, size_t N_len, const uint8_t *p, size_t p_len, const uint8_t *q,
+                          size_t q_len);
+/* Signer.BlindSign (pbrsa.go:350-375): blinded (n rows of kLen) -> sig = c^d' mod N under the key of metadata i.
+ * status: 1 = c > N (ErrInvalidMessageLength), 2 = s^e' mod N != c (DecryptAndCheck's "rsa: internal error", also the
+ * result of c = N or a wrong qinv). */
+int cb200_pbrsa_blind_sign(const uint8_t *N, size_t N_len, const uint8_t *p, size_t p_len, const uint8_t *q,
+                           size_t q_len, const uint8_t *qinv, size_t qinv_len, const uint8_t *blinded,
+                           const uint8_t *meta, const uint64_t *meta_off, uint8_t *sig, uint8_t *status, size_t n);
+/* Verifier.Verify (pbrsa.go:244-251): message i = msgs[msg_off[i] .. msg_off[i + 1]) under metadata i and sigs row i:
+ * RSA-PSS-SHA-384 with a 48-byte salt over "msg" || I2OSP(len(metadata), 4) || metadata || message under (N, e').
+ * status: 0 = valid, 1 = s >= N, 2 = an inconsistent EMSA-PSS encoding (both rsa.ErrVerification). */
+int cb200_pbrsa_verify(const uint8_t *N, size_t N_len, const uint8_t *msgs, const uint64_t *msg_off,
+                       const uint8_t *meta, const uint64_t *meta_off, const uint8_t *sigs, uint8_t *status, size_t n);
+
 /* ---- P-384 and P-521 ECDH (crypto/ecdh.P384() / P521()) ----
  * cb200_p384 / cb200_p521: the contract of cb200_p256 with 48-byte scalars and Shared outputs and 97-byte points and
  * KeyGen outputs (P-384), or 66 and 133 bytes (P-521).  A 66-byte P-521 scalar whose leading byte is above 0x01 is

@@ -1086,4 +1086,123 @@ class Verifier {
 inline Signer NewSigner(const PrivateKey& sk) { return Signer(sk); }
 inline Verifier NewVerifier(Variant v, const PublicKey& pk) { return Verifier(v, pk); }
 }  // namespace blindrsa
+
+// Partially blind RSA signatures (RSAPBSSA-SHA384), server side: the reference's blindsign/blindrsa/partiallyblindrsa
+// package (pbrsa.go).  Each op's metadata selects the key it is signed and verified under.  Keys are blindrsa's;
+// a private key needs N, P, Q and Qinv (E, Dp and Dq are not used).  Signer runs NewSigner's safe-prime test once
+// (cb200_pbrsa_check_key) and throws ErrInvalidPrivateKey for a key that fails it or lies outside the served range;
+// Verifier throws ErrInvalidPublicKey for a modulus outside the range.  Errors are blindrsa's otherwise.
+namespace partiallyblindrsa {
+using blindrsa::BlindRSAError;
+using blindrsa::ErrInternal;
+using blindrsa::ErrInvalidMessageLength;
+using blindrsa::ErrUnexpectedSize;
+using blindrsa::ErrVerification;
+using blindrsa::PrivateKey;
+using blindrsa::PublicKey;
+struct ErrInvalidPrivateKey : BlindRSAError {
+  explicit ErrInvalidPrivateKey(const std::string& m) : BlindRSAError(m) {}
+};
+struct ErrInvalidPublicKey : BlindRSAError {
+  explicit ErrInvalidPublicKey(const std::string& m) : BlindRSAError(m) {}
+};
+
+namespace detail {
+// strings back to back with their n + 1 offsets; the blob is never empty
+inline void pack(const std::vector<Bytes>& v, Bytes* blob, std::vector<uint64_t>* off) {
+  off->assign(v.size() + 1, 0);
+  for (size_t i = 0; i < v.size(); i++) {
+    blob->insert(blob->end(), v[i].begin(), v[i].end());
+    (*off)[i + 1] = blob->size();
+  }
+  blob->push_back(0);
+}
+}  // namespace detail
+
+class Signer {
+ public:
+  explicit Signer(PrivateKey sk) : sk_(std::move(sk)) {
+    using blindrsa::detail::p;
+    uint8_t z[1] = {0};
+    uint64_t off[1] = {0};
+    const PublicKey& k = sk_.pub;
+    if (call(z, z, off, z, z, 0) == CB200_ERR_ARG ||
+        cb200_pbrsa_check_key(p(k.N), k.N.size(), p(sk_.P), sk_.P.size(), p(sk_.Q), sk_.Q.size()) == CB200_ERR_ARG)
+      throw ErrInvalidPrivateKey(cb200_last_error());
+  }
+  size_t KLen() const { return sk_.pub.Size(); }
+  // n blinded rows of KLen bytes back to back, op i under metadata[i] -> n blind signatures; throws
+  // ErrInvalidMessageLength (c > N) or ErrInternal (the s^e' mod N == c check) with the status bytes
+  Bytes BlindSignBatch(const Bytes& blinded, const std::vector<Bytes>& metadata) const {
+    const size_t k = KLen();
+    if (blinded.size() % k || blinded.size() / k != metadata.size()) throw ErrUnexpectedSize();
+    const size_t n = metadata.size();
+    Bytes sig(n * k), meta;
+    std::vector<uint64_t> off;
+    detail::pack(metadata, &meta, &off);
+    std::vector<uint8_t> st(n);
+    if (n) blindrsa::detail::check_call(call(blinded.data(), meta.data(), off.data(), sig.data(), st.data(), n));
+    for (uint8_t bit : {1, 2})
+      for (uint8_t s : st)
+        if (s == bit) {
+          if (bit == 1) throw ErrInvalidMessageLength(st);
+          throw ErrInternal(st);
+        }
+    return sig;
+  }
+  Bytes BlindSign(const Bytes& data, const Bytes& metadata) const {  // pbrsa.go:350-375
+    if (data.size() != KLen()) throw ErrUnexpectedSize();
+    return BlindSignBatch(data, {metadata});
+  }
+
+ private:
+  int call(const uint8_t* in, const uint8_t* meta, const uint64_t* off, uint8_t* out, uint8_t* st, size_t n) const {
+    using blindrsa::detail::p;
+    const PublicKey& k = sk_.pub;
+    return cb200_pbrsa_blind_sign(p(k.N), k.N.size(), p(sk_.P), sk_.P.size(), p(sk_.Q), sk_.Q.size(), p(sk_.Qinv),
+                                  sk_.Qinv.size(), in, meta, off, out, st, n);
+  }
+  PrivateKey sk_;
+};
+
+class Verifier {
+ public:
+  explicit Verifier(PublicKey pk) : pk_(std::move(pk)) {
+    uint8_t z[1] = {0};
+    uint64_t off[1] = {0};
+    if (call(z, off, z, off, z, z, 0) == CB200_ERR_ARG) throw ErrInvalidPublicKey(cb200_last_error());
+  }
+  size_t KLen() const { return pk_.Size(); }
+  // status bytes of messages[i] under metadata[i] against signature row i: 0 valid, 1 s >= N, 2 an inconsistent
+  // encoding; throws ErrVerification with them if any op fails
+  std::vector<uint8_t> VerifyBatch(const std::vector<Bytes>& messages, const std::vector<Bytes>& metadata,
+                                   const Bytes& sigs) const {
+    const size_t n = messages.size();
+    if (sigs.size() != n * KLen() || metadata.size() != n) throw ErrUnexpectedSize();
+    Bytes msgs, meta;
+    std::vector<uint64_t> off, moff;
+    detail::pack(messages, &msgs, &off);
+    detail::pack(metadata, &meta, &moff);
+    std::vector<uint8_t> st(n);
+    if (n) blindrsa::detail::check_call(call(msgs.data(), off.data(), meta.data(), moff.data(), sigs.data(), st.data(), n));
+    for (uint8_t s : st)
+      if (s) throw ErrVerification(st);
+    return st;
+  }
+  void Verify(const Bytes& message, const Bytes& metadata, const Bytes& signature) const {  // pbrsa.go:244-251
+    if (signature.size() != KLen()) throw ErrVerification();
+    VerifyBatch({message}, {metadata}, signature);
+  }
+
+ private:
+  int call(const uint8_t* msgs, const uint64_t* off, const uint8_t* meta, const uint64_t* moff, const uint8_t* sigs,
+           uint8_t* st, size_t n) const {
+    using blindrsa::detail::p;
+    return cb200_pbrsa_verify(p(pk_.N), pk_.N.size(), msgs, off, meta, moff, sigs, st, n);
+  }
+  PublicKey pk_;
+};
+inline Signer NewSigner(const PrivateKey& sk) { return Signer(sk); }
+inline Verifier NewVerifier(const PublicKey& pk) { return Verifier(pk); }
+}  // namespace partiallyblindrsa
 }  // namespace circl
