@@ -94,8 +94,28 @@ def _rows(x, klen):
     return _prep(x, klen, ErrUnexpectedSize(f"blindrsa: rows must be (n, {klen}) uint8"))
 
 
+def _strings(x):
+    """(bytes, offsets, n) of a list of bytes (host arrays) or of (bytes, offsets) CUDA tensors"""
+    if isinstance(x, tuple) and _is_torch(x[0]):
+        data, off = x
+        return data, off, off.shape[0] - 1
+    lens = [len(m) for m in x]
+    off = np.zeros(len(x) + 1, dtype=np.uint64)
+    np.cumsum(lens, out=off[1:])
+    data = np.frombuffer(b"".join(bytes(m) for m in x) or b"\0", dtype=np.uint8).copy()
+    return data, off, len(x)
+
+
 def _host(st):
     return st.cpu().numpy() if _is_torch(st) else st
+
+
+def _raise_sign_status(st, sig, n, scheme):
+    """raises the error of the first failing BlindSign status class (1, then 2) of a batch, if any"""
+    s = _host(st)
+    for bit, cls, what in ((1, ErrInvalidMessageLength, "invalid message length"), (2, ErrInternal, "internal error")):
+        if (s == bit).any():
+            raise cls(f"{scheme}: {what} in {int((s == bit).sum())} of {n} ops", st, sig)
 
 
 class Signer:
@@ -123,10 +143,7 @@ class Signer:
         n = data.shape[0]
         sig, st = _new(data, (n, self.kLen)), _new(data, (n,))
         check(lib().cb200_brsa_blind_sign(*self._args(), _ptr(data), _ptr(sig), _ptr(st), n))
-        s = _host(st)
-        for bit, cls, what in ((1, ErrInvalidMessageLength, "invalid message length"), (2, ErrInternal, "internal error")):
-            if (s == bit).any():
-                raise cls(f"blindrsa: {what} in {int((s == bit).sum())} of {n} ops", st, sig)
+        _raise_sign_status(st, sig, n, "blindrsa")
         return sig
 
     def BlindSign(self, data: bytes) -> bytes:
@@ -155,15 +172,7 @@ class Verifier:
     def VerifyBatch(self, messages, sigs):
         """status bytes (n,) of messages (a list of bytes, or (msgs, msg_off) CUDA tensors: uint8 bytes and n + 1
         int64 offsets) and signatures (n, kLen); raises ErrVerification if any op fails"""
-        if isinstance(messages, tuple) and _is_torch(messages[0]):
-            msgs, off = messages
-            n = off.shape[0] - 1
-        else:
-            lens = [len(m) for m in messages]
-            off = np.zeros(len(messages) + 1, dtype=np.uint64)
-            np.cumsum(lens, out=off[1:])
-            msgs = np.frombuffer(b"".join(bytes(m) for m in messages) or b"\0", dtype=np.uint8).copy()
-            n = len(messages)
+        msgs, off, n = _strings(messages)
         sig = _rows(sigs, self.kLen)
         if sig.shape[0] != n:
             raise ErrUnexpectedSize("blindrsa: one signature per message")

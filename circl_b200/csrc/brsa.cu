@@ -43,15 +43,12 @@ __global__ void __launch_bounds__(128) brsa_verify_kernel(const rsa::VerifyKey<W
   status[i] = m1 < m0 || m1 - m0 > 0x7fffffff ? 2 : (uint8_t)rsa::verify<WN>(msgs + m0, m1 - m0, sig + i * sig_stride, *K);
 }
 
-static inline unsigned blocks(size_t units, size_t per) { return (unsigned)((units + per - 1) / per); }
-
 // ---------------------------------------------------------------- host side
 using namespace rsah;
 
 struct PubKey {
-  Words n;
+  Modulus m;
   uint32_t e;
-  int nbits, klen, wn;
 };
 // N of 2048 to 4096 bits and an odd e with 3 <= e < 2^32
 static int parse_public(const char* fn, const uint8_t* N, size_t N_len, const uint8_t* e, size_t e_len, PubKey* k) {
@@ -59,19 +56,14 @@ static int parse_public(const char* fn, const uint8_t* N, size_t N_len, const ui
     set_error("%s: null key field", fn);
     return CB200_ERR_ARG;
   }
-  Modulus m;
-  int rc = parse_modulus(fn, N, N_len, &m);
+  int rc = parse_modulus(fn, N, N_len, &k->m);
   if (rc) return rc;
-  k->n = m.n;
-  k->nbits = m.nbits;
   const Words ew = be_words(e, e_len);
   if (ew.size() != 1 || ew[0] < 3 || !(ew[0] & 1)) {
     set_error("%s: the public exponent must be odd, at least 3 and below 2^32", fn);
     return CB200_ERR_ARG;
   }
   k->e = ew[0];
-  k->klen = m.klen;
-  k->wn = m.wn;
   return 0;
 }
 
@@ -88,7 +80,7 @@ static int parse_private(const char* fn, const uint8_t* const* f, const size_t* 
       set_error("%s: null key field", fn);
       return CB200_ERR_ARG;
     }
-  rc = parse_primes(fn, k->pub.n, f[2], len[2], f[3], len[3], &k->p, &k->q, &k->wp);
+  rc = parse_primes(fn, k->pub.m.n, f[2], len[2], f[3], len[3], &k->p, &k->q, &k->wp);
   if (rc) return rc;
   k->dp = be_words(f[4], len[4]);
   k->dq = be_words(f[5], len[5]);
@@ -100,68 +92,35 @@ static int parse_private(const char* fn, const uint8_t* const* f, const size_t* 
   return 0;
 }
 
-// the sign body at one pair of word counts: key constants once per call, then run_batch
+// the sign body at one pair of word counts: key constants once per call, then the batch
 template <int WP, int WN>
 static int sign(const char* fn, const PrivKey& k, const uint8_t* blinded, uint8_t* sig, uint8_t* status, size_t n) {
-  using Key = rsa::SignKey<WP, WN>;
-  uint32_t w[WN > WP ? WN : WP];
-  Key K;
-  fill(w, WP, k.p);
-  rsa::mod_init<WP>(K.p, w);
-  fill(w, WP, k.q);
-  rsa::mod_init<WP>(K.q, w);
+  rsa::SignKey<WP, WN> K;
+  load_crt<WP, WN>(K, k.pub.m, k.p, k.q, k.qinv);
   fill(K.dp, WP, k.dp);
   fill(K.dq, WP, k.dq);
-  fill(K.qinv, WP, k.qinv);
-  fill(w, WN, k.pub.n);
-  rsa::mod_init<WN>(K.n, w);
   K.e = k.pub.e;
-  K.klen = k.pub.klen;
-  const size_t kl = (size_t)k.pub.klen;
+  const size_t kl = (size_t)K.klen;
   Batch b{fn, n, sig, 1u << 14, 1u << 10, {{blinded, kl, kl, kIn}, {sig, kl, kl, kOut}, {status, 1, 1, kStatus}}, {}};
-  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) -> int {
-    Arena A;
-    int rc = arena(slot, sizeof(Key), &A);
-    if (rc) return rc;
-    Key* dk = (Key*)A.take(sizeof(Key));
-    CB200_CUDA(cudaMemcpyAsync(dk, &K, sizeof(Key), cudaMemcpyHostToDevice, st));
-    {
-      KernelScope ks(KID_RSA, st);
-      brsa_sign_kernel<WP, WN><<<blocks(cnt, 128), 128, 0, st>>>(dk, r[0].p, r[0].stride, r[1].p, r[1].stride, r[2].p,
-                                                                 cnt);
-    }
-    CB200_CUDA(cudaGetLastError());
-    return 0;
+  return run_keyed(b, K, [&](const rsa::SignKey<WP, WN>* dk, const Rows& r, size_t cnt, cudaStream_t st) {
+    brsa_sign_kernel<WP, WN><<<blocks(cnt, 128), 128, 0, st>>>(dk, r[0].p, r[0].stride, r[1].p, r[1].stride, r[2].p,
+                                                               cnt);
   });
 }
 
 template <int WN>
 static int verify(const char* fn, const PubKey& k, int slen, const uint8_t* msgs, const uint64_t* msg_off,
                   const uint8_t* sigs, uint8_t* status, size_t n) {
-  using Key = rsa::VerifyKey<WN>;
-  uint32_t w[WN];
-  Key K;
-  fill(w, WN, k.n);
-  rsa::mod_init<WN>(K.n, w);
+  rsa::VerifyKey<WN> K;
+  load_mod<WN>(K.n, k.m.n);
   K.e = k.e;
-  K.klen = k.klen;
+  K.klen = k.m.klen;
   K.slen = slen;
-  const size_t kl = (size_t)k.klen;
+  const size_t kl = (size_t)K.klen;
   Batch b{fn, n, sigs, 1u << 14, 1u << 10, {{sigs, kl, kl, kIn}, {status, 1, 1, kStatus}},
           {{!aligned({msg_off}, {}, 8), "%s: device msg_off must be 8-byte aligned"}}, msgs, msg_off};
-  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) -> int {
-    Arena A;
-    int rc = arena(slot, sizeof(Key), &A);
-    if (rc) return rc;
-    Key* dk = (Key*)A.take(sizeof(Key));
-    CB200_CUDA(cudaMemcpyAsync(dk, &K, sizeof(Key), cudaMemcpyHostToDevice, st));
-    {
-      KernelScope ks(KID_RSA, st);
-      brsa_verify_kernel<WN><<<blocks(cnt, 128), 128, 0, st>>>(dk, r.msgs, r.msg_off, r[0].p, r[0].stride, r[1].p,
-                                                               cnt);
-    }
-    CB200_CUDA(cudaGetLastError());
-    return 0;
+  return run_keyed(b, K, [&](const rsa::VerifyKey<WN>* dk, const Rows& r, size_t cnt, cudaStream_t st) {
+    brsa_verify_kernel<WN><<<blocks(cnt, 128), 128, 0, st>>>(dk, r.msgs, r.msg_off, r[0].p, r[0].stride, r[1].p, cnt);
   });
 }
 
@@ -196,14 +155,7 @@ int cb200_brsa_blind_sign(const uint8_t* N, size_t N_len, const uint8_t* e, size
   rc = require_ready();
   if (rc) return rc;
   if (n == 0) return 0;
-  switch (k.wp * 1000 + k.pub.wn) {
-    case 32064: return sign<32, 64>(fn, k, blinded, sig, status, n);
-    case 48064: return sign<48, 64>(fn, k, blinded, sig, status, n);
-    case 48096: return sign<48, 96>(fn, k, blinded, sig, status, n);
-    case 64064: return sign<64, 64>(fn, k, blinded, sig, status, n);
-    case 64096: return sign<64, 96>(fn, k, blinded, sig, status, n);
-    default: return sign<64, 128>(fn, k, blinded, sig, status, n);
-  }
+  return with_words(k.wp, k.pub.m.wn, [&](auto wp, auto wn) { return sign<wp, wn>(fn, k, blinded, sig, status, n); });
 }
 
 int cb200_brsa_verify(int variant, const uint8_t* N, size_t N_len, const uint8_t* e, size_t e_len,
@@ -232,11 +184,7 @@ int cb200_brsa_verify(int variant, const uint8_t* N, size_t N_len, const uint8_t
   const int slen = (variant == CB200_BRSA_SHA384_PSS_RANDOMIZED || variant == CB200_BRSA_SHA384_PSS_DETERMINISTIC)
                        ? rsa::kHash
                        : 0;
-  switch (k.wn) {
-    case 64: return verify<64>(fn, k, slen, msgs, msg_off, sigs, status, n);
-    case 96: return verify<96>(fn, k, slen, msgs, msg_off, sigs, status, n);
-    default: return verify<128>(fn, k, slen, msgs, msg_off, sigs, status, n);
-  }
+  return with_words(k.m.wn, [&](auto wn) { return verify<wn>(fn, k, slen, msgs, msg_off, sigs, status, n); });
 }
 
 }  // extern "C"

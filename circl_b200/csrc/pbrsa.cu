@@ -79,8 +79,6 @@ __global__ void __launch_bounds__(128) pbrsa_verify_kernel(const rsa::PbVerifyKe
   status[i] = bad || bad_lengths(ml, gl) ? 2 : (uint8_t)rsa::pb_verify<WN>(gp, (int)gl, mp, (int)ml, sig + i * sig_stride, *K);
 }
 
-static inline unsigned blocks(size_t units, size_t per) { return (unsigned)((units + per - 1) / per); }
-
 // ---------------------------------------------------------------- host side
 using namespace rsah;
 
@@ -142,41 +140,20 @@ static void salt_states(const Modulus& m, uint64_t (&si)[8], uint64_t (&so)[8]) 
 template <int WP, int WN>
 static int sign(const char* fn, const Key& k, const uint8_t* blinded, const uint8_t* meta, const uint64_t* meta_off,
                 uint8_t* sig, uint8_t* status, size_t n) {
-  using K_t = rsa::PbSignKey<WP, WN>;
-  uint32_t w[WN > WP ? WN : WP];
-  K_t K;
-  fill(w, WP, k.p);
-  rsa::mod_init<WP>(K.p, w);
-  fill(w, WP, k.q);
-  rsa::mod_init<WP>(K.q, w);
+  rsa::PbSignKey<WP, WN> K;
+  load_crt<WP, WN>(K, k.m, k.p, k.q, k.qinv);
   const Words ph = half(k.p), qh = half(k.q);
-  fill(w, WP, ph);
-  rsa::mod_init<WP>(K.ph, w);
-  fill(w, WP, qh);
-  rsa::mod_init<WP>(K.qh, w);
+  load_mod<WP>(K.ph, ph);
+  load_mod<WP>(K.qh, qh);
   fill(K.ph2, WP, minus2(ph));
   fill(K.qh2, WP, minus2(qh));
-  fill(K.qinv, WP, k.qinv);
-  fill(w, WN, k.m.n);
-  rsa::mod_init<WN>(K.n, w);
   salt_states(k.m, K.si, K.so);
-  K.klen = k.m.klen;
-  const size_t kl = (size_t)k.m.klen;
+  const size_t kl = (size_t)K.klen;
   Batch b{fn, n, sig, 1u << 14, 1u << 10, {{blinded, kl, kl, kIn}, {sig, kl, kl, kOut}, {status, 1, 1, kStatus}},
           {{!aligned({meta_off}, {}, 8), "%s: device meta_off must be 8-byte aligned"}}, meta, meta_off};
-  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) -> int {
-    Arena A;
-    int rc = arena(slot, sizeof(K_t), &A);
-    if (rc) return rc;
-    K_t* dk = (K_t*)A.take(sizeof(K_t));
-    CB200_CUDA(cudaMemcpyAsync(dk, &K, sizeof(K_t), cudaMemcpyHostToDevice, st));
-    {
-      KernelScope ks(KID_RSA, st);
-      pbrsa_sign_kernel<WP, WN><<<blocks(cnt, 128), 128, 0, st>>>(dk, r[0].p, r[0].stride, r.msgs, r.msg_off, r[1].p,
-                                                                  r[1].stride, r[2].p, cnt);
-    }
-    CB200_CUDA(cudaGetLastError());
-    return 0;
+  return run_keyed(b, K, [&](const rsa::PbSignKey<WP, WN>* dk, const Rows& r, size_t cnt, cudaStream_t st) {
+    pbrsa_sign_kernel<WP, WN><<<blocks(cnt, 128), 128, 0, st>>>(dk, r[0].p, r[0].stride, r.msgs, r.msg_off, r[1].p,
+                                                                r[1].stride, r[2].p, cnt);
   });
 }
 
@@ -185,31 +162,17 @@ static int sign(const char* fn, const Key& k, const uint8_t* blinded, const uint
 template <int WN>
 static int verify(const char* fn, const Modulus& m, const uint8_t* msgs, const uint64_t* msg_off, const uint8_t* meta,
                   const uint64_t* meta_off, const uint64_t* mlen, const uint8_t* sigs, uint8_t* status, size_t n) {
-  using K_t = rsa::PbVerifyKey<WN>;
-  uint32_t w[WN];
-  K_t K;
-  fill(w, WN, m.n);
-  rsa::mod_init<WN>(K.n, w);
+  rsa::PbVerifyKey<WN> K;
+  load_mod<WN>(K.n, m.n);
   salt_states(m, K.si, K.so);
   K.klen = m.klen;
   const size_t kl = (size_t)m.klen;
   Batch b{fn, n, sigs, 1u << 14, 1u << 10, {{sigs, kl, kl, kIn}, {mlen, 8, 8, kIn}, {status, 1, 1, kStatus}},
           {{!aligned({msg_off, meta_off}, {}, 8), "%s: device msg_off and meta_off must be 8-byte aligned"}}, msgs,
           msg_off};
-  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) -> int {
-    Arena A;
-    int rc = arena(slot, sizeof(K_t), &A);
-    if (rc) return rc;
-    K_t* dk = (K_t*)A.take(sizeof(K_t));
-    CB200_CUDA(cudaMemcpyAsync(dk, &K, sizeof(K_t), cudaMemcpyHostToDevice, st));
-    {
-      KernelScope ks(KID_RSA, st);
-      pbrsa_verify_kernel<WN><<<blocks(cnt, 128), 128, 0, st>>>(dk, r.msgs, r.msg_off, meta, meta_off,
-                                                                (const uint64_t*)r[1].p, r[0].p, r[0].stride, r[2].p,
-                                                                cnt);
-    }
-    CB200_CUDA(cudaGetLastError());
-    return 0;
+  return run_keyed(b, K, [&](const rsa::PbVerifyKey<WN>* dk, const Rows& r, size_t cnt, cudaStream_t st) {
+    pbrsa_verify_kernel<WN><<<blocks(cnt, 128), 128, 0, st>>>(dk, r.msgs, r.msg_off, meta, meta_off,
+                                                              (const uint64_t*)r[1].p, r[0].p, r[0].stride, r[2].p, cnt);
   });
 }
 
@@ -279,14 +242,8 @@ int cb200_pbrsa_blind_sign(const uint8_t* N, size_t N_len, const uint8_t* p, siz
   rc = require_ready();
   if (rc) return rc;
   if (n == 0) return 0;
-  switch (k.wp * 1000 + k.m.wn) {
-    case 32064: return sign<32, 64>(fn, k, blinded, meta, meta_off, sig, status, n);
-    case 48064: return sign<48, 64>(fn, k, blinded, meta, meta_off, sig, status, n);
-    case 48096: return sign<48, 96>(fn, k, blinded, meta, meta_off, sig, status, n);
-    case 64064: return sign<64, 64>(fn, k, blinded, meta, meta_off, sig, status, n);
-    case 64096: return sign<64, 96>(fn, k, blinded, meta, meta_off, sig, status, n);
-    default: return sign<64, 128>(fn, k, blinded, meta, meta_off, sig, status, n);
-  }
+  return with_words(k.wp, k.m.wn,
+                    [&](auto wp, auto wn) { return sign<wp, wn>(fn, k, blinded, meta, meta_off, sig, status, n); });
 }
 
 int cb200_pbrsa_verify(const uint8_t* N, size_t N_len, const uint8_t* msgs, const uint64_t* msg_off,
@@ -341,11 +298,8 @@ int cb200_pbrsa_verify(const uint8_t* N, size_t N_len, const uint8_t* msgs, cons
     meta = nullptr;
     meta_off = nullptr;
   }
-  switch (m.wn) {
-    case 64: return verify<64>(fn, m, msgs, msg_off, meta, meta_off, mlen.empty() ? nullptr : mlen.data(), sigs, status, n);
-    case 96: return verify<96>(fn, m, msgs, msg_off, meta, meta_off, mlen.empty() ? nullptr : mlen.data(), sigs, status, n);
-    default: return verify<128>(fn, m, msgs, msg_off, meta, meta_off, mlen.empty() ? nullptr : mlen.data(), sigs, status, n);
-  }
+  const uint64_t* ml = mlen.empty() ? nullptr : mlen.data();
+  return with_words(m.wn, [&](auto wn) { return verify<wn>(fn, m, msgs, msg_off, meta, meta_off, ml, sigs, status, n); });
 }
 
 }  // extern "C"

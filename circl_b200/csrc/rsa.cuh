@@ -8,11 +8,15 @@
 //   exp_secret    x^d by fixed 4-bit windows over every window of the modulus' bit length, the 16-entry table read
 //                 whole under a mask at each window
 //   exp_public    x^e by left-to-right square-and-multiply on the bits of the public e < 2^32
-//   blind_sign    s_p = c^dp mod p, s_q = c^dq mod q, Garner's recombination with qinv, the check s^e mod N == c
-//   verify        s^e mod N and the EMSA-PSS decode with MGF1-SHA-384
+//   crt_sign      the BlindSign body: s_p = c^d_p mod p and s_q = c^d_q mod q by the caller's exponentiations,
+//                 Garner's recombination with qinv, the check s^e mod N == c by the caller's public exponentiation
+//   pss_verify    the Verify body: s^e mod N by the caller's exponentiation, SHA-384 of the message bytes the caller
+//                 gives and the EMSA-PSS decode with MGF1-SHA-384
+//   blind_sign    crt_sign with dp and dq from the key and its 32-bit e
+//   verify        pss_verify with the 32-bit e and the message as it is
 //   pb_*          partially blind RSA (RSAPBSSA-SHA384, partiallyblindrsa/pbrsa.go): e' from the metadata by
 //                 HKDF-SHA-384, d' by Fermat inversion mod p' = (p - 1) / 2 and q', exp_public_words for the
-//                 multi-word e'; see that section
+//                 multi-word e', on the same two bodies; see that section
 //
 // Secret values (p, q, dp, dq, qinv, s_p, s_q) reach no branch and no address: every loop count and index comes from
 // the word counts and the public bit lengths of p and q, the window digit only forms masks, and the final subtraction
@@ -266,36 +270,43 @@ CB200_XHD void garner(uint32_t* s, const uint32_t* spm, const uint32_t* sq, cons
   for (int j = 0; j < WN; j++) s[j] = acc[j];
 }
 
-// BlindSign of the kLen-byte blinded message c under K: status 0 and s = c^d mod N in out (kLen bytes), or 1 for c > N
-// (ErrInvalidMessageLength) and 2 for s^e mod N != c ("rsa: internal error"), with out all zero
-template <int WP, int WN>
-CB200_XHD uint32_t blind_sign(uint8_t* out, const uint8_t* in, const SignKey<WP, WN>& K) {
+// CRT BlindSign of the kLen-byte blinded message c under K (members p, q, qinv, n, klen), the body of blind_sign and
+// pb_blind_sign: status 0 and s = c^d mod N in out (kLen bytes), or 1 for c > N (ErrInvalidMessageLength) and 2 for
+// s^e mod N != c ("rsa: internal error"), with out all zero.  The caller supplies the exponentiations:
+//   prep()            runs once after the c > N test
+//   half_p(r, cm)     r = c^d_p R mod p from cm = c R mod p; half_q the same mod q
+//   pub(v, sm)        v = s^e R mod N from sm = s R mod N
+template <int WP, int WN, class Key, class Prep, class HalfP, class HalfQ, class Pub>
+CB200_XHD uint32_t crt_sign(uint8_t* out, const uint8_t* in, const Key& K, const Prep& prep, const HalfP& half_p,
+                            const HalfQ& half_q, const Pub& pub) {
   const int klen = K.klen;
   uint32_t c[WN], nw[WN];
   from_be<WN>(c, in, klen);
   for (int j = 0; j < WN; j++) nw[j] = ldk(&K.n.m[j]);
   uint32_t st = cmp<WN>(c, nw) > 0 ? 1u : 0u;
+  prep();
   // c R mod p = c_hi R^3 R^-1 + c_lo R^2 R^-1 with c = c_hi R + c_lo (both below R = 2^(32 WP))
   uint32_t lo[WP], hi[WP], x[WP], y[WP], sp[WP], sq[WP];
   for (int j = 0; j < WP; j++) {
     lo[j] = c[j];
     hi[j] = j + WP < WN ? c[j + WP] : 0;
   }
-  mont_mul<WP>(x, hi, K.p.r3, &K.p);
-  mont_mul<WP>(y, lo, K.p.r2, &K.p);
-  add_mod<WP>(x, x, y, &K.p);
-  exp_secret<WP>(sp, x, K.dp, &K.p);  // s_p R mod p
-  mont_mul<WP>(x, hi, K.q.r3, &K.q);
-  mont_mul<WP>(y, lo, K.q.r2, &K.q);
-  add_mod<WP>(x, x, y, &K.q);
-  exp_secret<WP>(y, x, K.dq, &K.q);  // s_q R mod q
+  auto to_mont = [&](const Mod<WP>& P) {  // x = c R mod P
+    mont_mul<WP>(x, hi, P.r3, &P);
+    mont_mul<WP>(y, lo, P.r2, &P);
+    add_mod<WP>(x, x, y, &P);
+  };
+  to_mont(K.p);
+  half_p(sp, x);  // s_p R mod p
+  to_mont(K.q);
+  half_q(y, x);  // s_q R mod q
   for (int j = 0; j < WP; j++) x[j] = j == 0;
   mont_mul<WP>(sq, y, x, &K.q);  // s_q
   uint32_t s[WN], sm[WN], v[WN];
   garner<WP, WN>(s, sp, sq, K);
   // the check on the full modulus (DecryptAndCheck): s^e mod N must equal c
   mont_mul<WN>(sm, s, K.n.r2, &K.n);
-  exp_public<WN>(v, sm, ldk(&K.e), &K.n);
+  pub(v, sm);
   for (int j = 0; j < WN; j++) sm[j] = j == 0;
   mont_mul<WN>(v, v, sm, &K.n);
   uint32_t diff = 0;
@@ -304,6 +315,16 @@ CB200_XHD uint32_t blind_sign(uint8_t* out, const uint8_t* in, const SignKey<WP,
   const uint32_t keep = st ? 0u : ~0u;
   for (int i = 0; i < klen; i++) out[i] = be_byte(s, klen, i) & keep;
   return st;
+}
+
+// BlindSign of the kLen-byte blinded message c under K: crt_sign with s_p = c^dp mod p, s_q = c^dq mod q and the
+// 32-bit e
+template <int WP, int WN>
+CB200_XHD uint32_t blind_sign(uint8_t* out, const uint8_t* in, const SignKey<WP, WN>& K) {
+  return crt_sign<WP, WN>(
+      out, in, K, [] {}, [&](uint32_t* r, const uint32_t* cm) { exp_secret<WP>(r, cm, K.dp, &K.p); },
+      [&](uint32_t* r, const uint32_t* cm) { exp_secret<WP>(r, cm, K.dq, &K.q); },
+      [&](uint32_t* v, const uint32_t* sm) { exp_public<WN>(v, sm, ldk(&K.e), &K.n); });
 }
 
 // ---------------------------------------------------------------- Verify
@@ -354,23 +375,38 @@ CB200_XHD uint32_t emsa_pss_verify(const uint32_t* m, int klen, int nbits, const
   return bad ? 2 : 0;
 }
 
-// Verify of the message msg[0 .. len) and the kLen-byte signature sig under K: 0, 1 for s >= N, 2 for an inconsistent
-// encoding (both rsa.ErrVerification in the reference)
-template <int WN>
-CB200_XHD uint32_t verify(const uint8_t* msg, uint64_t len, const uint8_t* sig, const VerifyKey<WN>& K) {
+// Verify of the kLen-byte signature sig under K (members n, klen), the body of verify and pb_verify, for the message
+// of len bytes whose byte j is msg(j), with a salt of salt_len(K) bytes: 0, 1 for s >= N, 2 for an inconsistent
+// encoding (both rsa.ErrVerification in the reference).  prep() runs once after the s >= N test; pub(v, sm) gives
+// v = s^e R mod N from sm = s R mod N.
+template <int WN, class Key, class Prep, class Pub, class Msg>
+CB200_XHD uint32_t pss_verify(const uint8_t* sig, const Key& K, const Prep& prep, const Pub& pub, uint64_t len,
+                              const Msg& msg) {
   const int klen = K.klen;
   uint32_t s[WN], nw[WN], sm[WN], v[WN];
   from_be<WN>(s, sig, klen);
   for (int j = 0; j < WN; j++) nw[j] = ldk(&K.n.m[j]);
   if (cmp<WN>(s, nw) >= 0) return 1;
+  prep();
   mont_mul<WN>(sm, s, K.n.r2, &K.n);
-  exp_public<WN>(v, sm, ldk(&K.e), &K.n);
+  pub(v, sm);
   for (int j = 0; j < WN; j++) sm[j] = j == 0;
   mont_mul<WN>(v, v, sm, &K.n);
   uint64_t mh[8];
   sha2::Sha384::iv(mh);
-  sha2::absorb<sha2::Sha384>(mh, 0, (int)len, [&](int j) -> uint8_t { return msg[j]; });
-  return emsa_pss_verify<WN>(v, klen, ldk((const uint32_t*)&K.n.bits), mh, ldk((const uint32_t*)&K.slen));
+  sha2::absorb<sha2::Sha384>(mh, 0, (int)len, msg);
+  return emsa_pss_verify<WN>(v, klen, ldk((const uint32_t*)&K.n.bits), mh, salt_len(K));
+}
+
+// RSABSSA-SHA384's salt: 48 bytes or none by the variant
+template <int WN>
+CB200_XHD int salt_len(const VerifyKey<WN>& K) { return ldk((const uint32_t*)&K.slen); }
+// Verify of the message msg[0 .. len) and the kLen-byte signature sig under K: pss_verify with the 32-bit e
+template <int WN>
+CB200_XHD uint32_t verify(const uint8_t* msg, uint64_t len, const uint8_t* sig, const VerifyKey<WN>& K) {
+  return pss_verify<WN>(
+      sig, K, [] {}, [&](uint32_t* v, const uint32_t* sm) { exp_public<WN>(v, sm, ldk(&K.e), &K.n); }, len,
+      [&](int j) -> uint8_t { return msg[j]; });
 }
 
 // ---------------------------------------------------------------- partially blind RSA (RSAPBSSA-SHA384)
@@ -486,75 +522,42 @@ CB200_XHD void pb_half(uint32_t* sm, const uint32_t* cm, const uint32_t* e, cons
   exp_secret_own<WP>(sm, cm, d, &P);
 }
 
-// BlindSign (pbrsa.go:350-375) of the kLen-byte blinded message c under the key of meta[0 .. mlen): status 0 and
-// s = c^d' mod N in out, or 1 for c > N (ErrInvalidMessageLength) and 2 for s^e' mod N != c (DecryptAndCheck's
-// "rsa: internal error"), with out all zero
+// BlindSign (pbrsa.go:350-375) of the kLen-byte blinded message c under the key of meta[0 .. mlen): crt_sign with e'
+// derived once c has been read, d'_p and d'_q by pb_half, and the check s^e' mod N == c
 template <int WP, int WN>
 CB200_XHD uint32_t pb_blind_sign(uint8_t* out, const uint8_t* in, const uint8_t* meta, int mlen,
                                  const PbSignKey<WP, WN>& K) {
-  const int klen = K.klen, nbits = ldk((const uint32_t*)&K.n.bits);
-  uint32_t c[WN], nw[WN];
-  from_be<WN>(c, in, klen);
-  for (int j = 0; j < WN; j++) nw[j] = ldk(&K.n.m[j]);
-  uint32_t st = cmp<WN>(c, nw) > 0 ? 1u : 0u;
+  const int nbits = ldk((const uint32_t*)&K.n.bits);
   uint32_t e[WP];
-  derive_exponent<WN>(e, nbits, meta, mlen, K.si, K.so);
-  for (int j = WN / 2; j < WP; j++) e[j] = 0;
-  // c R mod p and c R mod q as in blind_sign
-  uint32_t lo[WP], hi[WP], x[WP], y[WP], sp[WP], sq[WP];
-  for (int j = 0; j < WP; j++) {
-    lo[j] = c[j];
-    hi[j] = j + WP < WN ? c[j + WP] : 0;
-  }
-  auto to_mont = [&](const Mod<WP>& P) {
-    mont_mul<WP>(x, hi, P.r3, &P);
-    mont_mul<WP>(y, lo, P.r2, &P);
-    add_mod<WP>(x, x, y, &P);
-  };
-  to_mont(K.p);
-  pb_half<WP>(sp, x, e, K.p, K.ph, K.ph2);  // s_p R mod p
-  to_mont(K.q);
-  pb_half<WP>(y, x, e, K.q, K.qh, K.qh2);  // s_q R mod q
-  for (int j = 0; j < WP; j++) x[j] = j == 0;
-  mont_mul<WP>(sq, y, x, &K.q);
-  uint32_t s[WN], sm[WN], v[WN];
-  garner<WP, WN>(s, sp, sq, K);
-  mont_mul<WN>(sm, s, K.n.r2, &K.n);
-  exp_public_words<WN>(v, sm, e, pb_exp_bits(nbits), &K.n);
-  for (int j = 0; j < WN; j++) sm[j] = j == 0;
-  mont_mul<WN>(v, v, sm, &K.n);
-  uint32_t diff = 0;
-  for (int j = 0; j < WN; j++) diff |= v[j] ^ c[j];
-  if (!st && diff) st = 2;
-  const uint32_t keep = st ? 0u : ~0u;
-  for (int i = 0; i < klen; i++) out[i] = be_byte(s, klen, i) & keep;
-  return st;
+  return crt_sign<WP, WN>(
+      out, in, K,
+      [&] {
+        derive_exponent<WN>(e, nbits, meta, mlen, K.si, K.so);
+        for (int j = WN / 2; j < WP; j++) e[j] = 0;
+      },
+      [&](uint32_t* r, const uint32_t* cm) { pb_half<WP>(r, cm, e, K.p, K.ph, K.ph2); },
+      [&](uint32_t* r, const uint32_t* cm) { pb_half<WP>(r, cm, e, K.q, K.qh, K.qh2); },
+      [&](uint32_t* v, const uint32_t* sm) { exp_public_words<WN>(v, sm, e, pb_exp_bits(nbits), &K.n); });
 }
 
+// RSAPBSSA-SHA384's salt: 48 bytes
+template <int WN>
+CB200_XHD int salt_len(const PbVerifyKey<WN>&) { return kHash; }
 // Verify (pbrsa.go:244-251) of msg[0 .. len) under the metadata meta[0 .. mlen) and the kLen-byte signature: the
-// message framed as "msg" || I2OSP(mlen, 4) || meta || msg, RSA-PSS-SHA-384 with a 48-byte salt under (N, e').
-// 0, 1 for s >= N, 2 for an inconsistent encoding.  7 + mlen + len < 2^31.
+// message framed as "msg" || I2OSP(mlen, 4) || meta || msg, pss_verify under (N, e').  7 + mlen + len < 2^31.
 template <int WN>
 CB200_XHD uint32_t pb_verify(const uint8_t* msg, int len, const uint8_t* meta, int mlen, const uint8_t* sig,
                              const PbVerifyKey<WN>& K) {
-  const int klen = K.klen, nbits = ldk((const uint32_t*)&K.n.bits);
-  uint32_t s[WN], nw[WN], sm[WN], v[WN], e[WN / 2];
-  from_be<WN>(s, sig, klen);
-  for (int j = 0; j < WN; j++) nw[j] = ldk(&K.n.m[j]);
-  if (cmp<WN>(s, nw) >= 0) return 1;
-  derive_exponent<WN>(e, nbits, meta, mlen, K.si, K.so);
-  mont_mul<WN>(sm, s, K.n.r2, &K.n);
-  exp_public_words<WN>(v, sm, e, pb_exp_bits(nbits), &K.n);
-  for (int j = 0; j < WN; j++) sm[j] = j == 0;
-  mont_mul<WN>(v, v, sm, &K.n);
-  uint64_t mh[8];
-  sha2::Sha384::iv(mh);
-  sha2::absorb<sha2::Sha384>(mh, 0, 7 + mlen + len, [&](int j) -> uint8_t {
-    if (j < 3) return (uint8_t)"msg"[j];
-    if (j < 7) return (uint8_t)((uint32_t)mlen >> (8 * (6 - j)));
-    return j - 7 < mlen ? meta[j - 7] : msg[j - 7 - mlen];
-  });
-  return emsa_pss_verify<WN>(v, klen, nbits, mh, kHash);
+  const int nbits = ldk((const uint32_t*)&K.n.bits);
+  uint32_t e[WN / 2];
+  return pss_verify<WN>(
+      sig, K, [&] { derive_exponent<WN>(e, nbits, meta, mlen, K.si, K.so); },
+      [&](uint32_t* v, const uint32_t* sm) { exp_public_words<WN>(v, sm, e, pb_exp_bits(nbits), &K.n); },
+      7 + mlen + len, [&](int j) -> uint8_t {
+        if (j < 3) return (uint8_t)"msg"[j];
+        if (j < 7) return (uint8_t)((uint32_t)mlen >> (8 * (6 - j)));
+        return j - 7 < mlen ? meta[j - 7] : msg[j - 7 - mlen];
+      });
 }
 
 // ---------------------------------------------------------------- host preparation

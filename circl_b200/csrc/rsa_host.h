@@ -1,12 +1,17 @@
 // Host side of the RSA entry points (brsa.cu, pbrsa.cu): multi-precision values as word vectors, the word counts that
-// serve a key, and the checks of the modulus and its two primes.
+// serve a key, the checks of the modulus and its two primes, the key structs' CRT part, and the launch of a batch
+// under the call's key.
 #pragma once
 #include <algorithm>
 #include <cstdint>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/circl_b200.h"
 #include "common.cuh"
+#include "context.h"
+#include "flow_internal.h"
+#include "rsa.cuh"
 
 namespace cb200 {
 namespace rsah {
@@ -90,6 +95,69 @@ inline int parse_primes(const char* fn, const Words& n, const uint8_t* P, size_t
     return CB200_ERR_ARG;
   }
   return 0;
+}
+
+// a word count as a type, so that a generic lambda can use it as a template argument
+template <int W>
+using WordCount = std::integral_constant<int, W>;
+// f(WP, WN) for the word counts of a sign key: the five served pairs below, else (64, 128)
+template <class F>
+int with_words(int wp, int wn, const F& f) {
+  switch (wp * 1000 + wn) {
+    case 32064: return f(WordCount<32>(), WordCount<64>());
+    case 48064: return f(WordCount<48>(), WordCount<64>());
+    case 48096: return f(WordCount<48>(), WordCount<96>());
+    case 64064: return f(WordCount<64>(), WordCount<64>());
+    case 64096: return f(WordCount<64>(), WordCount<96>());
+    default: return f(WordCount<64>(), WordCount<128>());
+  }
+}
+// f(WN) for the word count of N: 64, 96, else 128
+template <class F>
+int with_words(int wn, const F& f) {
+  switch (wn) {
+    case 64: return f(WordCount<64>());
+    case 96: return f(WordCount<96>());
+    default: return f(WordCount<128>());
+  }
+}
+
+// M of the value x (at most W words)
+template <int W>
+void load_mod(rsa::Mod<W>& M, const Words& x) {
+  uint32_t w[W];
+  fill(w, W, x);
+  rsa::mod_init<W>(M, w);
+}
+// the CRT part of a sign key (rsa::SignKey or rsa::PbSignKey): p, q, qinv, N and klen
+template <int WP, int WN, class Key>
+void load_crt(Key& K, const Modulus& m, const Words& p, const Words& q, const Words& qinv) {
+  load_mod<WP>(K.p, p);
+  load_mod<WP>(K.q, q);
+  fill(K.qinv, WP, qinv);
+  load_mod<WN>(K.n, m.n);
+  K.klen = m.klen;
+}
+
+inline unsigned blocks(size_t units, size_t per) { return (unsigned)((units + per - 1) / per); }
+
+// run_batch under the call's key K: every sub-batch copies K into its slot's level-1 work area and starts its kernel
+// by launch(dk, rows, count, st) with dk the device copy, timed under the profiling class rsa
+template <class Key, class Launch>
+int run_keyed(const Batch& b, const Key& K, const Launch& launch) {
+  return run_batch(b, [&](const Rows& r, size_t cnt, cudaStream_t st, int slot) -> int {
+    Arena A;
+    int rc = arena(slot, sizeof(Key), &A);
+    if (rc) return rc;
+    Key* dk = (Key*)A.take(sizeof(Key));
+    CB200_CUDA(cudaMemcpyAsync(dk, &K, sizeof(Key), cudaMemcpyHostToDevice, st));
+    {
+      KernelScope ks(KID_RSA, st);
+      launch(dk, r, cnt, st);
+    }
+    CB200_CUDA(cudaGetLastError());
+    return 0;
+  });
 }
 
 }  // namespace rsah

@@ -26,8 +26,8 @@ import numpy as np
 
 from ._ffi import check, lib
 from .blindrsa import (BlindRSAError, ErrInternal, ErrInvalidMessageLength, ErrUnexpectedSize, ErrVerification,
-                       PrivateKey, PublicKey, _be, _host, _rows)
-from .hybrid import _is_torch, _new, _ptr
+                       PrivateKey, PublicKey, _be, _host, _raise_sign_status, _rows, _strings)
+from .hybrid import _new, _ptr
 
 __all__ = ["SHA384", "NewSigner", "NewVerifier", "Signer", "Verifier", "PrivateKey", "PublicKey",
            "ErrInvalidPrivateKey", "ErrInvalidPublicKey", "ErrUnexpectedSize", "ErrInvalidMessageLength", "ErrInternal",
@@ -47,18 +47,6 @@ class ErrInvalidPublicKey(BlindRSAError):  # partiallyblindrsa.ErrInvalidPublicK
 def _check_hash(h):
     if h != SHA384:
         raise ValueError("partiallyblindrsa: only SHA384 is served")
-
-
-def _strings(x):
-    """(bytes, offsets, n) of a list of bytes (host arrays) or of (bytes, offsets) CUDA tensors"""
-    if isinstance(x, tuple) and _is_torch(x[0]):
-        data, off = x
-        return data, off, off.shape[0] - 1
-    lens = [len(m) for m in x]
-    off = np.zeros(len(x) + 1, dtype=np.uint64)
-    np.cumsum(lens, out=off[1:])
-    data = np.frombuffer(b"".join(bytes(m) for m in x) or b"\0", dtype=np.uint8).copy()
-    return data, off, len(x)
 
 
 class Signer:
@@ -97,10 +85,7 @@ class Signer:
         if n:
             check(lib().cb200_pbrsa_blind_sign(*self._key(), _ptr(data), _ptr(meta), _ptr(off), _ptr(sig), _ptr(st),
                                                n))
-        s = _host(st)
-        for bit, cls, what in ((1, ErrInvalidMessageLength, "invalid message length"), (2, ErrInternal, "internal error")):
-            if (s == bit).any():
-                raise cls(f"partiallyblindrsa: {what} in {int((s == bit).sum())} of {n} ops", st, sig)
+        _raise_sign_status(st, sig, n, "partiallyblindrsa")
         return sig
 
     def BlindSign(self, data: bytes, metadata: bytes) -> bytes:

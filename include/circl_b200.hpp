@@ -1001,6 +1001,24 @@ inline void check_call(int rc) {
   if (rc == CB200_ERR_ARG) throw std::logic_error(cb200_last_error());
   if (rc != 0) throw Error(cb200_last_error());
 }
+// strings back to back with their n + 1 offsets; the blob is never empty
+inline void pack(const std::vector<Bytes>& v, Bytes* blob, std::vector<uint64_t>* off) {
+  off->assign(v.size() + 1, 0);
+  for (size_t i = 0; i < v.size(); i++) {
+    blob->insert(blob->end(), v[i].begin(), v[i].end());
+    (*off)[i + 1] = blob->size();
+  }
+  blob->push_back(0);
+}
+// BlindSign status bytes: throws ErrInvalidMessageLength if any op has status 1, else ErrInternal if any has 2
+inline void throw_sign_status(const std::vector<uint8_t>& st) {
+  for (uint8_t bit : {1, 2})
+    for (uint8_t s : st)
+      if (s == bit) {
+        if (bit == 1) throw ErrInvalidMessageLength(st);
+        throw ErrInternal(st);
+      }
+}
 }  // namespace detail
 
 class Signer {
@@ -1019,12 +1037,7 @@ class Signer {
     Bytes sig(n * k);
     std::vector<uint8_t> st(n);
     if (n) detail::check_call(call(blinded.data(), sig.data(), st.data(), n));
-    for (uint8_t bit : {1, 2})
-      for (uint8_t s : st)
-        if (s == bit) {
-          if (bit == 1) throw ErrInvalidMessageLength(st);
-          throw ErrInternal(st);
-        }
+    detail::throw_sign_status(st);
     return sig;
   }
   Bytes BlindSign(const Bytes& data) const {  // brsa.go:237-257
@@ -1057,13 +1070,9 @@ class Verifier {
   std::vector<uint8_t> VerifyBatch(const std::vector<Bytes>& messages, const Bytes& sigs) const {
     const size_t n = messages.size(), k = KLen();
     if (sigs.size() != n * k) throw ErrUnexpectedSize();
-    std::vector<uint64_t> off(n + 1, 0);
     Bytes blob;
-    for (size_t i = 0; i < n; i++) {
-      blob.insert(blob.end(), messages[i].begin(), messages[i].end());
-      off[i + 1] = blob.size();
-    }
-    blob.push_back(0);  // never empty
+    std::vector<uint64_t> off;
+    detail::pack(messages, &blob, &off);
     std::vector<uint8_t> st(n);
     if (n) detail::check_call(call(blob.data(), off.data(), sigs.data(), st.data(), n));
     for (uint8_t s : st)
@@ -1107,18 +1116,6 @@ struct ErrInvalidPublicKey : BlindRSAError {
   explicit ErrInvalidPublicKey(const std::string& m) : BlindRSAError(m) {}
 };
 
-namespace detail {
-// strings back to back with their n + 1 offsets; the blob is never empty
-inline void pack(const std::vector<Bytes>& v, Bytes* blob, std::vector<uint64_t>* off) {
-  off->assign(v.size() + 1, 0);
-  for (size_t i = 0; i < v.size(); i++) {
-    blob->insert(blob->end(), v[i].begin(), v[i].end());
-    (*off)[i + 1] = blob->size();
-  }
-  blob->push_back(0);
-}
-}  // namespace detail
-
 class Signer {
  public:
   explicit Signer(PrivateKey sk) : sk_(std::move(sk)) {
@@ -1139,15 +1136,10 @@ class Signer {
     const size_t n = metadata.size();
     Bytes sig(n * k), meta;
     std::vector<uint64_t> off;
-    detail::pack(metadata, &meta, &off);
+    blindrsa::detail::pack(metadata, &meta, &off);
     std::vector<uint8_t> st(n);
     if (n) blindrsa::detail::check_call(call(blinded.data(), meta.data(), off.data(), sig.data(), st.data(), n));
-    for (uint8_t bit : {1, 2})
-      for (uint8_t s : st)
-        if (s == bit) {
-          if (bit == 1) throw ErrInvalidMessageLength(st);
-          throw ErrInternal(st);
-        }
+    blindrsa::detail::throw_sign_status(st);
     return sig;
   }
   Bytes BlindSign(const Bytes& data, const Bytes& metadata) const {  // pbrsa.go:350-375
@@ -1181,8 +1173,8 @@ class Verifier {
     if (sigs.size() != n * KLen() || metadata.size() != n) throw ErrUnexpectedSize();
     Bytes msgs, meta;
     std::vector<uint64_t> off, moff;
-    detail::pack(messages, &msgs, &off);
-    detail::pack(metadata, &meta, &moff);
+    blindrsa::detail::pack(messages, &msgs, &off);
+    blindrsa::detail::pack(metadata, &meta, &moff);
     std::vector<uint8_t> st(n);
     if (n) blindrsa::detail::check_call(call(msgs.data(), off.data(), meta.data(), moff.data(), sigs.data(), st.data(), n));
     for (uint8_t s : st)
