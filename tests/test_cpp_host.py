@@ -6,28 +6,29 @@ import subprocess
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXE = os.path.join(ROOT, "tests", "cpp", "test_scheme")
 
 
-def build_exe():
+def build_exe(out_dir):
+    """Link tests/cpp/test_scheme.cpp against the library into out_dir: the source tree may be read-only."""
     from circl_b200 import _ffi
     assert os.path.exists(_ffi.LIB_PATH)
+    exe = os.path.join(str(out_dir), "test_scheme")
     cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-I", os.path.join(ROOT, "include"),
-           os.path.join(ROOT, "tests", "cpp", "test_scheme.cpp"), "-o", EXE,
+           os.path.join(ROOT, "tests", "cpp", "test_scheme.cpp"), "-o", exe,
            "-L", os.path.join(ROOT, "circl_b200"), "-lcirclb200", "-Wl,-rpath," + os.path.join(ROOT, "circl_b200")]
     r = subprocess.run(cmd, capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
-    return EXE
+    return exe
 
 
-def test_cpp_host_layer_compiles_and_links():
-    build_exe()
+def test_cpp_host_layer_compiles_and_links(tmp_path):
+    build_exe(tmp_path)
 
 
 @pytest.mark.gpu
-def test_cpp_host_layer_matches_oracle():
+def test_cpp_host_layer_matches_oracle(tmp_path):
     import oracle
-    exe = build_exe()
+    exe = build_exe(tmp_path)
     r = subprocess.run([exe], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "ALL OK" in r.stdout

@@ -1,6 +1,8 @@
 """circl_b200/csrc/ed25519.cuh compiled for the host (g++, no GPU) through tests/cpp/test_ed25519_host.cpp: SHA-512
-against hashlib, scalars mod L against Python integers, point decoding edge cases, and keygen / sign / verify against
-OpenSSL's Ed25519 (the `cryptography` package) and the reference's RFC 8032 and Wycheproof vectors."""
+against hashlib, scalars mod L against Python integers, point decoding edge cases, keygen / sign / verify against
+OpenSSL's Ed25519 (the `cryptography` package) and the reference's RFC 8032 and Wycheproof vectors, and decoding, the
+double multiplication and verify on small-order and mixed-order keys and non-canonical encodings against the
+Python-integer model (tests/ed25519_model.py)."""
 import hashlib
 import os
 import random
@@ -8,12 +10,12 @@ import subprocess
 
 import pytest
 
+import ed25519_model as M
 from conftest import load_golden
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 P = 2**255 - 19
 L = 2**252 + 27742317777372353535851937790883648493
-D = (-121665 * pow(121666, P - 2, P)) % P
 
 
 @pytest.fixture(scope="module")
@@ -69,22 +71,6 @@ def test_calculate_s(run):
     assert run(["canon " + _le(s) for s in ss]) == ["1" if s < L else "0" for s in ss]
 
 
-def _recover_x(y, sign):
-    if y >= P:
-        return None
-    x2 = (y * y - 1) * pow(D * y * y + 1, P - 2, P) % P
-    if x2 == 0:
-        return None if sign else 0
-    x = pow(x2, (P + 3) // 8, P)
-    if (x * x - x2) % P:
-        x = x * pow(2, (P - 1) // 4, P) % P
-    if (x * x - x2) % P:
-        return None
-    if x & 1 != sign:
-        x = P - x
-    return x
-
-
 def test_decode_edge_cases(run):
     rng = random.Random(4)
     ys = [(0, 0), (1, 0), (1, 1), (P - 1, 0), (P - 1, 1), (P, 0), (P + 1, 0), (2**255 - 1, 0), (2**255 - 1, 1), (2, 0)]
@@ -92,12 +78,12 @@ def test_decode_edge_cases(run):
     got = run(["decode " + _le(y | (s << 255)) for y, s in ys])
     n_bad = 0
     for (y, s), g in zip(ys, got):
-        x = _recover_x(y, s)
-        if x is None:
+        pt = M.decode(bytes.fromhex(_le(y | (s << 255))))
+        if pt is None:
             assert g == "0", (y, s)
             n_bad += 1
         else:
-            assert g == "1" + _le(y | ((x & 1) << 255)), (y, s)
+            assert g == "1" + M.encode(pt).hex(), (y, s)
     assert 50 < n_bad < 190  # about half of the random y have no square root
 
 
@@ -157,3 +143,31 @@ def test_rfc8032_and_wycheproof_vectors(run):
         lines.append("verify %s %s %s" % (t["pk"], _h(bytes.fromhex(t["msg"])), t["sig"]))
         exp.append("1" if t["valid"] else "0")
     assert run(lines) == exp
+
+
+def test_decode_torsion_and_non_canonical_encodings(run):
+    """The 8 points of order dividing 8 decode to themselves; the 38 encodings with y >= p, and x = 0 with the sign
+    bit (y = 1, y = p - 1), are rejected."""
+    tors = [M.encode(T) for T in M.TORSION]
+    assert run(["decode " + e.hex() for e in tors]) == ["1" + e.hex() for e in tors]
+    bad = [y | s << 255 for y in range(P, 2**255) for s in (0, 1)] + [1 | 1 << 255, P - 1 | 1 << 255]
+    assert len(bad) == 40 and all(M.decode(bytes.fromhex(_le(v))) is None for v in bad)
+    assert run(["decode " + _le(v) for v in bad]) == ["0"] * 40
+
+
+def test_double_mult_small_order_points(run):
+    """encode([s] B + [k] T) for every T of order dividing 8, at k around multiples of 8 and at random k, where the
+    table of the multiples 1..8 T passes through the identity."""
+    rng = random.Random(8)
+    ks = [0, 1, 2, 3, 4, 7, 8, 9, 15, 16, 17, L - 1, 2**252] + [rng.randrange(L) for _ in range(4)]
+    cases = [(rng.randrange(L), k, j) for j in range(8) for k in ks]
+    got = run(["dmul %s %s %s" % (_le(s), _le(k), M.encode(M.TORSION[j]).hex()) for s, k, j in cases])
+    sB = {s: M.mul(s, M.B) for s, _, _ in cases}
+    assert got == [M.encode(M.add(sB[s], M.TORSION[(k * j) % 8])).hex() for s, k, j in cases]
+
+
+def test_torsion_cases_against_model(run):
+    """verify gives the model's verdict on every small-order, mixed-order and non-canonical case."""
+    cases = M.torsion_cases()
+    got = run(["verify %s %s %s" % (pk.hex(), _h(msg), sig.hex()) for _, pk, msg, sig, _ in cases])
+    assert got == ["1" if c[4] else "0" for c in cases], [c[0] for c, g in zip(cases, got) if g != ("1" if c[4] else "0")]

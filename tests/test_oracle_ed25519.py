@@ -1,11 +1,13 @@
 """CPU: the Ed25519 / Ed25519-Dilithium2 oracle (oracle/ed25519.c) against the reference's RFC 8032, sign.input and
-Wycheproof vectors, OpenSSL's Ed25519 and hashlib, and the composite rebuilt from OpenSSL Ed25519 + hashlib SHAKE256 +
-the oracle's round-3 Dilithium2."""
+Wycheproof vectors, OpenSSL's Ed25519 and hashlib, the composite rebuilt from OpenSSL Ed25519 + hashlib SHAKE256 +
+the oracle's round-3 Dilithium2, and the Python-integer model (tests/ed25519_model.py) on small-order and mixed-order
+keys and non-canonical encodings."""
 import hashlib
 import random
 
 import pytest
 
+import ed25519_model as M
 from conftest import load_golden
 
 L = 2**252 + 27742317777372353535851937790883648493
@@ -96,3 +98,66 @@ def test_eddilithium2_rebuilt_from_parts(oe):
             bad[pos] ^= 1
             assert not oe.eddilithium2_verify(pk, msg, bytes(bad))
         assert not oe.eddilithium2_verify(pk, msg, sig[:-1])
+
+
+@pytest.fixture(scope="module")
+def cases():
+    return M.torsion_cases()
+
+
+def test_model_against_openssl_and_vectors():
+    """The model's public / sign equal OpenSSL's on random seeds, its verify accepts them and rejects a flipped bit,
+    and it gives every Wycheproof verdict."""
+    rng = random.Random(8)
+    for n in (0, 1, 64, 200):
+        seed = bytes(rng.randrange(256) for _ in range(32))
+        msg = bytes(rng.randrange(256) for _ in range(n))
+        k = _ossl(seed)
+        A = M.public(seed)
+        assert A == k.public_key().public_bytes_raw()
+        sig = M.sign(seed, A, msg)
+        assert sig == k.sign(msg) and M.verify(A, msg, sig)
+        assert not M.verify(A, msg, sig[:7] + bytes([sig[7] ^ 4]) + sig[8:])
+    for t in load_golden("ed25519_vectors.json.gz")["wycheproof"]:
+        assert M.verify(bytes.fromhex(t["pk"]), bytes.fromhex(t["msg"]), bytes.fromhex(t["sig"])) == t["valid"], t["tcId"]
+
+
+def test_torsion_cases_cover_every_order(cases):
+    """Low-order keys of every order, mixed-order keys with T of order 2, 4 and 8, both verdicts for each nonzero
+    order, and all 38 encodings with y >= p."""
+    low, mixed = {}, {}
+    for name, pk, msg, sig, want in cases:
+        A = M.decode(pk)
+        if A is None:
+            continue
+        n = M.order(A)
+        if n:
+            low.setdefault(n, set()).add(want)
+        elif M.order(M.mul(M.L, A)) > 1:
+            mixed.setdefault(M.order(M.mul(M.L, A)), set()).add(want)
+    assert set(low) == {1, 2, 4, 8} and all(low[n] == {True, False} for n in (2, 4, 8))
+    assert mixed == {2: {True, False}, 4: {True, False}, 8: {True, False}}
+    big = {pk for _, pk, _, _, _ in cases if int.from_bytes(pk, "little") & (2**255 - 1) >= M.P}
+    assert len(big) == 38
+
+
+def test_torsion_cases(oe, cases):
+    """The oracle gives the model's verdict on every small-order, mixed-order and non-canonical case."""
+    got = [oe.ed25519_verify(pk, msg, sig) for _, pk, msg, sig, _ in cases]
+    assert got == [c[4] for c in cases], [c[0] for c, g in zip(cases, got) if g != c[4]]
+
+
+def test_eddilithium2_torsion_cases(oe, cases):
+    """With a valid Dilithium2 half, the composite's verdict is the model's verdict on the Ed25519 half; with a
+    corrupted one it is false."""
+    import oracle
+    dpk, dsk = oracle.mldsa_keygen(2, bytes(range(32)))
+    got = []
+    for name, pk, msg, sig, want in cases:
+        dsig = oracle.mldsa_sign(2, dsk, msg)[0]
+        got.append(oe.eddilithium2_verify(dpk + pk, msg, dsig + sig))
+        if want:
+            bad = bytearray(dsig)
+            bad[100] ^= 1
+            assert not oe.eddilithium2_verify(dpk + pk, msg, bytes(bad) + sig), name
+    assert got == [c[4] for c in cases]
