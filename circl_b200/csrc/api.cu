@@ -60,7 +60,7 @@ static const char* kKernelNames[KID_COUNT] = {
     "dil_ntt", "dil_invntt", "dil_dot", "dil_elementwise",
     "mldsa_expand_key", "mldsa_mu_rhoprime", "mldsa_mask", "mldsa_w", "mldsa_challenge", "mldsa_response",
     "mldsa_compact", "x25519", "hybrid_glue", "keccak_f1600", "sampler", "mlkem_sample_fix", "x448", "ed25519", "ed448",
-    "hpke", "frodo", "frodo_gemm", "p256", "p384", "p521", "rsa"};
+    "hpke", "frodo", "frodo_gemm", "p256", "p384", "p521", "rsa", "prio3"};
 const char* kernel_name(int id) { return (id >= 0 && id < KID_COUNT) ? kKernelNames[id] : "?"; }
 
 KernelScope::KernelScope(int id_, cudaStream_t st_) : st(st_), id(id_) {

@@ -109,7 +109,7 @@ enum KernelId {
   KID_DIL_NTT, KID_DIL_INVNTT, KID_DIL_DOT, KID_DIL_EW,
   KID_MLDSA_EXPAND, KID_MLDSA_MU, KID_MLDSA_MASK, KID_MLDSA_W, KID_MLDSA_CHALLENGE, KID_MLDSA_RESPONSE,
   KID_MLDSA_COMPACT, KID_X25519, KID_HYBRID_GLUE, KID_KECCAK, KID_SAMPLER, KID_MLKEM_SAMPLE_FIX, KID_X448, KID_ED25519, KID_ED448,
-  KID_HPKE, KID_FRODO, KID_FRODO_GEMM, KID_P256, KID_P384, KID_P521, KID_RSA, KID_COUNT
+  KID_HPKE, KID_FRODO, KID_FRODO_GEMM, KID_P256, KID_P384, KID_P521, KID_RSA, KID_PRIO3, KID_COUNT
 };
 const char* kernel_name(int id);
 

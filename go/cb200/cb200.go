@@ -11,6 +11,7 @@ package cb200
 /*
 #cgo CFLAGS: -I${SRCDIR}/../../include
 #cgo LDFLAGS: -L${SRCDIR}/../../circl_b200 -lcirclb200 -Wl,-rpath,${SRCDIR}/../../circl_b200
+#include <stdlib.h>
 #include "circl_b200.h"
 */
 import "C"
@@ -1172,5 +1173,125 @@ func PBRSAVerify(N []byte, msgs, metadata [][]byte, sigs, status []byte) error {
 	return call(func() C.int {
 		return C.cb200_pbrsa_verify(u8(N), C.size_t(len(N)), u8(blob), (*C.uint64_t)(unsafe.Pointer(&off[0])),
 			u8(mblob), (*C.uint64_t)(unsafe.Pointer(&moff[0])), u8(sigs), u8(status), C.size_t(n))
+	})
+}
+
+// Prio3Config describes one Prio3 instance (draft-irtf-cfrg-vdaf-14, the reference's vdaf/prio3): Kind is the
+// reference's algorithm ID (1 Count, 2 Sum, 3 SumVec, 4 Histogram, 5 MultiHotCountVec); only the parameters of that
+// kind are read.
+type Prio3Config struct {
+	Kind, NumShares                                     uint32
+	MaxMeasurement, Length, Bits, ChunkLength, MaxWeight uint64
+	Context                                             []byte
+}
+
+// Prio3Sizes are the wire sizes of one instance (cb200_prio3_get_sizes).
+type Prio3Sizes struct {
+	InputShareLeader, InputShareHelper, PublicShare, PrepShare, PrepMsg, PrepState, OutShare, AggShare int
+}
+
+// cfgOf returns the C configuration; the context is copied to C memory by the caller's pinning rules (cgo allows Go
+// memory that holds no Go pointers to be passed for the duration of the call).
+func cfgOf(c *Prio3Config) C.cb200_prio3_config {
+	var k C.cb200_prio3_config
+	k.kind, k.num_shares = C.uint32_t(c.Kind), C.uint32_t(c.NumShares)
+	k.max_measurement, k.length, k.bits = C.uint64_t(c.MaxMeasurement), C.uint64_t(c.Length), C.uint64_t(c.Bits)
+	k.chunk_length, k.max_weight = C.uint64_t(c.ChunkLength), C.uint64_t(c.MaxWeight)
+	k.context_len = C.size_t(len(c.Context))
+	return k
+}
+
+func u8opt(b []byte) *C.uint8_t {
+	if len(b) == 0 {
+		return nil
+	}
+	return u8(b)
+}
+
+// prio3Call runs f with the configuration whose context points at a C copy of c.Context.
+func prio3Call(c *Prio3Config, f func(k *C.cb200_prio3_config) C.int) error {
+	k := cfgOf(c)
+	if len(c.Context) > 0 {
+		p := C.CBytes(c.Context)
+		defer C.free(p)
+		k.context = (*C.uint8_t)(p)
+	}
+	return call(func() C.int { return f(&k) })
+}
+
+// Prio3GetSizes validates the configuration as the reference's New does (an error otherwise) and returns its sizes.
+// It needs no device.
+func Prio3GetSizes(c *Prio3Config) (Prio3Sizes, error) {
+	var z C.cb200_prio3_sizes
+	err := prio3Call(c, func(k *C.cb200_prio3_config) C.int { return C.cb200_prio3_get_sizes(k, &z) })
+	return Prio3Sizes{int(z.input_share_leader), int(z.input_share_helper), int(z.public_share), int(z.prep_share),
+		int(z.prep_msg), int(z.prep_state), int(z.out_share), int(z.agg_share)}, err
+}
+
+// Prio3PrepInit: PrepInit (prio3.go:245-324) of len(status) reports under one verify key as aggregator aggID; rows
+// back to back in the reference's encodings.  status: 1 an element >= p, 2 ErrJointRand, 4 ErrInvalidEval; failed
+// rows are zero.  Buffers of the wrong length panic.
+func Prio3PrepInit(c *Prio3Config, z Prio3Sizes, verifyKey []byte, aggID uint8, nonces, publicShares, inputShares,
+	prepStates, prepShares, status []byte) error {
+	n := len(status)
+	in := z.InputShareLeader
+	if aggID != 0 {
+		in = z.InputShareHelper
+	}
+	if len(verifyKey) != 32 || len(nonces) != 16*n || len(publicShares) != z.PublicShare*n ||
+		len(inputShares) != in*n || len(prepStates) != z.PrepState*n || len(prepShares) != z.PrepShare*n {
+		panic("cb200: Prio3PrepInit buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return prio3Call(c, func(k *C.cb200_prio3_config) C.int {
+		return C.cb200_prio3_prep_init(k, u8(verifyKey), C.uint32_t(aggID), u8(nonces), u8opt(publicShares),
+			u8(inputShares), u8(prepStates), u8(prepShares), u8(status), C.size_t(n))
+	})
+}
+
+// Prio3PrepSharesToPrep: PrepSharesToPrep (:332-377); row i of prepShares is the NumShares prep shares of report i.
+// status: 1 an element >= p, 8 ErrProofVerify.
+func Prio3PrepSharesToPrep(c *Prio3Config, z Prio3Sizes, prepShares, prepMsgs, status []byte) error {
+	n := len(status)
+	if len(prepShares) != int(c.NumShares)*z.PrepShare*n || len(prepMsgs) != z.PrepMsg*n {
+		panic("cb200: Prio3PrepSharesToPrep buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return prio3Call(c, func(k *C.cb200_prio3_config) C.int {
+		return C.cb200_prio3_prep_shares_to_prep(k, u8(prepShares), u8opt(prepMsgs), u8(status), C.size_t(n))
+	})
+}
+
+// Prio3PrepNext: PrepNext (:386-403).  status: 2 ErrJointRand.
+func Prio3PrepNext(c *Prio3Config, z Prio3Sizes, prepStates, prepMsgs, outShares, status []byte) error {
+	n := len(status)
+	if len(prepStates) != z.PrepState*n || len(prepMsgs) != z.PrepMsg*n || len(outShares) != z.OutShare*n {
+		panic("cb200: Prio3PrepNext buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return prio3Call(c, func(k *C.cb200_prio3_config) C.int {
+		return C.cb200_prio3_prep_next(k, u8(prepStates), u8opt(prepMsgs), u8(outShares), u8(status), C.size_t(n))
+	})
+}
+
+// Prio3Aggregate: AggregateInit + AggregateUpdate (:408-420) of the out shares whose status byte is 0 (all of them
+// for a nil status) into aggShare.
+func Prio3Aggregate(c *Prio3Config, z Prio3Sizes, outShares, status, aggShare []byte) error {
+	n := len(outShares) / max(z.OutShare, 1)
+	if len(outShares) != z.OutShare*n || (status != nil && len(status) != n) || len(aggShare) != z.AggShare {
+		panic("cb200: Prio3Aggregate buffers have the wrong length")
+	}
+	if n == 0 {
+		clear(aggShare)
+		return nil
+	}
+	return prio3Call(c, func(k *C.cb200_prio3_config) C.int {
+		return C.cb200_prio3_aggregate(k, u8opt(outShares), u8opt(status), u8(aggShare), C.size_t(n))
 	})
 }

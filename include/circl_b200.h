@@ -412,6 +412,68 @@ int cb200_brsa_verify(int variant, const uint8_t *N, size_t N_len, const uint8_t
  * that passes by chance fails every op with status 2. */
 int cb200_pbrsa_check_key(const uint8_t *N, size_t N_len, const uint8_t *p, size_t p_len, const uint8_t *q,
                           size_t q_len);
+
+/* ---- Prio3 aggregators (draft-irtf-cfrg-vdaf-14): the reference's vdaf/prio3 package, aggregator side ----
+ * One instance is a cb200_prio3_config: kind (the reference's algorithm ID, which the XOF header also hashes), the
+ * number of shares (2..255), the circuit's parameters (only those of its kind are read: Sum max_measurement; SumVec
+ * length, bits, chunk_length; Histogram length, chunk_length; MultiHotCountVec length, max_weight, chunk_length) and
+ * the application context (at most 65527 bytes, host memory).  A configuration the reference's New refuses
+ * (ErrNumShares, ErrContextSize, the circuits' parameter errors), an unknown kind, an agg_id >= num_shares (ErrAggID),
+ * a null required pointer, or a circuit whose PrepInit work area exceeds 64 MiB per report (about 2^22 Field128
+ * elements: measurement, proof and a 2^k-point Lagrange domain) is CB200_ERR_ARG before the device is touched.
+ * Every row is the reference's wire encoding (elements little-endian, 8 bytes in Field64 for Count and Sum, 16 in
+ * Field128 for the others; seeds 32 bytes; nonces 16 bytes); cb200_prio3_get_sizes gives the lengths.  Rows are dense, one
+ * per report, and device rows may start at any byte.  Buffers are all host or all device memory.
+ * status (required, one byte per report): 1 = an element that does not decode (a leader input-share element or a
+ * prep-share element >= p, UnmarshalBinary), 2 = ErrJointRand (PrepInit: the report's joint-rand part does not match
+ * the public share; PrepNext: the prep message's seed is not the corrected one), 4 = ErrInvalidEval (t^p = 1), 8 =
+ * ErrProofVerify (Decide rejects).  The outputs of a failed report are all zero; the call itself returns 0. */
+#define CB200_PRIO3_COUNT 1
+#define CB200_PRIO3_SUM 2
+#define CB200_PRIO3_SUMVEC 3
+#define CB200_PRIO3_HISTOGRAM 4
+#define CB200_PRIO3_MULTIHOT 5
+typedef struct {
+  uint32_t kind;
+  uint32_t num_shares;
+  uint64_t max_measurement; /* Sum */
+  uint64_t length;          /* SumVec, Histogram, MultiHotCountVec */
+  uint64_t bits;            /* SumVec */
+  uint64_t chunk_length;    /* SumVec, Histogram, MultiHotCountVec */
+  uint64_t max_weight;      /* MultiHotCountVec */
+  const uint8_t *context;
+  size_t context_len;
+} cb200_prio3_config;
+typedef struct {
+  size_t input_share_leader; /* meas share || proof share (|| blind) */
+  size_t input_share_helper; /* seed (|| blind) */
+  size_t public_share;       /* num_shares joint-rand parts, or 0 */
+  size_t prep_share;         /* verifier share (|| joint-rand part) */
+  size_t prep_msg;           /* joint-rand seed, or 0 */
+  size_t prep_state;         /* out share (|| corrected joint-rand seed); private to this library */
+  size_t out_share;
+  size_t agg_share;
+} cb200_prio3_sizes;
+/* Validates cfg as above and fills *out. */
+int cb200_prio3_get_sizes(const cb200_prio3_config *cfg, cb200_prio3_sizes *out);
+/* PrepInit (prio3.go:245-324) of n reports under one 32-byte verify key as aggregator agg_id (0 = leader): nonces,
+ * public_shares (unused without joint randomness) and input_shares (leader or helper rows by agg_id) -> prep_states
+ * and prep_shares. */
+int cb200_prio3_prep_init(const cb200_prio3_config *cfg, const uint8_t *verify_key, uint32_t agg_id,
+                          const uint8_t *nonces, const uint8_t *public_shares, const uint8_t *input_shares,
+                          uint8_t *prep_states, uint8_t *prep_shares, uint8_t *status, size_t n);
+/* PrepSharesToPrep (:332-377): row i of prep_shares is the num_shares prep shares of report i, in aggregator order
+ * -> prep_msgs (unused without joint randomness). */
+int cb200_prio3_prep_shares_to_prep(const cb200_prio3_config *cfg, const uint8_t *prep_shares, uint8_t *prep_msgs,
+                                    uint8_t *status, size_t n);
+/* PrepNext (:386-403): prep_states and prep_msgs -> out_shares. */
+int cb200_prio3_prep_next(const cb200_prio3_config *cfg, const uint8_t *prep_states, const uint8_t *prep_msgs,
+                          uint8_t *out_shares, uint8_t *status, size_t n);
+/* AggregateInit + AggregateUpdate (:408-420): agg_share = the sum mod p of the out shares of the reports whose status
+ * byte is 0 (all of them when status is null).  n = 0 gives the zero agg share.  A host batch split across GPUs adds
+ * the per-GPU sums on the host. */
+int cb200_prio3_aggregate(const cb200_prio3_config *cfg, const uint8_t *out_shares, const uint8_t *status,
+                          uint8_t *agg_share, size_t n);
 /* Signer.BlindSign (pbrsa.go:350-375): blinded (n rows of kLen) -> sig = c^d' mod N under the key of metadata i.
  * status: 1 = c > N (ErrInvalidMessageLength), 2 = s^e' mod N != c (DecryptAndCheck's "rsa: internal error", also the
  * result of c = N or a wrong qinv). */

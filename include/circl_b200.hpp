@@ -1197,4 +1197,186 @@ class Verifier {
 inline Signer NewSigner(const PrivateKey& sk) { return Signer(sk); }
 inline Verifier NewVerifier(const PublicKey& pk) { return Verifier(pk); }
 }  // namespace partiallyblindrsa
+// Prio3 aggregators (draft-irtf-cfrg-vdaf-14): the reference's vdaf/prio3 packages count, sum, sumvec, histogram and
+// mhcv, aggregator side, on host buffers.  The constructors validate as the reference's New does and throw
+// std::invalid_argument with the library's message.  Rows are the reference's wire encodings, one per report, back to
+// back.  The batch calls return the per-report status bytes (1 an element >= p, 2 ErrJointRand, 4 ErrInvalidEval, 8
+// ErrProofVerify; failed rows are zero); the per-report calls throw the error of the status instead.
+namespace prio3 {
+struct Prio3Error : Error {
+  uint8_t status;
+  Prio3Error(const std::string& m, uint8_t st) : Error(m), status(st) {}
+};
+#define CIRCL_PRIO3_ERR(name)                                        \
+  struct name : Prio3Error {                                         \
+    explicit name(uint8_t st) : Prio3Error("prio3: " #name, st) {} \
+  };
+CIRCL_PRIO3_ERR(ErrDecode)
+CIRCL_PRIO3_ERR(ErrJointRand)
+CIRCL_PRIO3_ERR(ErrInvalidEval)
+CIRCL_PRIO3_ERR(ErrProofVerify)
+#undef CIRCL_PRIO3_ERR
+
+class Prio3 {
+ public:
+  const cb200_prio3_sizes& Params() const { return z_; }
+  unsigned Shares() const { return cfg_.num_shares; }
+  // n reports as aggregator aggID -> prep states and prep shares (n rows each)
+  std::vector<uint8_t> PrepInitBatch(const Bytes& verifyKey, uint8_t aggID, const Bytes& nonces,
+                                     const Bytes& publicShares, const Bytes& inputShares, Bytes* states,
+                                     Bytes* shares) const {
+    const size_t n = nonces.size() / 16;
+    const size_t in = aggID ? z_.input_share_helper : z_.input_share_leader;
+    if (verifyKey.size() != 32 || nonces.size() != 16 * n || inputShares.size() != in * n ||
+        publicShares.size() != z_.public_share * n)
+      throw std::invalid_argument("prio3: row sizes do not match the configuration");
+    states->assign(n * z_.prep_state, 0);
+    shares->assign(n * z_.prep_share, 0);
+    std::vector<uint8_t> st(n);
+    check(cb200_prio3_prep_init(&cfg_, verifyKey.data(), aggID, nonces.data(), ptr(publicShares), inputShares.data(),
+                                states->data(), shares->data(), st.data(), n));
+    return st;
+  }
+  // row i of prepShares: the Shares() prep shares of report i -> prep messages
+  std::vector<uint8_t> PrepSharesToPrepBatch(const Bytes& prepShares, Bytes* msgs) const {
+    const size_t row = cfg_.num_shares * z_.prep_share, n = prepShares.size() / row;
+    if (prepShares.size() != n * row) throw std::invalid_argument("prio3: row sizes do not match the configuration");
+    msgs->assign(n * z_.prep_msg, 0);
+    std::vector<uint8_t> st(n);
+    check(cb200_prio3_prep_shares_to_prep(&cfg_, prepShares.data(), ptr(*msgs), st.data(), n));
+    return st;
+  }
+  std::vector<uint8_t> PrepNextBatch(const Bytes& states, const Bytes& msgs, Bytes* outShares) const {
+    const size_t n = states.size() / z_.prep_state;
+    if (states.size() != n * z_.prep_state || msgs.size() != n * z_.prep_msg)
+      throw std::invalid_argument("prio3: row sizes do not match the configuration");
+    outShares->assign(n * z_.out_share, 0);
+    std::vector<uint8_t> st(n);
+    check(cb200_prio3_prep_next(&cfg_, states.data(), ptr(msgs), outShares->data(), st.data(), n));
+    return st;
+  }
+  // the agg share of the out shares whose status byte is 0 (all of them for an empty status)
+  Bytes AggregateBatch(const Bytes& outShares, const std::vector<uint8_t>& status = {}) const {
+    const size_t n = outShares.size() / z_.out_share;
+    if (outShares.size() != n * z_.out_share || (!status.empty() && status.size() != n))
+      throw std::invalid_argument("prio3: row sizes do not match the configuration");
+    Bytes agg(z_.agg_share);
+    check(cb200_prio3_aggregate(&cfg_, outShares.data(), status.empty() ? nullptr : status.data(), agg.data(), n));
+    return agg;
+  }
+  // one report (prio3.go:245-403)
+  void PrepInit(const Bytes& verifyKey, const Bytes& nonce, uint8_t aggID, const Bytes& publicShare,
+                const Bytes& inputShare, Bytes* state, Bytes* share) const {
+    throw_status(PrepInitBatch(verifyKey, aggID, nonce, publicShare, inputShare, state, share)[0]);
+  }
+  Bytes PrepSharesToPrep(const std::vector<Bytes>& prepShares) const {
+    if (prepShares.size() != cfg_.num_shares) throw std::invalid_argument("prio3: invalid prep shares length");
+    Bytes rows, msg;
+    for (const Bytes& b : prepShares) rows.insert(rows.end(), b.begin(), b.end());
+    throw_status(PrepSharesToPrepBatch(rows, &msg)[0]);
+    return msg;
+  }
+  Bytes PrepNext(const Bytes& state, const Bytes& msg) const {
+    Bytes out;
+    throw_status(PrepNextBatch(state, msg, &out)[0]);
+    return out;
+  }
+  Bytes AggregateInit() const { return Bytes(z_.agg_share); }
+  void AggregateUpdate(Bytes* aggShare, const Bytes& outShare) const {
+    *aggShare = AggregateBatch(merge_rows({*aggShare, outShare}));
+  }
+  // the sum of the agg shares, as integers (Decode of every circuit: one element for Count and Sum)
+  std::vector<uint64_t> Unshard(const std::vector<Bytes>& aggShares, uint64_t numMeas) const {
+    if (aggShares.size() != cfg_.num_shares) throw std::invalid_argument("prio3: invalid aggregate shares length");
+    if (cfg_.kind == CB200_PRIO3_SUM) {
+      const unsigned __int128 bound = (unsigned __int128)numMeas * cfg_.max_measurement;
+      if (bound >= 0xffffffff00000001ull) throw std::invalid_argument("prio3: sum aggregate bound is not representable");
+    }
+    const Bytes s = AggregateBatch(merge_rows(aggShares));
+    const size_t B = cfg_.kind <= CB200_PRIO3_SUM ? 8 : 16;
+    std::vector<uint64_t> out(s.size() / B);
+    for (size_t i = 0; i < out.size(); i++) {  // GetUint64: a Field128 element must fit in 64 bits
+      uint64_t v = 0, hi = 0;
+      for (int j = 0; j < 8; j++) v |= (uint64_t)s[B * i + j] << (8 * j);
+      for (size_t j = 8; j < B; j++) hi |= s[B * i + j];
+      if (hi) throw std::range_error("prio3: number of bits is not enough to represent the number");
+      out[i] = v;
+    }
+    return out;
+  }
+
+ protected:
+  Prio3(uint32_t kind, uint8_t shares, const Bytes& context) : ctx_(context) {
+    cfg_ = cb200_prio3_config{};
+    cfg_.kind = kind;
+    cfg_.num_shares = shares;
+  }
+  void finish() {
+    cfg_.context = ctx_.empty() ? nullptr : ctx_.data();
+    cfg_.context_len = ctx_.size();
+    if (cb200_prio3_get_sizes(&cfg_, &z_) != 0) throw std::invalid_argument(cb200_last_error());
+  }
+  cb200_prio3_config cfg_;
+
+ private:
+  static const uint8_t* ptr(const Bytes& b) { return b.empty() ? nullptr : b.data(); }
+  static uint8_t* ptr(Bytes& b) { return b.empty() ? nullptr : b.data(); }
+  static void check(int rc) {
+    if (rc == CB200_ERR_ARG) throw std::invalid_argument(cb200_last_error());
+    if (rc != 0) throw Error(cb200_last_error());
+  }
+  static void throw_status(uint8_t st) {
+    if (st & 1) throw ErrDecode(st);
+    if (st & 2) throw ErrJointRand(st);
+    if (st & 4) throw ErrInvalidEval(st);
+    if (st & 8) throw ErrProofVerify(st);
+  }
+  Bytes merge_rows(const std::vector<Bytes>& rows) const {
+    Bytes all;
+    for (const Bytes& b : rows) {
+      if (b.size() != z_.agg_share) throw std::invalid_argument("prio3: agg share size");
+      all.insert(all.end(), b.begin(), b.end());
+    }
+    return all;
+  }
+  Bytes ctx_;
+  cb200_prio3_sizes z_{};
+};
+
+struct Count : Prio3 {
+  Count(uint8_t numShares, const Bytes& context) : Prio3(CB200_PRIO3_COUNT, numShares, context) { finish(); }
+};
+struct Sum : Prio3 {
+  Sum(uint8_t numShares, uint64_t maxMeasurement, const Bytes& context) : Prio3(CB200_PRIO3_SUM, numShares, context) {
+    cfg_.max_measurement = maxMeasurement;
+    finish();
+  }
+};
+struct SumVec : Prio3 {
+  SumVec(uint8_t numShares, uint64_t length, uint64_t bits, uint64_t chunkLength, const Bytes& context)
+      : Prio3(CB200_PRIO3_SUMVEC, numShares, context) {
+    cfg_.length = length;
+    cfg_.bits = bits;
+    cfg_.chunk_length = chunkLength;
+    finish();
+  }
+};
+struct Histogram : Prio3 {
+  Histogram(uint8_t numShares, uint64_t length, uint64_t chunkLength, const Bytes& context)
+      : Prio3(CB200_PRIO3_HISTOGRAM, numShares, context) {
+    cfg_.length = length;
+    cfg_.chunk_length = chunkLength;
+    finish();
+  }
+};
+struct MultiHotCountVec : Prio3 {
+  MultiHotCountVec(uint8_t numShares, uint64_t length, uint64_t maxWeight, uint64_t chunkLength, const Bytes& context)
+      : Prio3(CB200_PRIO3_MULTIHOT, numShares, context) {
+    cfg_.length = length;
+    cfg_.max_weight = maxWeight;
+    cfg_.chunk_length = chunkLength;
+    finish();
+  }
+};
+}  // namespace prio3
 }  // namespace circl
