@@ -237,17 +237,20 @@ def info_scalar(s, info: bytes) -> int:
     return hash_to_scalar(s, PARTIAL, b"Info" + i2osp(len(info), 2) + info)
 
 
+def _weights(s, mode, Y, bencs, cencs):
+    """The composite weights d_j of ComputeComposites for the compressed B_j and C_j."""
+    bm = compress(s, Y)
+    sdst = b"Seed-" + context(s, mode)
+    seed = s.hash(i2osp(len(bm), 2) + bm + i2osp(len(sdst), 2) + sdst).digest()
+    return [hash_to_scalar(s, mode, i2osp(len(seed), 2) + seed + i2osp(j, 2) + i2osp(len(bj), 2) + bj
+                           + i2osp(len(cj), 2) + cj + b"Composite") for j, (bj, cj) in enumerate(zip(bencs, cencs))]
+
+
 def _composites(s, mode, k, Y, Bs, Cs):
     """(M, Z) of ComputeComposites; with k, Z = [k] M (the prover's shortcut), else Z = sum d_j C_j."""
-    ctx = context(s, mode)
-    bm = compress(s, Y)
-    sdst = b"Seed-" + ctx
-    seed = s.hash(i2osp(len(bm), 2) + bm + i2osp(len(sdst), 2) + sdst).digest()
+    ds = _weights(s, mode, Y, [compress(s, b) for b in Bs], [compress(s, c) for c in Cs])
     M = Z = None
-    for j, (b, c) in enumerate(zip(Bs, Cs)):
-        bj, cj = compress(s, b), compress(s, c)
-        d = hash_to_scalar(s, mode, i2osp(len(seed), 2) + seed + i2osp(j, 2) + i2osp(len(bj), 2) + bj
-                           + i2osp(len(cj), 2) + cj + b"Composite")
+    for d, b, c in zip(ds, Bs, Cs):
         M = add(s, M, mul(s, d, b))
         if k is None:
             Z = add(s, Z, mul(s, d, c))
@@ -316,6 +319,38 @@ def evaluate(s, mode, sk: bytes, blinded, r: bytes = None, info: bytes = b""):
     if mode == VERIFIABLE:
         return ev, prove(s, mode, kp, mul(s, kp, s.g), Bs, Ds, rv)
     return ev, prove(s, mode, kp, mul(s, kp, s.g), Ds, Bs, rv)
+
+
+def evaluate_grouped(s, mode, sk: bytes, blinded, r: bytes = None, info: bytes = b""):
+    """evaluate() for requests whose m elements come from a few distinct ones: one [ke] B per distinct B, and
+    M = sum over distinct b of (sum of the d_j with B_j = b mod n) b, so the weights are still hashed per element but
+    there are only as many scalar multiplications as distinct elements.  The same results and errors as evaluate()."""
+    k = int.from_bytes(sk, "big")
+    pts = {b: decompress(s, b) for b in dict.fromkeys(bytes(b) for b in blinded)}
+    st = (1 if any(p is None for p in pts.values()) else 0) | (0 if 0 < k < s.n else 2)
+    rv = int.from_bytes(r, "big") if r is not None else 1
+    if mode != BASE and not 0 < rv < s.n:
+        st |= 4
+    if st:
+        raise OprfError(st)
+    kp, ke = _secret(s, mode, k, info)
+    D = {b: mul(s, ke, p) for b, p in pts.items()}
+    enc = {b: compress(s, d) for b, d in D.items()}
+    ev = [enc[bytes(b)] for b in blinded]
+    if mode == BASE:
+        return ev, None
+    Y = mul(s, kp, s.g)
+    # mode 1 proves D = [k]B; mode 2 proves B = [t]D, with the roles of B and D swapped
+    benc = [bytes(b) for b in blinded]
+    ds = _weights(s, mode, Y, benc, ev) if mode == VERIFIABLE else _weights(s, mode, Y, ev, benc)
+    w = dict.fromkeys(pts, 0)
+    for b, d in zip(benc, ds):
+        w[b] = (w[b] + d) % s.n
+    M = None
+    for b, wb in w.items():
+        M = add(s, M, mul(s, wb, pts[b] if mode == VERIFIABLE else D[b]))
+    c = _challenge(s, mode, [Y, M, mul(s, kp, M), mul(s, rv, s.g), mul(s, rv, M)])
+    return ev, i2osp(c, s.Ns) + i2osp((rv - c * kp) % s.n, s.Ns)
 
 
 def finalize_hash(s, mode, inp: bytes, info: bytes, elem: bytes) -> bytes:

@@ -95,3 +95,36 @@ def test_partial_key_with_t_zero_fails(s):
     with pytest.raises(om.OprfError) as e:
         om.full_evaluate(s, om.PARTIAL, sk, b"x", info)
     assert e.value.status == 8
+
+
+@pytest.mark.parametrize("mode", [om.BASE, om.VERIFIABLE, om.PARTIAL])
+@pytest.mark.parametrize("s", list(om.SUITES.values()), ids=list(om.SUITES))
+def test_grouped_evaluate_matches_evaluate(s, mode):
+    """evaluate_grouped, which the large GPU batches are checked with, gives evaluate's elements, proof and errors
+    byte for byte, at m from 1 to 40 with repeated elements (a weight sum that wraps mod n included)."""
+    import random
+    rng = random.Random(9497 + 10 * mode + s.bits)
+    pool = [om.compress(s, om.mul(s, rng.randrange(1, s.n), s.g)) for _ in range(4)]
+    info = b"grouped" if mode == om.PARTIAL else b""
+    for m in (1, 2, 3, 7, 16, 40):
+        sk = om.i2osp(rng.randrange(1, s.n), s.Ns)
+        r = om.i2osp(rng.randrange(1, s.n), s.Ns)
+        bl = [pool[0]] * m if m == 16 else [pool[rng.randrange(len(pool))] for _ in range(m)]
+        assert om.evaluate_grouped(s, mode, sk, bl, r, info) == om.evaluate(s, mode, sk, bl, r, info), m
+    # the same status bits on failing requests
+    x = next(v for v in range(1, 200) if not om._is_square(s, (v ** 3 - 3 * v + s.b) % s.p))
+    bad = [b"\x02" + om.i2osp(x, s.nbytes), b"\x04" + pool[0][1:]]
+    t0 = om.i2osp(s.n - om.info_scalar(s, info), s.Ns) if mode == om.PARTIAL else bytes(s.Ns)
+    one = om.i2osp(1, s.Ns)
+    for sk, bl, r in ((bytes(s.Ns), pool[:2], one), (om.i2osp(s.n, s.Ns), pool[:2], one), (one, pool[:1] + bad, one),
+                      (one, pool[:2], bytes(s.Ns)), (t0, pool[:2], one), (bytes(s.Ns), bad, bytes(s.Ns))):
+        want = got = None
+        try:
+            want = om.evaluate(s, mode, sk, bl, r, info)
+        except om.OprfError as e:
+            want = e.status
+        try:
+            got = om.evaluate_grouped(s, mode, sk, bl, r, info)
+        except om.OprfError as e:
+            got = e.status
+        assert got == want
