@@ -17,6 +17,8 @@
 //   pb_*          partially blind RSA (RSAPBSSA-SHA384, partiallyblindrsa/pbrsa.go): e' from the metadata by
 //                 HKDF-SHA-384, d' by Fermat inversion mod p' = (p - 1) / 2 and q', exp_public_words for the
 //                 multi-word e', on the same two bodies; see that section
+//   tss_*         threshold RSA (tss/rsa): signature shares by exp_windows over a public bound, and the combination of
+//                 k shares with mod_inverse for the public values it inverts; see that section
 //
 // Secret values (p, q, dp, dq, qinv, s_p, s_q) reach no branch and no address: every loop count and index comes from
 // the word counts and the public bit lengths of p and q, the window digit only forms masks, and the final subtraction
@@ -167,11 +169,11 @@ CB200_XHD void add_mod(uint32_t* r, const uint32_t* a, const uint32_t* b, const 
   for (int j = 0; j < W; j++) r[j] = (s[j] & keep) | (d[j] & ~keep);
 }
 
-// r = x^d R mod m from xm = x R mod m, for the secret d of W words of which the low M->bits count (d < m).  Every
-// one of the ceil(bits / 4) windows costs four squarings and one product with a table entry selected by masks.
-// digit(w) reads window w of d.
-template <int W, class Digit>
-CB200_XHD void exp_windows(uint32_t* r, const uint32_t* xm, const Digit& digit_of, const Mod<W>* M) {
+// r = x^d R mod m from xm = x R mod m, for the secret d below 2^bits(), with bits() public: bitlen(m) for an exponent
+// reduced mod m, a public bound otherwise (read once, after the table is built).  Every one of the ceil(bits / 4)
+// windows costs four squarings and one product with a table entry selected by masks.  digit(w) reads window w of d.
+template <int W, class Digit, class Bits>
+CB200_XHD void exp_windows(uint32_t* r, const uint32_t* xm, const Digit& digit_of, const Bits& bits, const Mod<W>* M) {
   uint32_t tbl[16][W], one[W];
   for (int j = 0; j < W; j++) one[j] = j == 0;
   mont_mul<W>(tbl[0], M->r2, one, M);  // R mod m
@@ -179,7 +181,7 @@ CB200_XHD void exp_windows(uint32_t* r, const uint32_t* xm, const Digit& digit_o
 #pragma unroll 1
   for (int k = 2; k < 16; k++) mont_mul<W>(tbl[k], tbl[k - 1], xm, M);
   for (int j = 0; j < W; j++) r[j] = tbl[0][j];
-  const int nwin = (ldk((const uint32_t*)&M->bits) + 3) / 4;
+  const int nwin = (bits() + 3) / 4;
   uint32_t sel[W];
 #pragma unroll 1
   for (int w = nwin - 1; w >= 0; w--) {
@@ -200,12 +202,14 @@ CB200_XHD void exp_windows(uint32_t* r, const uint32_t* xm, const Digit& digit_o
 // d in the key (global memory on the device)
 template <int W>
 CB200_RSA_NOINLINE void exp_secret(uint32_t* r, const uint32_t* xm, const uint32_t* d, const Mod<W>* M) {
-  exp_windows<W>(r, xm, [&](int w) { return (ldk(&d[w >> 3]) >> (4 * (w & 7))) & 15; }, M);
+  exp_windows<W>(r, xm, [&](int w) { return (ldk(&d[w >> 3]) >> (4 * (w & 7))) & 15; },
+                 [&] { return ldk((const uint32_t*)&M->bits); }, M);
 }
 // d in the thread's own memory (an exponent computed per operation)
 template <int W>
 CB200_RSA_NOINLINE void exp_secret_own(uint32_t* r, const uint32_t* xm, const uint32_t* d, const Mod<W>* M) {
-  exp_windows<W>(r, xm, [&](int w) { return (d[w >> 3] >> (4 * (w & 7))) & 15; }, M);
+  exp_windows<W>(r, xm, [&](int w) { return (d[w >> 3] >> (4 * (w & 7))) & 15; },
+                 [&] { return ldk((const uint32_t*)&M->bits); }, M);
 }
 
 // r = x^e R mod m from xm = x R mod m for a public e >= 1
@@ -560,6 +564,267 @@ CB200_XHD uint32_t pb_verify(const uint8_t* msg, int len, const uint8_t* meta, i
       });
 }
 
+// ---------------------------------------------------------------- threshold RSA (tss/rsa, Shoup's protocol 1)
+// The reference's tss/rsa package: a party holding the key share s_i signs x with x^(2 Delta s_i) mod N
+// (KeyShare.Sign, keyshare.go:188-256), and a combiner turns k >= threshold such shares into the RSA signature
+// (CombineSignShares, rsa_threshold.go:207-293), with Delta = players!.  Served: 2 <= players <= kTssMaxPlayers,
+// u16 indices, k <= kTssMaxPlayers shares per op.  Then 2 Delta < 2^297 (kDeltaWords), e' = 4 Delta^2 < 2^594
+// (kEpWords) and |2 lambda| < 2 Delta 65535^63 < 2^1305 (kLambdaWords).
+//   tss_sign_share  x^E mod N for the secret E = 2 Delta s_i (or the share's cached value) by exp_windows over the
+//                   public bound bitlen(N) - 2 + bitlen(2 Delta) on bitlen(E); E reaches no branch and no address
+//   mod_inverse     a^-1 R mod m from a R mod m for a public a and an odd composite m, by binary extended Euclid
+//                   (variable-time: every value Combine inverts is public)
+//   tss_lambda      lambda_j of computeLambda (rsa_threshold.go:315-349) for i = 0
+//   tss_combine     CombineSignShares of one op from the k shares, its index set and x
+constexpr int kTssMaxPlayers = 64;
+constexpr int kDeltaWords = 10;
+constexpr int kEpWords = 19;
+constexpr int kLambdaWords = 41;
+
+template <int WN>
+struct TssSignKey {
+  Mod<WN> n;
+  uint32_t e[WN + kDeltaWords];  // E, little-endian
+  int ebits;                     // the public bound on bitlen(E) the windows run over
+  int klen;
+};
+template <int WN>
+struct TssCombineKey {
+  Mod<WN> n;
+  uint32_t e;                    // the public exponent
+  uint32_t delta[kDeltaWords];   // Delta = players!
+  uint32_t a;                    // |a| and |b| of e' a + e b = gcd(e', e), with their signs and bit lengths
+  uint32_t b[kEpWords];
+  int a_neg, b_neg, a_bits, b_bits;
+  int k;                         // shares per op
+  int klen;
+};
+
+// xi = x^E mod N (kLen bytes) of the kLen-byte x (x < R, so x R mod N = x R^2 R^-1 reduces it, as Exp does)
+template <int WN>
+CB200_XHD void tss_sign_share(uint8_t* out, const uint8_t* in, const TssSignKey<WN>& K) {
+  const int klen = K.klen;
+  uint32_t x[WN], r[WN];
+  from_be<WN>(x, in, klen);
+  mont_mul<WN>(x, x, K.n.r2, &K.n);
+  exp_windows<WN>(r, x, [&](int w) { return (ldk(&K.e[w >> 3]) >> (4 * (w & 7))) & 15; },
+                  [&] { return ldk((const uint32_t*)&K.ebits); }, &K.n);
+  for (int j = 0; j < WN; j++) x[j] = j == 0;
+  mont_mul<WN>(r, r, x, &K.n);
+  for (int i = 0; i < klen; i++) out[i] = be_byte(r, klen, i);
+}
+
+// trailing and leading zero bits of x != 0
+CB200_XHD int ctz32(uint32_t x) {
+#if defined(__CUDA_ARCH__)
+  return __ffs(x) - 1;
+#else
+  return __builtin_ctz(x);
+#endif
+}
+CB200_XHD int clz32(uint32_t x) {
+#if defined(__CUDA_ARCH__)
+  return __clz(x);
+#else
+  return __builtin_clz(x);
+#endif
+}
+
+// r = a^-1 R mod m from a = a' R mod m (a < m), for the odd m: true, or false if gcd(a, m) != 1 (a = 0 included).
+// Binary extended Euclid on (u, v) = (a, m) with x1 a = u, x2 a = v mod m: strip u's (v's) trailing zeros, up to 32 a
+// step, dividing x1 (x2) by 2^s mod m as Montgomery's reduction does (add k m with k = x1 (-m^-1) mod 2^s), then
+// subtract the smaller of u, v from the larger.  Ends at u = 1 or v = 1 with x = (a' R)^-1, and x R^3 R^-1 = a'^-1 R.
+// Every value it sees is public, so it branches freely.
+template <int W>
+CB200_RSA_NOINLINE bool mod_inverse(uint32_t* r, const uint32_t* a, const Mod<W>* M) {
+  uint32_t u[W], v[W], x1[W], x2[W];
+  for (int j = 0; j < W; j++) u[j] = a[j], v[j] = ldk(&M->m[j]), x1[j] = j == 0, x2[j] = 0;
+  const uint32_t n0 = ldk(&M->n0);
+  auto is_small = [](const uint32_t* x, uint32_t c) {
+    if (x[0] != c) return false;
+    for (int j = 1; j < W; j++)
+      if (x[j]) return false;
+    return true;
+  };
+  auto strip = [&](uint32_t* x, uint32_t* c) {  // x even and not zero: x >>= s, c = c 2^-s mod m
+    while (!(x[0] & 1)) {
+      const int s = x[0] ? ctz32(x[0]) : 32;
+      for (int j = 0; j < W; j++)
+        x[j] = (uint32_t)(((uint64_t)(j + 1 < W ? x[j + 1] : 0) << 32 | x[j]) >> s);
+      const uint32_t k = (c[0] * n0) & (s == 32 ? ~0u : (1u << s) - 1);
+      uint64_t cy = 0;
+      uint32_t lo = 0;
+      for (int j = 0; j < W; j++) {  // (c + k m) >> s < m
+        cy += (uint64_t)k * ldk(&M->m[j]) + c[j];
+        const uint32_t t = (uint32_t)cy;
+        cy >>= 32;
+        if (j) c[j - 1] = (uint32_t)(((uint64_t)t << 32 | lo) >> s);
+        lo = t;
+      }
+      c[W - 1] = (uint32_t)((cy << 32 | lo) >> s);
+    }
+  };
+  auto sub = [](uint32_t* x, const uint32_t* y) {
+    uint32_t br = 0;
+    for (int j = 0; j < W; j++) {
+      const uint64_t d = (uint64_t)x[j] - y[j] - br;
+      x[j] = (uint32_t)d;
+      br = (uint32_t)(d >> 63);
+    }
+  };
+  if (is_small(u, 0)) return false;
+  while (!is_small(u, 1) && !is_small(v, 1)) {
+    if (is_small(u, 0) || is_small(v, 0)) return false;  // the gcd is the other one, above 1
+    strip(u, x1);
+    strip(v, x2);
+    if (cmp<W>(u, v) >= 0) {
+      sub(u, v);
+      sub_mod<W>(x1, x1, x2, M);
+    } else {
+      sub(v, u);
+      sub_mod<W>(x2, x2, x1, M);
+    }
+  }
+  mont_mul<W>(r, is_small(u, 1) ? x1 : x2, M->r3, M);
+  return true;
+}
+
+// |lambda_j| (kLambdaWords words, returned in lam) and its sign for j = idx(t) over the index set idx(0 .. k) with
+// i = 0: lambda = Delta prod_{j' != j} (0 - j') / prod_{j' != j} (j - j'), as computeLambda.  Returns 1 (ErrInvalidCalc)
+// if an index is 0 (checkIndices: i = 0 must not be in S) or the quotient is not an integer, else 0.  Delta prod j' is
+// formed first, then divided by each |j - j'| in turn: the divisions are all exact iff the product of the divisors
+// divides it.  A repeated index is skipped like j itself, as the reference does, so the denominator is never zero.
+template <class Idx>
+CB200_XHD uint32_t tss_lambda(uint32_t* lam, bool* neg, const Idx& idx, int t, int k, const uint32_t* delta) {
+  const uint32_t j = idx(t);
+  for (int i = 0; i < kLambdaWords; i++) lam[i] = i < kDeltaWords ? ldk(&delta[i]) : 0;
+  bool s = false;
+  for (int u = 0; u < k; u++) {
+    const uint32_t jp = idx(u);
+    if (jp == 0) return 1;
+    if (jp == j) continue;
+    s = s != (jp < j);  // (0 - j') / (j - j') < 0 iff j' < j: the sign flips exactly then
+    uint64_t c = 0;
+    for (int i = 0; i < kLambdaWords; i++) {
+      c += (uint64_t)lam[i] * jp;
+      lam[i] = (uint32_t)c;
+      c >>= 32;
+    }
+  }
+  for (int u = 0; u < k; u++) {
+    const uint32_t jp = idx(u);
+    if (jp == j) continue;
+    const uint32_t d = jp > j ? jp - j : j - jp;
+    uint64_t rem = 0;
+    for (int i = kLambdaWords - 1; i >= 0; i--) {
+      const uint64_t cur = rem << 32 | lam[i];
+      lam[i] = (uint32_t)(cur / d);
+      rem = cur % d;
+    }
+    if (rem) return 1;
+  }
+  *neg = s;
+  return 0;
+}
+
+// bit length of a public value of n words
+CB200_XHD int bits_of(const uint32_t* x, int n) {
+  for (int j = n - 1; j >= 0; j--)
+    if (x[j]) return 32 * j + 32 - clz32(x[j]);
+  return 0;
+}
+
+// CombineSignShares (rsa_threshold.go:207-293) of one op: the k shares xi(t) (kLen bytes each) of the indices idx(t)
+// and the kLen-byte x -> y (kLen bytes) and 0, or 1 (ErrInvalidCalc from computeLambda) or 2 ("rsa: internal error":
+// y^e mod N != x, x unreduced), with out all zero.  The parameter checks before the lambdas are the host's.
+//   w = prod_t xi_t^(2 lambda_t) = P / Q with P the product of the terms of positive lambda and Q of the negative ones,
+//   y = w^a x^b mod N.
+// The reference inverts each negative term, then w if a < 0, then x if b < 0.  All of them are invertible iff
+// D = Q (P if a < 0) (x if b < 0) is, and one inverse of D then gives each of them.  Otherwise the reference's
+// sequence runs as it is: a term whose inverse fails stays as it was (ModInverse leaves it unchanged), and a power
+// with a negative exponent of a base without an inverse is 0 (Exp leaves its fresh result at 0).
+template <int WN, class Idx, class Xi>
+CB200_XHD uint32_t tss_combine(uint8_t* out, const Idx& idx, const Xi& xi, const uint8_t* msg,
+                               const TssCombineKey<WN>& K) {
+  const int klen = K.klen, k = ldk((const uint32_t*)&K.k);
+  const Mod<WN>* M = &K.n;
+  uint32_t lam[kLambdaWords];
+  bool neg;
+  for (int i = 0; i < klen; i++) out[i] = 0;
+  for (int t = 0; t < k; t++)
+    if (tss_lambda(lam, &neg, idx, t, k, K.delta)) return 1;
+  uint32_t one[WN], mone[WN], P[WN], Q[WN], x[WN], xm[WN], tm[WN];
+  for (int j = 0; j < WN; j++) one[j] = j == 0;
+  mont_mul<WN>(mone, M->r2, one, M);  // R mod N
+  // tm = xi_t^|2 lambda_t| R mod N
+  auto term = [&](int t) {
+    tss_lambda(lam, &neg, idx, t, k, K.delta);
+    for (int i = kLambdaWords - 1; i > 0; i--) lam[i] = lam[i] << 1 | lam[i - 1] >> 31;
+    lam[0] <<= 1;
+    from_be<WN>(tm, xi(t), klen);
+    mont_mul<WN>(tm, tm, M->r2, M);
+    exp_public_words<WN>(tm, tm, lam, bits_of(lam, kLambdaWords), M);
+  };
+  for (int j = 0; j < WN; j++) P[j] = Q[j] = mone[j];
+  for (int t = 0; t < k; t++) {
+    term(t);
+    mont_mul<WN>(neg ? Q : P, neg ? Q : P, tm, M);
+  }
+  from_be<WN>(x, msg, klen);
+  mont_mul<WN>(xm, x, M->r2, M);
+  const bool a_neg = ldk((const uint32_t*)&K.a_neg), b_neg = ldk((const uint32_t*)&K.b_neg);
+  uint32_t D[WN], ba[WN], bb[WN];  // the bases of |a| and |b|
+  bool za = false, zb = false;     // a base that is 0 (a failed inverse of Exp)
+  for (int j = 0; j < WN; j++) D[j] = Q[j];
+  if (a_neg) mont_mul<WN>(D, D, P, M);
+  if (b_neg) mont_mul<WN>(D, D, xm, M);
+  if (mod_inverse<WN>(D, D, M)) {
+    // D^-1 Q = (P if a < 0)^-1 (x if b < 0)^-1, D^-1 (D / Q) = Q^-1
+    mont_mul<WN>(tm, D, Q, M);
+    if (b_neg) mont_mul<WN>(bb, tm, a_neg ? P : mone, M);  // x^-1
+    else for (int j = 0; j < WN; j++) bb[j] = xm[j];
+    if (a_neg) {  // w^-1 = Q P^-1 = Q (D^-1 Q (x if b < 0))
+      mont_mul<WN>(ba, tm, b_neg ? xm : mone, M);
+      mont_mul<WN>(ba, ba, Q, M);
+    } else {  // w = P Q^-1 = P D^-1 (x if b < 0)
+      mont_mul<WN>(ba, D, b_neg ? xm : mone, M);
+      mont_mul<WN>(ba, ba, P, M);
+    }
+  } else {
+    for (int j = 0; j < WN; j++) ba[j] = mone[j];
+    for (int t = 0; t < k; t++) {
+      term(t);
+      if (neg) mod_inverse<WN>(tm, tm, M);  // unchanged when there is no inverse
+      mont_mul<WN>(ba, ba, tm, M);
+    }
+    if (a_neg) za = !mod_inverse<WN>(ba, ba, M);
+    for (int j = 0; j < WN; j++) bb[j] = xm[j];
+    if (b_neg) zb = !mod_inverse<WN>(bb, bb, M);
+  }
+  // w^a and x^b: Exp by 0 is 1
+  uint32_t ea[1] = {ldk(&K.a)};
+  const int abits = ldk((const uint32_t*)&K.a_bits), bbits = ldk((const uint32_t*)&K.b_bits);
+  if (abits) exp_public_words<WN>(ba, ba, ea, abits, M);
+  else for (int j = 0; j < WN; j++) ba[j] = mone[j];
+  if (bbits) {
+    uint32_t eb[kEpWords];
+    for (int j = 0; j < kEpWords; j++) eb[j] = ldk(&K.b[j]);
+    exp_public_words<WN>(bb, bb, eb, bbits, M);
+  } else {
+    for (int j = 0; j < WN; j++) bb[j] = mone[j];
+  }
+  uint32_t y[WN];
+  mont_mul<WN>(y, ba, bb, M);
+  if (za || zb)
+    for (int j = 0; j < WN; j++) y[j] = 0;
+  exp_public<WN>(tm, y, ldk(&K.e), M);  // y^e R
+  mont_mul<WN>(tm, tm, one, M);
+  mont_mul<WN>(y, y, one, M);
+  if (cmp<WN>(tm, x)) return 2;
+  for (int i = 0; i < klen; i++) out[i] = be_byte(y, klen, i);
+  return 0;
+}
+
 // ---------------------------------------------------------------- host preparation
 // M from the odd modulus m > 1 of W words: n0 by Newton's iteration, R^2 mod m from R mod m (32 W modular doublings of
 // 1) by t more doublings and s Montgomery squarings with t 2^s = 32 W (each squaring doubles the exponent of 2 over R),
@@ -636,6 +901,61 @@ inline bool probably_prime(const uint32_t* n, int rounds, Rnd& rnd) {
     if (witness) return false;
   }
   return true;
+}
+
+// (a, b) with e' a + e b = gcd(e', e) for e' = ep (kEpWords words) and e < 2^32: the classical extended Euclid
+// coefficients, as Go's GCD gives them.  Its first step is e' = q e + r; the rest runs on (e, r) in 64-bit integers,
+// giving s e + t r = g, so a = t and b = s - t q.  |a| < 2^32 and |b| <= e' fit their fields.
+inline void tss_bezout(uint32_t* a, int* a_neg, uint32_t* b, int* b_neg, const uint32_t* ep, uint32_t e) {
+  uint32_t q[kEpWords];
+  uint64_t rem = 0;
+  for (int i = kEpWords - 1; i >= 0; i--) {
+    const uint64_t cur = rem << 32 | ep[i];
+    q[i] = (uint32_t)(cur / e);
+    rem = cur % e;
+  }
+  int64_t r0 = e, r1 = (int64_t)rem, s0 = 1, s1 = 0, t0 = 0, t1 = 1;
+  while (r1) {
+    const int64_t qq = r0 / r1, r2 = r0 - qq * r1, s2 = s0 - qq * s1, t2 = t0 - qq * t1;
+    r0 = r1, r1 = r2, s0 = s1, s1 = s2, t0 = t1, t1 = t2;
+  }
+  *a_neg = t0 < 0;
+  *a = (uint32_t)(t0 < 0 ? -t0 : t0);
+  // b = s - t q from |t| q and |s| (both below 2^32 in magnitude for t and s)
+  const uint64_t at = (uint64_t)(t0 < 0 ? -t0 : t0), as = (uint64_t)(s0 < 0 ? -s0 : s0);
+  uint32_t tq[kEpWords];
+  uint64_t c = 0;
+  for (int i = 0; i < kEpWords; i++) {
+    c += (uint64_t)q[i] * at;
+    tq[i] = (uint32_t)c;
+    c >>= 32;
+  }
+  // -t q and s: the same sign (add magnitudes) or opposite (subtract the smaller)
+  const bool tq_neg = t0 > 0, s_neg = s0 < 0;
+  uint32_t sw[kEpWords] = {(uint32_t)as, (uint32_t)(as >> 32)};
+  if (tq_neg == s_neg || !at) {
+    uint64_t cy = 0;
+    for (int i = 0; i < kEpWords; i++) {
+      cy += (uint64_t)tq[i] + sw[i];
+      b[i] = (uint32_t)cy;
+      cy >>= 32;
+    }
+    *b_neg = at ? tq_neg : s_neg;
+  } else {
+    const bool big = cmp<kEpWords>(tq, sw) >= 0;
+    const uint32_t* hi = big ? tq : sw;
+    const uint32_t* lo = big ? sw : tq;
+    uint32_t br = 0;
+    for (int i = 0; i < kEpWords; i++) {
+      const uint64_t d = (uint64_t)hi[i] - lo[i] - br;
+      b[i] = (uint32_t)d;
+      br = (uint32_t)(d >> 63);
+    }
+    *b_neg = big ? tq_neg : s_neg;
+  }
+  bool zero = true;
+  for (int i = 0; i < kEpWords; i++) zero = zero && !b[i];
+  if (zero) *b_neg = 0;
 }
 
 }  // namespace rsa

@@ -1295,3 +1295,46 @@ func Prio3Aggregate(c *Prio3Config, z Prio3Sizes, outShares, status, aggShare []
 		return C.cb200_prio3_aggregate(k, u8opt(outShares), u8opt(status), u8(aggShare), C.size_t(n))
 	})
 }
+
+// ---- Threshold RSA (the reference's tss/rsa, Shoup's protocol 1).  N and e are big-endian byte strings; rows are
+// kLen = BRSAModulusBytes(N) bytes back to back.  Served: 2 <= players <= 64, threshold <= k <= 64, u16 indices.
+
+// TSSRSASignShare: KeyShare.Sign (keyshare.go:188-256) of n digests (n rows of kLen) with the exponent E = 2 Delta s_i
+// (or the share's cached twoDeltaSi); xi receives the n shares.
+func TSSRSASignShare(N []byte, players int, E, digests, xi []byte) error {
+	k := BRSAModulusBytes(N)
+	n := 0
+	if k != 0 {
+		n = len(digests) / k
+	}
+	if k == 0 || len(E) == 0 || len(digests) != n*k || len(xi) != n*k {
+		panic("cb200: TSSRSASignShare buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return call(func() C.int {
+		return C.cb200_tssrsa_sign_share(u8(N), C.size_t(len(N)), C.int(players), u8(E), C.size_t(len(E)),
+			u8(digests), u8(xi), C.size_t(n))
+	})
+}
+
+// TSSRSACombine: CombineSignShares (rsa_threshold.go:207-293) of n ops after the share parameter checks: op i combines
+// the k shares xi row i (k kLen bytes) of the indices idx[i*k:(i+1)*k] for the padded message msgs row i; sig receives
+// n rows, status n bytes (0, 1 = ErrInvalidCalc, 2 = "rsa: internal error"; failed rows zero).
+func TSSRSACombine(N, e []byte, players, threshold, k int, idx []uint16, xi, msgs, sig, status []byte) error {
+	kl := BRSAModulusBytes(N)
+	n := len(status)
+	if kl == 0 || len(e) == 0 || k < 1 || len(idx) != n*k || len(xi) != n*k*kl || len(msgs) != n*kl ||
+		len(sig) != n*kl {
+		panic("cb200: TSSRSACombine buffers have the wrong length")
+	}
+	if n == 0 {
+		return nil
+	}
+	return call(func() C.int {
+		return C.cb200_tssrsa_combine(u8(N), C.size_t(len(N)), u8(e), C.size_t(len(e)), C.int(players),
+			C.int(threshold), C.int(k), (*C.uint16_t)(unsafe.Pointer(&idx[0])), u8(xi), u8(msgs), u8(sig), u8(status),
+			C.size_t(n))
+	})
+}

@@ -486,6 +486,28 @@ int cb200_pbrsa_blind_sign(const uint8_t *N, size_t N_len, const uint8_t *p, siz
 int cb200_pbrsa_verify(const uint8_t *N, size_t N_len, const uint8_t *msgs, const uint64_t *msg_off,
                        const uint8_t *meta, const uint64_t *meta_off, const uint8_t *sigs, uint8_t *status, size_t n);
 
+/* ---- Threshold RSA signatures (the reference's tss/rsa package, Shoup's protocol 1) ----
+ * A dealer splits an RSA key into players key shares s_i, of which any threshold sign: each party computes its share
+ * xi = x^(2 Delta s_i) mod N of the padded digest x (Delta = players!), and a combiner turns k >= threshold shares into
+ * the standard RSA signature y with y^e = x mod N.  N (2048 to 4096 bits) and e are big-endian byte strings in host
+ * memory, one key per call.  Served: 2 <= players <= 64 (the reference has no bound), u16 indices, k <= 64.  Rows are
+ * kLen = ceil(bitlen(N) / 8) bytes (cb200_brsa_modulus_bytes) and on device buffers may start at any byte.  An argument
+ * outside these rules or a null pointer is CB200_ERR_ARG with a message, before the device is touched. */
+/* KeyShare.Sign (keyshare.go:188-256): digests (n rows of kLen, x < 2^(8 kLen), reduced mod N as Exp does) -> xi = x^E
+ * mod N (n rows of kLen) for E = 2 Delta s_i (or the share's cached twoDeltaSi), a secret of at most
+ * bitlen(N) - 2 + bitlen(2 Delta) bits: the constant-time exponentiation runs over that bound, in place of the
+ * reference's optional blinding.  No per-op failure, so no status. */
+int cb200_tssrsa_sign_share(const uint8_t *N, size_t N_len, int players, const uint8_t *E, size_t E_len,
+                            const uint8_t *digests, uint8_t *xi, size_t n);
+/* CombineSignShares (rsa_threshold.go:207-293) with the share parameters already checked: op i combines the k shares
+ * xi[i] (k rows of kLen) of the indices idx[i] (k uint16 values in host byte order; a device idx must be 2-byte
+ * aligned) for msgs row i -> sig row i.  e odd, 3 <= e < 2^32; 1 <= threshold <= players; threshold <= k <= 64.
+ * status: 0, 1 = ErrInvalidCalc (an index 0, or a lambda that is not an integer), 2 = "rsa: internal error" (y^e mod N
+ * != x, x taken unreduced, so x >= N always fails).  A failed op's row is all zero; the call itself returns 0. */
+int cb200_tssrsa_combine(const uint8_t *N, size_t N_len, const uint8_t *e, size_t e_len, int players, int threshold,
+                         int k, const uint16_t *idx, const uint8_t *xi, const uint8_t *msgs, uint8_t *sig,
+                         uint8_t *status, size_t n);
+
 /* ---- P-384 and P-521 ECDH (crypto/ecdh.P384() / P521()) ----
  * cb200_p384 / cb200_p521: the contract of cb200_p256 with 48-byte scalars and Shared outputs and 97-byte points and
  * KeyGen outputs (P-384), or 66 and 133 bytes (P-521).  A 66-byte P-521 scalar whose leading byte is above 0x01 is

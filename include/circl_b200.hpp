@@ -1197,6 +1197,78 @@ class Verifier {
 inline Signer NewSigner(const PrivateKey& sk) { return Signer(sk); }
 inline Verifier NewVerifier(const PublicKey& pk) { return Verifier(pk); }
 }  // namespace partiallyblindrsa
+
+// Threshold RSA (the reference's tss/rsa, Shoup's protocol 1): a party's signature shares x^E mod N under its key
+// share, E = 2 Delta s_i (or the share's cached twoDeltaSi, as KeyShare.Sign uses it), and the combination of k shares
+// per op into the RSA signature (CombineSignShares after its share parameter checks).  Byte strings are big-endian;
+// rows are kLen = ceil(bitlen(N) / 8) bytes back to back.  Served: N of 2048 to 4096 bits, an odd e with
+// 3 <= e < 2^32, 2 <= players <= 64, threshold <= k <= 64 shares per op, u16 indices, E of at most
+// bitlen(N) - 2 + bitlen(2 players!) bits.  Arguments outside these throw std::logic_error with the library's message.
+namespace tssrsa {
+struct TSSRSAError : Error {
+  std::vector<uint8_t> status;  // per-op bytes of a failed batch
+  explicit TSSRSAError(const std::string& m, std::vector<uint8_t> st = {}) : Error(m), status(std::move(st)) {}
+};
+struct ErrUnexpectedSize : TSSRSAError {
+  ErrUnexpectedSize() : TSSRSAError("tssrsa: unexpected input size") {}
+};
+// status 1: an index 0 or a Lagrange coefficient that is not an integer (computeLambda)
+struct ErrInvalidCalc : TSSRSAError {
+  explicit ErrInvalidCalc(std::vector<uint8_t> st = {}) : TSSRSAError("tss/rsa: invalid calculation", std::move(st)) {}
+};
+// status 2: y^e mod N != x
+struct ErrInternal : TSSRSAError {
+  explicit ErrInternal(std::vector<uint8_t> st = {}) : TSSRSAError("rsa: internal error", std::move(st)) {}
+};
+
+struct PublicKey {
+  Bytes N, E;
+  size_t Size() const { return N.empty() ? 0 : cb200_brsa_modulus_bytes(N.data(), N.size()); }
+};
+
+// KeyShare.Sign on a batch: digests (n rows of kLen, reduced mod N as Exp does) -> the shares xi (n rows of kLen)
+inline Bytes SignShareBatch(const PublicKey& pub, int players, const Bytes& E, const Bytes& digests) {
+  const size_t k = pub.Size();
+  uint8_t z = 0;
+  auto call = [&](const uint8_t* in, uint8_t* out, size_t n) {
+    blindrsa::detail::check_call(cb200_tssrsa_sign_share(blindrsa::detail::p(pub.N), pub.N.size(), players,
+                                                         E.empty() ? &z : E.data(), E.size(), in, out, n));
+  };
+  if (!k) call(&z, &z, 0);  // a modulus outside the served range: the library's argument error
+  if (!k || digests.size() % k) throw ErrUnexpectedSize();
+  const size_t n = digests.size() / k;
+  Bytes xi(n * k);
+  call(n ? digests.data() : &z, n ? xi.data() : &z, n);
+  return xi;
+}
+
+// CombineSignShares on a batch of n ops, each with its k indices (idx: n * k values), its k shares (xi: n rows of
+// k kLen bytes) and its padded message (msgs: n rows of kLen) -> n signatures; throws ErrInvalidCalc if any op has
+// status 1, else ErrInternal if any has status 2, with the status bytes (failed rows are zero)
+inline Bytes CombineSignSharesBatch(const PublicKey& pub, int players, int threshold, int k,
+                                    const std::vector<uint16_t>& idx, const Bytes& xi, const Bytes& msgs) {
+  const size_t kl = pub.Size();
+  const uint16_t zi = 0;
+  uint8_t z = 0;
+  auto call = [&](const uint16_t* ix, const uint8_t* x, const uint8_t* m, uint8_t* out, uint8_t* st, size_t n) {
+    using blindrsa::detail::p;
+    blindrsa::detail::check_call(
+        cb200_tssrsa_combine(p(pub.N), pub.N.size(), p(pub.E), pub.E.size(), players, threshold, k, ix, x, m, out, st, n));
+  };
+  if (!kl) call(&zi, &z, &z, &z, &z, 0);  // a modulus outside the served range: the library's argument error
+  if (!kl || k < 1 || msgs.size() % kl) throw ErrUnexpectedSize();
+  const size_t n = msgs.size() / kl;
+  if (idx.size() != n * (size_t)k || xi.size() != n * (size_t)k * kl) throw ErrUnexpectedSize();
+  Bytes sig(n * kl);
+  std::vector<uint8_t> st(n);
+  call(n ? idx.data() : &zi, n ? xi.data() : &z, n ? msgs.data() : &z, n ? sig.data() : &z, n ? st.data() : &z, n);
+  for (uint8_t s : st)
+    if (s == 1) throw ErrInvalidCalc(st);
+  for (uint8_t s : st)
+    if (s == 2) throw ErrInternal(st);
+  return sig;
+}
+}  // namespace tssrsa
 // Prio3 aggregators (draft-irtf-cfrg-vdaf-14): the reference's vdaf/prio3 packages count, sum, sumvec, histogram and
 // mhcv, aggregator side, on host buffers.  The constructors validate as the reference's New does and throw
 // std::invalid_argument with the library's message.  Rows are the reference's wire encodings, one per report, back to
